@@ -4,6 +4,7 @@ window frames + <= 10 Gauss-Newton/dogleg iterations of stage C + stage D margin
 HDL-64 sweeps + IMU, window 10/10 (BASELINE.json configs[2], the configuration the metric is quoted on).
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--workload hdl64|vlp16|stress128]
+                  [--dump-outputs DIR]
 
 One "step" = one scan through the whole path.  `value` times the path with the raw sweep already resident
 in HBM; `e2e` times the same call chain through the C-ABI with HOST buffers (pinned host -> device copy of the
@@ -28,7 +29,8 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
-METRIC = "scans/sec + GN-iter ms, HDL-64 window=10 at 1/2/4/8 B200 vs CPU Ceres ref"
+METRIC = "scans/sec + GN-iter ms, HDL-64 window=10 at 1/2/4/8 H100 vs CPU Ceres ref"
+DUMP_LIMIT_BYTES = 64 << 20
 
 
 def env_int(name, default):
@@ -91,7 +93,7 @@ def load_peaks():
         p = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         return float(p["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, burst copy)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s HBM3)"
 
 
 # ------------------------------------------------------------------------------------------------
@@ -138,6 +140,20 @@ def host_cores():
         return os.cpu_count() or 1
 
 
+def dump_outputs(out_dir, arrays):
+    """Writes the arrays as out_dir/<name>.npy (float32 stays float32, everything else float64).  Above DUMP_LIMIT_BYTES in
+    all, the larger arrays are cut to a fixed, seeded sample of their rows (kept in order) so that two runs stay comparable."""
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {k: np.asarray(v, np.float32 if np.asarray(v).dtype == np.float32 else np.float64) for k, v in arrays.items()}
+    total = sum(a.nbytes for a in arrays.values())
+    for name, a in arrays.items():
+        if total > DUMP_LIMIT_BYTES and a.ndim >= 1 and a.shape[0] > 1:
+            keep = max(1, int(a.shape[0] * DUMP_LIMIT_BYTES / total))
+            rows = np.sort(np.random.default_rng(0).choice(a.shape[0], keep, replace=False))
+            a = a[rows]
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+
+
 def asm_traffic(kind):
     """dram__bytes_read+write per asm_ppp launch from the committed `ncu --set full` capture of the SAME workload
     (profiles/asm_ppp_traffic.json), else None."""
@@ -162,6 +178,8 @@ def main():
                     help="multi-GPU: peer = per-scan exchange of the features over peer memory (default); rows = S blocks stored from the "
                          "stage-C kernel tail at every evaluation; nccl = allreduce callback of the S blocks")
     ap.add_argument("--cpu-sample", type=int, default=4, help="scans of the cpu_baseline sample (rank 0, N=1 only)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed scan computed as DIR/<name>.npy (rank 0)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else max(args.warmup, 1)
 
@@ -267,7 +285,7 @@ def main():
     dev_raw = {k: torch.from_numpy(scn.raw[k]).to(dev) for k in range(W, n_total - 1)}
     pin_raw = {k: torch.from_numpy(np.ascontiguousarray(scn.raw[k], np.float32)).pin_memory() for k in range(W, n_total - 1)}
     pin_np = {k: v.numpy() for k, v in pin_raw.items()}       # numpy views of the page-locked buffers
-    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=dev)   # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=dev)   # > 50 MB L2
 
     def step_dev(k):
         t = dev_raw[k]
@@ -352,6 +370,17 @@ def main():
         total_ms = float(t.item())
     prof = est.kernel_profile()
     final_states = est.states()
+    if args.dump_outputs and rank == 0:
+        # what a caller of the timed path receives for the last timed scan: stage A's clouds, the newest frame's matched
+        # features (stage B), the local map and the solved window (stages C + D)
+        p_new, c_new, _ = est.features(W)
+        sm = est.summary()
+        dump_outputs(args.dump_outputs, dict(
+            {"pp_" + name: pp.cloud(name) for name in ("laser_scans", "corner_points_sharp", "corner_points_less_sharp",
+                                                       "surface_points_flat", "surface_points_less_flat")},
+            features_points=p_new, features_coef=c_new, local_map=est.local_map(), states=final_states,
+            extrinsic=est.extrinsic(),
+            solve=np.array([sm[kk] for kk in ("iterations", "initial_cost", "final_cost", "map_size", "num_features", "has_prior")])))
 
     if profiling:
         print(json.dumps({"profiling_run": True, "ms_per_step_under_profiler": total_ms / args.steps}))
@@ -435,7 +464,7 @@ def main():
                 line["roofline_stream"] = {"kernel": "asm_ppp", "features": 1 << 26, "bytes_per_launch": sb["bytes"],
                                            "avg_launch_ms": sb["avg_ms"], "achieved": sb["gbs"], "peak": peak, "unit": "GB/s",
                                            "frac": sb["gbs"] / peak,
-                                           "note": "the same kernel on a synthetic 67 M-feature stream (2 GB >> 126 MB L2, 8 frames, centimetre residuals like a converged window); CUDA events per launch"}
+                                           "note": "the same kernel on a synthetic 67 M-feature stream (2 GB >> 50 MB L2, 8 frames, centimetre residuals like a converged window); CUDA events per launch"}
             except Exception as exc:
                 line["roofline_stream"] = {"error": repr(exc)}
             try:

@@ -1,4 +1,4 @@
-/* lio_b200.h — C-ABI of liblio_b200.so: the B200-native (sm_100a) replacement of the compute hot
+/* lio_b200.h — C-ABI of liblio_b200.so: the H100-native (sm_90a) replacement of the compute hot
  * path of hyye/lio-mapping.  Plain pointers and sizes only; no C++/torch types.
  *
  * Each entry point names the reference interface (file:line under the reference tree) it stands

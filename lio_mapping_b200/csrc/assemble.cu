@@ -1,4 +1,4 @@
-// Stage C on sm_100a — one fused kernel per Gauss-Newton iteration evaluates every
+// Stage C on sm_90a — one fused kernel per Gauss-Newton iteration evaluates every
 // PivotPointPlaneFactor (reference: src/factor/PivotPointPlaneFactor.cc:43-137, residual blocks
 // added at src/imu_processor/Estimator.cc:1831-1889 with CauchyLoss(1.0), :1664) and reduces their
 // contribution to the normal equations.

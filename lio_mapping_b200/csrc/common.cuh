@@ -1,4 +1,4 @@
-// lio_mapping_b200 — shared device/host helpers for the sm_100a kernels behind the C-ABI.
+// lio_mapping_b200 — shared device/host helpers for the sm_90a kernels behind the C-ABI.
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdint>

@@ -108,7 +108,7 @@ struct lio_pm {
   struct Cube { float4 *p = nullptr; int n = 0, cap = 0; };
   int device = 0;
   cudaStream_t stream = nullptr;
-  int sm = 148;
+  int sm = 132;
   int max_points = 0;
   std::vector<Cube> cube[2];           // [0] corner, [1] surf: kCubes descriptors each
   int cen_l = 10, cen_w = 10, cen_h = 5;

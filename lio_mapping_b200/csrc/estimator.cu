@@ -1,4 +1,4 @@
-// lio::Estimator (steady state) on sm_100a — the host shell keeps the reference's control flow
+// lio::Estimator (steady state) on sm_90a — the host shell keeps the reference's control flow
 // (window bookkeeping, gates, slide; src/imu_processor/Estimator.cc) while every per-point /
 // per-feature loop runs in the CUDA kernels of this library:
 //   ProcessLaserOdom INITED branch :618-774 -> process_scan   (de-skew kernel, device VoxelGrid)
@@ -436,7 +436,7 @@ struct lio_est {
   bool poisoned = false;   // a scan failed half-way: the window bookkeeping is inconsistent, every later call fails fast
   int W = 0, O = 0, device = 0;
   cudaStream_t stream = 0;
-  int sm_count = 148;
+  int sm_count = 132;
   // ---- host window state
   std::vector<V3> Ps, Vs, Bas, Bgs;
   std::vector<M3> Rs;
@@ -2425,7 +2425,7 @@ extern "C" int lio_asm_ppp_host(const float *pts4, const float *coef4, int n, co
     double *dRt = nullptr;
     cudaMalloc(&dRt, sizeof(Rt));
     cudaMemcpy(dRt, Rt, sizeof(Rt), cudaMemcpyHostToDevice);
-    int sms = 148;
+    int sms = 132;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
     asm_plan(ap, sms);
     rc = asm_launch(ap, dRt, w, 0, nullptr);
@@ -2584,7 +2584,7 @@ extern "C" int lio_scan_to_map_host(const float *corner_map, int Kc, const float
   ScanToMapWork W;
   float4 *d_cmap = nullptr, *d_smap = nullptr, *d_corner = nullptr, *d_surf = nullptr;
   int *d_cnt = nullptr;
-  int rc = LIO_OK, sm = 148;
+  int rc = LIO_OK, sm = 132;
   cudaDeviceGetAttribute(&sm, cudaDevAttrMultiProcessorCount, device);
   auto alloc = [&](void **p, size_t bytes) { return cudaMalloc(p, bytes ? bytes : 16) == cudaSuccess; };
   if (W.init(Kc, Ks, Mc + Ms) != 0 || !(alloc((void **)&d_cmap, sizeof(float4) * Kc) && alloc((void **)&d_smap, sizeof(float4) * Ks) &&
@@ -2637,7 +2637,7 @@ extern "C" int lio_laser_odom_host(const float *map, int K, const float *surf, i
   TransformF *d_tf = nullptr;
   OdomState *d_odom = nullptr;
   double *d_partial = nullptr;
-  int rc = LIO_OK, sm = 148;
+  int rc = LIO_OK, sm = 132;
   cudaDeviceGetAttribute(&sm, cudaDevAttrMultiProcessorCount, device);
   const int Kc = K > 0 ? K : 1;
   if (h.init(Kc) != 0 || w.init(M) != 0) rc = LIO_ERR_CUDA;
@@ -2729,7 +2729,7 @@ extern "C" int lio_asm_stream_bench(long long n_features, int iters, int device,
     }
     cudaMalloc(&dRt, sizeof(hRt));
     cudaMemcpy(dRt, hRt, sizeof(hRt), cudaMemcpyHostToDevice);
-    int sms = 148;
+    int sms = 132;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
     asm_plan(ap, sms);
     double sum = 0, mn = 1e30;

@@ -1,4 +1,4 @@
-// Stage B on sm_100a — HBM-resident voxel-hash fixed-radius k-NN + plane fit, replacing
+// Stage B on sm_90a — HBM-resident voxel-hash fixed-radius k-NN + plane fit, replacing
 // pcl::KdTreeFLANN::nearestKSearch + the per-point body of Estimator::CalculateFeatures
 // (reference: src/imu_processor/Estimator.cc:970-1097; PointAssociateToMap PointMapping.cc:303-314).
 //

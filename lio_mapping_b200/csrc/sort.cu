@@ -1,4 +1,4 @@
-// Stable LSD radix sort of (u32 key, u32 value) pairs, 8 bits per pass, hand-written for sm_100a.
+// Stable LSD radix sort of (u32 key, u32 value) pairs, 8 bits per pass, hand-written for sm_90a.
 // Used by the device VoxelGrid (key = PCL voxel index, value = input index: stability makes the
 // in-voxel order the input order, which fixes the fp32 centroid summation order).
 //

@@ -1,4 +1,4 @@
-// Stage A on sm_100a — replaces lio::PointProcessor::PointToRing / ExtractFeaturePoints
+// Stage A on sm_90a — replaces lio::PointProcessor::PointToRing / ExtractFeaturePoints
 // (reference: src/point_processor/PointProcessor.cc:185-783, include/point_processor/
 // PointProcessor.h:104-156, include/utils/math_utils.h:38-110; per-ring pcl::VoxelGrid(0.2)).
 //
@@ -839,7 +839,7 @@ extern "C" int lio_pp_process_host_ring(lio_pp *pp, const float *xyzi, const uin
   LIO_CUDA_OK(cudaMemsetAsync(pp->d_end_bits, 0, sizeof(int), st));   // end_ori_ = 0
   a_classify_ring<<<nb, kClsThreads, 0, st>>>(pp->d_in, pp->d_rings_in, n, P, pp->d_ring_id, pp->d_azi, pp->d_first_valid, pp->d_hist);
   a_scan<<<1, kMaxRings, 0, st>>>(pp->d_hist, nb, R, pp->d_offsets, pp->d_ring_start);
-  a_endori<<<std::min(nb, 148), 256, 0, st>>>(pp->d_azi, pp->d_ring_id, n, pp->d_first_valid, pp->d_end_bits);
+  a_endori<<<std::min(nb, 132), 256, 0, st>>>(pp->d_azi, pp->d_ring_id, n, pp->d_first_valid, pp->d_end_bits);
   a_scatter_ring<<<nb, kClsThreads, 0, st>>>(pp->d_in, n, P, pp->d_ring_id, pp->d_azi, pp->d_first_valid, pp->d_end_bits, pp->d_offsets,
                                              pp->d_laser, pp->d_full, pp->d_orig, pp->d_start_ori);
   a_ring<<<R, kRingThreads, pp->ring_smem, st>>>(pp->d_laser, pp->d_ring_start, P, pp->d_start_ori, pp->d_mask, pp->d_label,

@@ -1,6 +1,6 @@
-// Micro-benchmark: latency of the serial pieces of the tiled Cholesky's critical path on sm_100a (one warp, one SM):
+// Micro-benchmark: latency of the serial pieces of the tiled Cholesky's critical path on sm_90a (H100) (one warp, one SM):
 // dependent DFMA / DMUL / SHFL / rsqrt / rcp / LDS chains and the 8x8 diagonal-tile factorisation variants.
-//   nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o diag_tile diag_tile.cu && ./diag_tile
+//   nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o diag_tile diag_tile.cu && ./diag_tile
 #include <cstdio>
 #include <cuda_runtime.h>
 

@@ -1,6 +1,6 @@
-// Micro-benchmark: fp64 FMA rate (DFMA) vs fp64 tensor rate (DMMA m8n8k4) per SM on sm_100a.
+// Micro-benchmark: fp64 FMA rate (DFMA) vs fp64 tensor rate (DMMA m8n8k4) per SM on sm_90a (H100).
 // Decides whether the 7x7 weighted rank-1 update of stage C / the Cholesky trailing update should use mma.sync f64.
-//   nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o dmma_rate dmma_rate.cu && ./dmma_rate
+//   nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o dmma_rate dmma_rate.cu && ./dmma_rate
 #include <cstdio>
 #include <cuda_runtime.h>
 
@@ -55,13 +55,13 @@ int main() {
     const int threads = warps * 32, blocks = sms * 2;
     float ms = time_ms([&] { k_dfma<<<blocks, threads>>>(out, iters); });
     double fma_per_s = (double)blocks * threads * iters * 8 / (ms * 1e-3);
-    printf("DFMA  warps/CTA %2d x2 CTA/SM: %.3f ms  %.2f TFMA/s  (%.1f FMA/clk/SM @1.965GHz)\n", warps, ms, fma_per_s / 1e12, fma_per_s / sms / 1.965e9);
+    printf("DFMA  warps/CTA %2d x2 CTA/SM: %.3f ms  %.2f TFMA/s  (%.1f FMA/clk/SM @1.98GHz)\n", warps, ms, fma_per_s / 1e12, fma_per_s / sms / 1.98e9);
     float ms1 = time_ms([&] { k_dmma<1><<<blocks, threads>>>(out, iters); });
     float ms4 = time_ms([&] { k_dmma<4><<<blocks, threads>>>(out, iters); });
     float ms8 = time_ms([&] { k_dmma<8><<<blocks, threads>>>(out, iters); });
     auto rate = [&](float m, int nacc) { return (double)blocks * warps * iters * nacc * 256.0 / (m * 1e-3); };
     printf("DMMA  warps/CTA %2d x2 CTA/SM: chain1 %.3f ms %.2f TFMA/s | 4 acc %.3f ms %.2f TFMA/s | 8 acc %.3f ms %.2f TFMA/s (%.1f FMA/clk/SM)\n", warps,
-           ms1, rate(ms1, 1) / 1e12, ms4, rate(ms4, 4) / 1e12, ms8, rate(ms8, 8) / 1e12, rate(ms8, 8) / sms / 1.965e9);
+           ms1, rate(ms1, 1) / 1e12, ms4, rate(ms4, 4) / 1e12, ms8, rate(ms8, 8) / 1e12, rate(ms8, 8) / sms / 1.98e9);
   }
   // single-warp latency of a dependent DMMA / DFMA chain
   float l1 = time_ms([&] { k_dmma<1><<<1, 32>>>(out, iters); });

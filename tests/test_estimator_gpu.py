@@ -54,7 +54,7 @@ def test_asm_ppp_product_fold_and_large_residuals():
     from lio_mapping_b200 import estimator, synth, _lib
     from tests.test_shard_gloo import s_blocks
     rng = np.random.default_rng(11)
-    n = 1500000                                            # 5 stages per tile on 148 SMs: several folds per thread
+    n = 1500000                                            # 6 stages per tile on 132 SMs: several folds per thread
     p = rng.uniform(-30, 30, (n, 4)).astype(np.float32)
     w = rng.normal(size=(n, 3)); w /= np.linalg.norm(w, axis=1, keepdims=True)
     q = rng.normal(size=4); q /= np.linalg.norm(q)
