@@ -160,6 +160,45 @@ int lio_pm_map_centre(lio_pm *pm, int centre3[3]);                 /* laser_clou
 int lio_pm_cube_size(lio_pm *pm, int cube_index, int which, int *n);  /* which: 0 corner, 1 surf */
 int lio_pm_cube_download(lio_pm *pm, int cube_index, int which, float *out_xyzi, int cap);
 
+/* ---- lio::MapBuilder, the global 4-D mapper (src/map_builder/MapBuilder.cc, src/map_builder_node.cc) ---------------------
+ * MapBuilder derives from PointMapping; here a map-builder context is an lio_pm handle created by lio_mb_create, so
+ * lio_pm_map_centre / lio_pm_cube_size / lio_pm_cube_download / lio_pm_destroy apply to it unchanged.  lio_pm_process_host on a
+ * map-builder handle, and lio_mb_* on a plain lio_pm handle, return LIO_ERR_INVALID. */
+typedef struct lio_mb_config {    /* MapBuilderConfig (include/map_builder/MapBuilder.h:41-48) + node parameters */
+  float corner_filter_size;       /* 0.2 */
+  float surf_filter_size;         /* 0.4 */
+  float map_filter_size;          /* 0.2: map_builder_node.cc overrides the struct's 0.6 (down_size_filter_map_, :96) */
+  float min_match_sq_dis;         /* 1.0 */
+  float min_plane_dis;            /* 0.2 */
+  int enable_4d;                  /* 1: Transform4DAssociateToMap + OptimizeMap; 0: the PointMapping steps (:246-251, :529-543) */
+  int skip_count;                 /* 2: optimise on every skip_count-th frame (MapBuilder.cc:109-110, :529) */
+  int max_iterations;             /* 10: num_max_iterations_ (PointMapping.cc:67-104) */
+} lio_mb_config;
+void lio_mb_default_config(lio_mb_config *cfg);   /* the node's values above */
+/* MapBuilder::MapBuilder(config) + SetupRos parameters (:92-110).  max_points bounds the corner / surf clouds of one call,
+ * max_full_points the full-resolution cloud.  The surround-map buffers grow on demand. */
+int lio_mb_create(const lio_mb_config *cfg, int max_points, int max_full_points, int device, void *cuda_stream, lio_pm **out);
+/* MapBuilder::ProcessMap (:220-622) for one matched set of the clouds and the odometry that HasNewData()
+ * (PointMapping.cc:291-297) gates: corner_last / surf_last / full_cloud are /laser_cloud_corner_last, /laser_cloud_surf_last and
+ * /full_odom_cloud, transform_sum7 the /laser_odom_to_init pose rounded to float as LaserOdometryHandler (PointMapping.cc:267-282)
+ * does.  The first call sets bef = tobe = aft = sum (:227-232).  Then Transform4DAssociateToMap (:55-75), the PointMapping stacks,
+ * re-centring, cube selection, map extraction and VoxelGrid (:286-526), the gate (:529-544: OptimizeMap on every skip_count-th
+ * call, Transform4DUpdate otherwise), UpdateMapDatabase (:553-557) and PublishMapBuilderResults (:144-218).
+ * Outputs (any may be NULL): transform_tobe_mapped_, transform_aft_mapped_ (/aft_4d_mapped) and
+ * info6 = {iterations, gate chose optimisation, corner_from_map size, surf_from_map size, surround map published by this call,
+ * size of the last published surround map}.  Synchronises the stream except for the registered full cloud's kernel. */
+int lio_mb_process_map_host(lio_pm *pm, const float *corner_last, int nc, const float *surf_last, int ns, const float *full_cloud, int nf,
+                            const float transform_sum7[7], float transform_tobe_mapped7[7], float transform_aft_mapped7[7], int info6[6]);
+/* laser_cloud_surround_downsampled_ (:156-168, published on calls 1, 6, 11, ...): the corner then surf cloud of every cube of the
+ * 5 x 5 x 5 block around the sensor (no FOV test) through VoxelGrid(map_filter_size) with one bounding box; equal to its input
+ * when PCL's voxel-index overflow check fires.  The last published map stays until the next publishing call. */
+int lio_mb_surround_download(lio_pm *pm, float *out_xyzi, int cap, int *n);
+/* full_cloud_ after PointAssociateToMap with the final transform_tobe_mapped_ (/cloud_registered, :178-185), last call. */
+int lio_mb_full_download(lio_pm *pm, float *out_xyzi, int cap, int *n);
+/* Device pointers (float4) and counts of the same clouds, valid until the next lio_mb_process_map_host; stream-ordered. */
+int lio_mb_surround_dev(lio_pm *pm, const float **ptr, int *n);
+int lio_mb_full_dev(lio_pm *pm, const float **ptr, int *n);
+
 /* ---- lio::PointOdometry: scan-to-scan odometry of the pre-initialisation phase + the /compact_data pass-through ---------
  * (src/point_processor/PointOdometry.cc; include/point_processor/PointOdometry.h).  lio_po_create mirrors the constructor
  * PointOdometry(scan_period, io_ratio, num_max_iterations) (:66-86; defaults 0.1, 2, 25); the capacities bound the four feature

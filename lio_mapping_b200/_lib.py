@@ -44,6 +44,13 @@ class EstConfig(C.Structure):
 ALLREDUCE_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_int)
 
 
+class MBConfig(C.Structure):
+    """lio_mb_config (include/lio_b200.h) == MapBuilderConfig (MapBuilder.h:41-48) + the node's enable_4d / skip_count."""
+    _fields_ = [("corner_filter_size", C.c_float), ("surf_filter_size", C.c_float), ("map_filter_size", C.c_float),
+                ("min_match_sq_dis", C.c_float), ("min_plane_dis", C.c_float), ("enable_4d", C.c_int), ("skip_count", C.c_int),
+                ("max_iterations", C.c_int)]
+
+
 class PPConfig(C.Structure):
     """lio_pp_config (include/lio_b200.h) == PointProcessorConfig (PointProcessor.h:104-120)."""
     _fields_ = [("lower_bound", C.c_float), ("upper_bound", C.c_float), ("num_rings", C.c_int),
@@ -98,6 +105,14 @@ def lib():
     L.lio_pm_map_centre.argtypes = [vp, i32p]
     L.lio_pm_cube_size.argtypes = [vp, ip, ip, C.POINTER(ip)]
     L.lio_pm_cube_download.argtypes = [vp, ip, ip, f32p, ip]
+    L.lio_mb_default_config.argtypes = [C.POINTER(MBConfig)]
+    L.lio_mb_default_config.restype = None
+    L.lio_mb_create.argtypes = [C.POINTER(MBConfig), ip, ip, ip, vp, C.POINTER(vp)]
+    L.lio_mb_process_map_host.argtypes = [vp, f32p, ip, f32p, ip, f32p, ip, f32p, f32p, f32p, i32p]
+    L.lio_mb_surround_download.argtypes = [vp, f32p, ip, C.POINTER(ip)]
+    L.lio_mb_full_download.argtypes = [vp, f32p, ip, C.POINTER(ip)]
+    L.lio_mb_surround_dev.argtypes = [vp, C.POINTER(vp), C.POINTER(ip)]
+    L.lio_mb_full_dev.argtypes = [vp, C.POINTER(vp), C.POINTER(ip)]
     L.lio_po_create.argtypes = [C.c_float, ip, ip, ip, ip, ip, vp, C.POINTER(vp)]
     L.lio_po_destroy.argtypes = [vp]
     L.lio_po_set_enable_odom.argtypes = [vp, ip]

@@ -7,9 +7,14 @@
 //   Process                    :765-1052     PointAssociateToMap / TobeMapped kernels, VoxelGrid of the stacks,
 //                                            OptimizeTransformTobeMapped (scan_to_map_run: voxel-hash k-NN + 6 x 6 float GN)
 //   UpdateMapDatabase          :1112-1208    order-preserving insert into the cubes + VoxelGrid of every touched valid cube
+// lio::MapBuilder::ProcessMap (src/map_builder/MapBuilder.cc:220-622) is the same context in map-builder mode (lio_mb_*):
+//   Transform4DAssociateToMap  :55-75       yaw-only correction of the odometry rotation (host, once per frame)
+//   optimisation gate          :529-544     OptimizeMap = scan_to_map_run variant 1 on every skip_count-th frame
+//   PublishMapBuilderResults   :144-218     surround map (k_gather_segments over <= 250 cube segments + VoxelGrid) every 5th
+//                                            frame, registered full cloud (k_associate mode 0) every frame
 // Per-point work runs in kernels; the 4851-entry cube directory (pointer, count, capacity per cube) lives on the host and is
 // the only thing the control logic touches.  Compiled with -fmad=false: the float expressions follow the reference's order,
-// clouds, cube contents and the mapped pose are compared with the oracle (oracle/o_cubemap.cc).
+// clouds, cube contents and the mapped pose are compared with the oracle (oracle/o_cubemap.cc; the map-builder mode with oracle/o_mapbuilder.cc).
 #include <algorithm>
 #include <cmath>
 #include <cstring>
@@ -121,7 +126,7 @@ struct lio_pm {
   float4 *d_in[2] = {nullptr, nullptr}, *d_stack[2] = {nullptr, nullptr}, *d_ds[2] = {nullptr, nullptr}, *d_mapped = nullptr, *d_tmp = nullptr;
   float4 *d_map[2] = {nullptr, nullptr};
   int map_cap[2] = {0, 0};
-  int *d_cnt = nullptr;                // [0,1] input sizes, [2,3] down-sampled sizes, [4..] voxel-grid outputs
+  int *d_cnt = nullptr;                // [0,1] input sizes, [2,3] down-sampled sizes, [4] full cloud, [5,6] surround map in / out
   int *d_cube = nullptr;
   float4 **d_dst = nullptr;
   Segment *d_seg = nullptr;
@@ -133,6 +138,16 @@ struct lio_pm {
   int last_iters = 0, last_from_map[2] = {0, 0};
   std::vector<int> h_cube;
   std::vector<float4 *> h_dst;
+  // map-builder mode (lio_mb_*: MapBuilder : PointMapping, src/map_builder/MapBuilder.cc)
+  bool mb = false, enable_4d = true, system_init = false;
+  int skip_count = 2, odom_count = 0;
+  int map_frame_count = 4;             // num_map_frames_ - 1 (PointMapping.cc:104): the first frame publishes
+  float map_leaf = 0.2f;
+  int max_full = 0, n_full = 0, n_surround = 0, sur_cap = 0;
+  float4 *d_full_in = nullptr, *d_full_out = nullptr, *d_sur = nullptr, *d_sur_ds = nullptr;
+  Segment *d_sur_seg = nullptr, *h_sur_seg = nullptr;   // h_sur_seg / h_sur_n: pinned, so their uploads need no sync
+  int *h_sur_n = nullptr;
+  VoxelGrid vg_sur;                    // down_size_filter_map_, sized for the surround map
 };
 
 static size_t to_index(int i, int j, int k) { return (size_t)i + (size_t)kCubeL * j + (size_t)kCubeL * kCubeW * k; }
@@ -150,9 +165,13 @@ extern "C" int lio_pm_destroy(lio_pm *m) {
     void *fr[] = {m->d_in[w], m->d_stack[w], m->d_ds[w], m->d_map[w]};
     for (void *q : fr) if (q) cudaFree(q);
   }
-  void *fr[] = {m->d_mapped, m->d_tmp, m->d_cnt, m->d_cube, m->d_dst, m->d_seg, m->d_vgout};
+  void *fr[] = {m->d_mapped, m->d_tmp, m->d_cnt, m->d_cube, m->d_dst, m->d_seg, m->d_vgout, m->d_full_in, m->d_full_out, m->d_sur,
+                m->d_sur_ds, m->d_sur_seg};
   for (void *q : fr) if (q) cudaFree(q);
+  if (m->h_sur_seg) cudaFreeHost(m->h_sur_seg);
+  if (m->h_sur_n) cudaFreeHost(m->h_sur_n);
   m->vg.destroy();
+  m->vg_sur.destroy();
   m->stm.destroy();
   delete m;
   return LIO_OK;
@@ -228,8 +247,11 @@ static void pm_recentre(lio_pm *m, float px, float py, float pz, int &ci, int &c
   while (ck >= kCubeH - 3) { shift(2, -1); --ck; --m->cen_h; }
 }
 
-static void pm_select(const lio_pm *m, float px, float py, float pz, const float z[3], int ci, int cj, int ck, std::vector<size_t> &valid) {   // :944-1003
+// valid: laser_cloud_valid_idx_; surround (optional): laser_cloud_surround_idx_, every in-range cube without the FOV test
+static void pm_select(const lio_pm *m, float px, float py, float pz, const float z[3], int ci, int cj, int ck, std::vector<size_t> &valid,
+                      std::vector<size_t> *surround) {   // :944-1003
   valid.clear();
+  if (surround) surround->clear();
   for (int i = ci - 2; i <= ci + 2; ++i)
     for (int j = cj - 2; j <= cj + 2; ++j)
       for (int k = ck - 2; k <= ck + 2; ++k) {
@@ -250,6 +272,7 @@ static void pm_select(const lio_pm *m, float px, float py, float pz, const float
               if (check1 < 0 && check2 > 0) is_in_laser_fov = true;
             }
         if (is_in_laser_fov) valid.push_back(to_index(i, j, k));
+        if (surround) surround->push_back(to_index(i, j, k));
       }
 }
 
@@ -347,74 +370,271 @@ static int pm_update(lio_pm *m, const std::vector<size_t> &valid, const int n_ds
   return LIO_OK;
 }
 
-// PointMapping::Process (:765-1052), imu_inited_ == false, num_stack_frames_ == 1.  Clouds: HOST arrays of n x 4 floats.
-extern "C" int lio_pm_process_host(lio_pm *m, const float *corner_last, int nc, const float *surf_last, int ns, const float transform_sum7[7],
-                                   float transform_tobe_mapped7[7], int info3[3]) {
-  if (!m || !transform_sum7 || nc < 0 || ns < 0 || (nc > 0 && !corner_last) || (ns > 0 && !surf_last)) return LIO_ERR_INVALID;
-  if (nc > m->max_points || ns > m->max_points) return LIO_ERR_CAPACITY;
-  LIO_CUDA_OK(cudaSetDevice(m->device));
+// ---- the steps of PointMapping::Process that MapBuilder::ProcessMap shares ------------------------------------------------
+// Stacks (:782-800, :1013-1016): the last features to the map frame with the predicted pose, and back.  In map-builder mode
+// the full-resolution cloud and its count are uploaded in the same pass.
+static int pm_stack(lio_pm *m, const float *const src[2], const int nin[2], const float *full, int nf) {
   cudaStream_t st = m->stream;
-  const float *src[2] = {corner_last, surf_last};
-  const int nin[2] = {nc, ns};
-  m->sum = TwistF{transform_sum7[0], transform_sum7[1], transform_sum7[2], transform_sum7[3], transform_sum7[4], transform_sum7[5], transform_sum7[6]};
-  m->tobe = twist_mul(m->tobe, twist_mul(twist_inverse(m->bef), m->sum));   // TransformAssociateToMap :753-756
-  int hcnt[4] = {nc, ns, 0, 0};
+  int hcnt[3] = {nin[0], nin[1], nf};
   LIO_CUDA_OK(cudaMemcpyAsync(m->d_cnt, hcnt, sizeof(int) * 2, cudaMemcpyHostToDevice, st));
   for (int w = 0; w < 2; ++w) {
     if (nin[w] == 0) continue;
     LIO_CUDA_OK(cudaMemcpyAsync(m->d_in[w], src[w], sizeof(float4) * nin[w], cudaMemcpyHostToDevice, st));
-    // to the map frame with the predicted pose, and back (the reference stacks in the map frame first, :782-800, :1013-1016)
     k_associate<<<(nin[w] + 255) / 256, 256, 0, st>>>(m->d_in[w], m->d_stack[w], m->d_cnt + w, m->tobe, 0);
     k_associate<<<(nin[w] + 255) / 256, 256, 0, st>>>(m->d_stack[w], m->d_stack[w], m->d_cnt + w, m->tobe, 1);
   }
-  LIO_CUDA_OK(cudaStreamSynchronize(st));   // hcnt is a stack array
-  float z[3];
-  {  // point_on_z_axis_ = tobe * (0, 0, 10)
-    rotate_host(m->tobe, 0.0f, 0.0f, 10.0f, z[0], z[1], z[2]);
-    z[0] += m->tobe.px; z[1] += m->tobe.py; z[2] += m->tobe.pz;
+  if (m->mb) {
+    LIO_CUDA_OK(cudaMemcpyAsync(m->d_cnt + 4, hcnt + 2, sizeof(int), cudaMemcpyHostToDevice, st));
+    if (nf > 0) LIO_CUDA_OK(cudaMemcpyAsync(m->d_full_in, full, sizeof(float4) * nf, cudaMemcpyHostToDevice, st));
   }
+  LIO_CUDA_OK(cudaStreamSynchronize(st));   // hcnt is a stack array
+  return LIO_OK;
+}
+
+// point_on_z_axis_ (:801-806), re-centring (:809-931), cube selection (:944-1003) and laser_cloud_*_from_map_ (:1005-1011)
+static int pm_locate(lio_pm *m, std::vector<size_t> &valid, std::vector<size_t> *surround, int K[2]) {
+  float z[3];
+  rotate_host(m->tobe, 0.0f, 0.0f, 10.0f, z[0], z[1], z[2]);
+  z[0] += m->tobe.px; z[1] += m->tobe.py; z[2] += m->tobe.pz;
   int ci, cj, ck;
   pm_recentre(m, m->tobe.px, m->tobe.py, m->tobe.pz, ci, cj, ck);
-  std::vector<size_t> valid;
-  pm_select(m, m->tobe.px, m->tobe.py, m->tobe.pz, z, ci, cj, ck, valid);
-  int K[2] = {0, 0};
+  pm_select(m, m->tobe.px, m->tobe.py, m->tobe.pz, z, ci, cj, ck, valid, surround);
   for (int w = 0; w < 2; ++w) { int rc = pm_from_map(m, valid, w, K[w]); if (rc != LIO_OK) return rc; }
   m->last_from_map[0] = K[0]; m->last_from_map[1] = K[1];
-  // down-sample the stacks
-  int n_ds[2] = {0, 0};
+  return LIO_OK;
+}
+
+// VoxelGrid of the stacks (:1016-1022)
+static int pm_downsample(lio_pm *m, const int nin[2], int n_ds[2]) {
+  cudaStream_t st = m->stream;
   for (int w = 0; w < 2; ++w) {
     if (nin[w] == 0) { LIO_CUDA_OK(cudaMemsetAsync(m->d_cnt + 2 + w, 0, sizeof(int), st)); continue; }
     int rc = m->vg.run(m->d_stack[w], m->d_cnt + w, nin[w], m->leaf[w], m->d_ds[w], m->max_points, m->d_cnt + 2 + w, nullptr, st, nullptr);
     if (rc != LIO_OK) return rc;
   }
-  LIO_CUDA_OK(cudaMemcpyAsync(hcnt + 2, m->d_cnt + 2, sizeof(int) * 2, cudaMemcpyDeviceToHost, st));
+  LIO_CUDA_OK(cudaMemcpyAsync(n_ds, m->d_cnt + 2, sizeof(int) * 2, cudaMemcpyDeviceToHost, st));
   LIO_CUDA_OK(cudaStreamSynchronize(st));
-  n_ds[0] = hcnt[2]; n_ds[1] = hcnt[3];
-  // OptimizeTransformTobeMapped against the pulled map
+  return LIO_OK;
+}
+
+// OptimizeTransformTobeMapped (variant 0, :325-753) / MapBuilder::OptimizeMap (variant 1, MapBuilder.cc:624-1014) of tobe against
+// the pulled map; the caller has checked the early return (Kc <= 10 or Ks <= 100)
+static int pm_optimise(lio_pm *m, const int K[2], const int n_ds[2], int variant) {
+  m->last_iters = 0;
+  if (m->max_iter <= 0) return LIO_OK;
+  if (K[0] > m->stm_cap[0] || K[1] > m->stm_cap[1] || n_ds[0] + n_ds[1] > m->stm_cap[2]) {
+    m->stm.destroy();
+    m->stm_cap[0] = std::max(2 * K[0], 1 << 15); m->stm_cap[1] = std::max(2 * K[1], 1 << 16); m->stm_cap[2] = std::max(2 * (n_ds[0] + n_ds[1]), 1 << 15);
+    if (m->stm.init(m->stm_cap[0], m->stm_cap[1], m->stm_cap[2]) != 0) { lio_set_last_error(__FILE__, __LINE__, "scan-to-map workspace allocation failed"); return LIO_ERR_CUDA; }
+  }
+  float tf7[7] = {m->tobe.qx, m->tobe.qy, m->tobe.qz, m->tobe.qw, m->tobe.px, m->tobe.py, m->tobe.pz};
+  int rc = scan_to_map_run(m->stm, m->d_map[0], K[0], m->d_map[1], K[1], m->d_ds[0], m->d_cnt + 2, std::max(n_ds[0], 1), m->d_ds[1], m->d_cnt + 3,
+                           std::max(n_ds[1], 1), tf7, m->min_match_sq_dis, m->min_plane_dis, m->max_iter, m->delta_r_abort, m->delta_t_abort, variant,
+                           nullptr, &m->last_iters, m->sm, m->stream);
+  if (rc != LIO_OK) return rc;
+  m->tobe = TwistF{tf7[0], tf7[1], tf7[2], tf7[3], tf7[4], tf7[5], tf7[6]};
+  return LIO_OK;
+}
+
+static TwistF tf7_to_twist(const float t[7]) { return TwistF{t[0], t[1], t[2], t[3], t[4], t[5], t[6]}; }
+static void twist_to_tf7(const TwistF &t, float o[7]) { o[0] = t.qx; o[1] = t.qy; o[2] = t.qz; o[3] = t.qw; o[4] = t.px; o[5] = t.py; o[6] = t.pz; }
+
+// PointMapping::Process (:765-1052), imu_inited_ == false, num_stack_frames_ == 1.  Clouds: HOST arrays of n x 4 floats.
+extern "C" int lio_pm_process_host(lio_pm *m, const float *corner_last, int nc, const float *surf_last, int ns, const float transform_sum7[7],
+                                   float transform_tobe_mapped7[7], int info3[3]) {
+  if (!m || m->mb || !transform_sum7 || nc < 0 || ns < 0 || (nc > 0 && !corner_last) || (ns > 0 && !surf_last)) return LIO_ERR_INVALID;
+  if (nc > m->max_points || ns > m->max_points) return LIO_ERR_CAPACITY;
+  LIO_CUDA_OK(cudaSetDevice(m->device));
+  const float *src[2] = {corner_last, surf_last};
+  const int nin[2] = {nc, ns};
+  m->sum = tf7_to_twist(transform_sum7);
+  m->tobe = twist_mul(m->tobe, twist_mul(twist_inverse(m->bef), m->sum));   // TransformAssociateToMap :753-756
+  int rc = pm_stack(m, src, nin, nullptr, 0);
+  if (rc != LIO_OK) return rc;
+  std::vector<size_t> valid;
+  int K[2] = {0, 0}, n_ds[2] = {0, 0};
+  if ((rc = pm_locate(m, valid, nullptr, K)) != LIO_OK) return rc;
+  if ((rc = pm_downsample(m, nin, n_ds)) != LIO_OK) return rc;
   const bool optimised = !(K[0] <= 10 || K[1] <= 100);
   m->last_iters = 0;
-  if (optimised && m->max_iter > 0) {
-    if (K[0] > m->stm_cap[0] || K[1] > m->stm_cap[1] || n_ds[0] + n_ds[1] > m->stm_cap[2]) {
-      m->stm.destroy();
-      m->stm_cap[0] = std::max(2 * K[0], 1 << 15); m->stm_cap[1] = std::max(2 * K[1], 1 << 16); m->stm_cap[2] = std::max(2 * (n_ds[0] + n_ds[1]), 1 << 15);
-      if (m->stm.init(m->stm_cap[0], m->stm_cap[1], m->stm_cap[2]) != 0) { lio_set_last_error(__FILE__, __LINE__, "scan-to-map workspace allocation failed"); return LIO_ERR_CUDA; }
-    }
-    float tf7[7] = {m->tobe.qx, m->tobe.qy, m->tobe.qz, m->tobe.qw, m->tobe.px, m->tobe.py, m->tobe.pz};
-    int rc = scan_to_map_run(m->stm, m->d_map[0], K[0], m->d_map[1], K[1], m->d_ds[0], m->d_cnt + 2, std::max(n_ds[0], 1), m->d_ds[1], m->d_cnt + 3,
-                             std::max(n_ds[1], 1), tf7, m->min_match_sq_dis, m->min_plane_dis, m->max_iter, m->delta_r_abort, m->delta_t_abort, 0, nullptr,
-                             &m->last_iters, m->sm, st);
-    if (rc != LIO_OK) return rc;
-    m->tobe = TwistF{tf7[0], tf7[1], tf7[2], tf7[3], tf7[4], tf7[5], tf7[6]};
-  }
+  if (optimised && (rc = pm_optimise(m, K, n_ds, 0)) != LIO_OK) return rc;
   if (optimised) { m->bef = m->sum; m->aft = m->tobe; }   // TransformUpdate sits behind the optimiser's early return (:327-329, :716)
-  int rc = pm_update(m, valid, n_ds);
-  if (rc != LIO_OK) return rc;
-  if (transform_tobe_mapped7) {
-    transform_tobe_mapped7[0] = m->tobe.qx; transform_tobe_mapped7[1] = m->tobe.qy; transform_tobe_mapped7[2] = m->tobe.qz; transform_tobe_mapped7[3] = m->tobe.qw;
-    transform_tobe_mapped7[4] = m->tobe.px; transform_tobe_mapped7[5] = m->tobe.py; transform_tobe_mapped7[6] = m->tobe.pz;
-  }
+  if ((rc = pm_update(m, valid, n_ds)) != LIO_OK) return rc;
+  if (transform_tobe_mapped7) twist_to_tf7(m->tobe, transform_tobe_mapped7);
   if (info3) { info3[0] = m->last_iters; info3[1] = K[0]; info3[2] = K[1]; }
   return LIO_OK;
+}
+
+// ---- lio::MapBuilder (src/map_builder/MapBuilder.cc) -----------------------------------------------------------------------
+static void mat3_mul(const float A[9], const float B[9], float C[9]) {   // Eigen's 3 x 3 float product, sum in k order
+  for (int i = 0; i < 3; ++i)
+    for (int j = 0; j < 3; ++j) { float s = 0.f; for (int k = 0; k < 3; ++k) s += A[i * 3 + k] * B[k * 3 + j]; C[i * 3 + j] = s; }
+}
+
+// Transform4DAssociateToMap (:55-75, DEBUG undefined): the odometry increment as in TransformAssociateToMap gives full_transform;
+// tobe keeps its position and takes sum's rotation turned about z by the yaw difference yaw(full) - yaw(sum).
+// R2ypr(R.cast<double>()).x() = atan2(R(1,0), R(0,0)) / M_PI * 180.0 (math_utils.h:188-203); ypr2R in float (:205-230) takes
+// (float)y_diff / 180.0 * M_PI in double, rounds it to float and evaluates cos / sin in double.  The product rot_diff * sum.rot
+// is a Matrix3f assigned to the quaternion by Eigen's matrix-to-quaternion conversion, without normalisation.
+static TwistF transform_4d_associate(const TwistF &tobe, const TwistF &bef, const TwistF &sum) {
+  const TwistF full = twist_mul(tobe, twist_mul(twist_inverse(bef), sum));
+  float Rf[9], Rs[9];
+  quat_to_matrix_normalized(full, Rf);
+  quat_to_matrix_normalized(sum, Rs);
+  const double yaw_full = std::atan2((double)Rf[3], (double)Rf[0]) / M_PI * 180.0;
+  const double yaw_sum = std::atan2((double)Rs[3], (double)Rs[0]) / M_PI * 180.0;
+  const float ypr[3] = {(float)(yaw_full - yaw_sum), 0.f, 0.f};
+  float a[3], c[3], s[3];
+  for (int i = 0; i < 3; ++i) { a[i] = (float)(ypr[i] / 180.0 * M_PI); c[i] = (float)std::cos((double)a[i]); s[i] = (float)std::sin((double)a[i]); }
+  const float Rz[9] = {c[0], -s[0], 0.f, s[0], c[0], 0.f, 0.f, 0.f, 1.f};
+  const float Ry[9] = {c[1], 0.f, s[1], 0.f, 1.f, 0.f, -s[1], 0.f, c[1]};
+  const float Rx[9] = {1.f, 0.f, 0.f, 0.f, c[2], -s[2], 0.f, s[2], c[2]};
+  float Rzy[9], rot_diff[9], R[9], q[4];
+  mat3_mul(Rz, Ry, Rzy);
+  mat3_mul(Rzy, Rx, rot_diff);
+  mat3_mul(rot_diff, Rs, R);
+  matrix_to_quat(R, q);
+  return TwistF{q[0], q[1], q[2], q[3], full.px, full.py, full.pz};
+}
+
+// laser_cloud_surround_ (:156-163): each surround cube's corner cloud then its surf cloud, gathered into d_sur, followed by
+// down_size_filter_map_ over the whole cloud (:166-168).  Buffers grow on demand; the count stays on the device in d_cnt[6].
+static int mb_surround(lio_pm *m, const std::vector<size_t> &surround) {
+  cudaStream_t st = m->stream;
+  int nseg = 0, total = 0;
+  for (size_t v : surround)
+    for (int w = 0; w < 2; ++w) {
+      const lio_pm::Cube &c = m->cube[w][v];
+      if (c.n > 0) { m->h_sur_seg[nseg++] = Segment{c.p, c.n, total}; total += c.n; }
+    }
+  if (total == 0) { LIO_CUDA_OK(cudaMemsetAsync(m->d_cnt + 6, 0, sizeof(int), st)); return LIO_OK; }
+  if (total > m->sur_cap) {
+    if (m->d_sur) cudaFree(m->d_sur);
+    if (m->d_sur_ds) cudaFree(m->d_sur_ds);
+    m->d_sur = m->d_sur_ds = nullptr;
+    m->vg_sur.destroy();
+    m->sur_cap = 0;
+    const int cap = std::max(2 * total, 1 << 16);
+    LIO_CUDA_OK(cudaMalloc(&m->d_sur, sizeof(float4) * cap));
+    LIO_CUDA_OK(cudaMalloc(&m->d_sur_ds, sizeof(float4) * cap));
+    if (m->vg_sur.init(cap) != 0) { lio_set_last_error(__FILE__, __LINE__, "surround VoxelGrid allocation failed"); return LIO_ERR_CUDA; }
+    m->sur_cap = cap;
+  }
+  *m->h_sur_n = total;
+  LIO_CUDA_OK(cudaMemcpyAsync(m->d_sur_seg, m->h_sur_seg, sizeof(Segment) * nseg, cudaMemcpyHostToDevice, st));
+  LIO_CUDA_OK(cudaMemcpyAsync(m->d_cnt + 5, m->h_sur_n, sizeof(int), cudaMemcpyHostToDevice, st));
+  k_gather_segments<<<dim3(16, (unsigned)nseg), 256, 0, st>>>(m->d_sur_seg, nseg, m->d_sur);
+  return m->vg_sur.run(m->d_sur, m->d_cnt + 5, total, m->map_leaf, m->d_sur_ds, m->sur_cap, m->d_cnt + 6, nullptr, st, nullptr);
+}
+
+extern "C" void lio_mb_default_config(lio_mb_config *cfg) {
+  if (!cfg) return;
+  cfg->corner_filter_size = 0.2f; cfg->surf_filter_size = 0.4f; cfg->map_filter_size = 0.2f;
+  cfg->min_match_sq_dis = 1.0f; cfg->min_plane_dis = 0.2f;
+  cfg->enable_4d = 1; cfg->skip_count = 2; cfg->max_iterations = 10;
+}
+
+extern "C" int lio_mb_create(const lio_mb_config *cfg, int max_points, int max_full_points, int device, void *cuda_stream, lio_pm **out) {
+  if (!cfg || !out || max_full_points < 1 || !(cfg->map_filter_size > 0) || cfg->skip_count < 1) return LIO_ERR_INVALID;
+  lio_pm *m = nullptr;
+  int rc = lio_pm_create(max_points, cfg->corner_filter_size, cfg->surf_filter_size, cfg->min_match_sq_dis, cfg->min_plane_dis,
+                         cfg->max_iterations, device, cuda_stream, &m);
+  if (rc != LIO_OK) return rc;
+  m->mb = true; m->enable_4d = cfg->enable_4d != 0; m->skip_count = cfg->skip_count; m->map_leaf = cfg->map_filter_size;
+  m->max_full = max_full_points;
+  bool ok = cudaMalloc(&m->d_full_in, sizeof(float4) * max_full_points) == cudaSuccess;
+  ok = ok && cudaMalloc(&m->d_full_out, sizeof(float4) * max_full_points) == cudaSuccess;
+  ok = ok && cudaMalloc(&m->d_sur_seg, sizeof(Segment) * 2 * 125) == cudaSuccess;
+  ok = ok && cudaMallocHost(&m->h_sur_seg, sizeof(Segment) * 2 * 125) == cudaSuccess;
+  ok = ok && cudaMallocHost(&m->h_sur_n, sizeof(int)) == cudaSuccess;
+  if (!ok) { lio_set_last_error(__FILE__, __LINE__, "lio_mb_create: allocation failed"); lio_pm_destroy(m); return LIO_ERR_CUDA; }
+  *out = m;
+  return LIO_OK;
+}
+
+// MapBuilder::ProcessMap (:220-622) for one synchronised (corner, surf, full, odometry) set + PublishMapBuilderResults (:144-218)
+extern "C" int lio_mb_process_map_host(lio_pm *m, const float *corner_last, int nc, const float *surf_last, int ns, const float *full_cloud, int nf,
+                                       const float transform_sum7[7], float transform_tobe_mapped7[7], float transform_aft_mapped7[7], int info6[6]) {
+  if (!m || !m->mb || !transform_sum7 || nc < 0 || ns < 0 || nf < 0 || (nc > 0 && !corner_last) || (ns > 0 && !surf_last) ||
+      (nf > 0 && !full_cloud))
+    return LIO_ERR_INVALID;
+  if (nc > m->max_points || ns > m->max_points || nf > m->max_full) return LIO_ERR_CAPACITY;
+  LIO_CUDA_OK(cudaSetDevice(m->device));
+  cudaStream_t st = m->stream;
+  const float *src[2] = {corner_last, surf_last};
+  const int nin[2] = {nc, ns};
+  m->sum = tf7_to_twist(transform_sum7);
+  if (!m->system_init) { m->system_init = true; m->bef = m->sum; m->tobe = m->sum; m->aft = m->tobe; }   // :227-232
+  if (m->enable_4d) m->tobe = transform_4d_associate(m->tobe, m->bef, m->sum);
+  else m->tobe = twist_mul(m->tobe, twist_mul(twist_inverse(m->bef), m->sum));   // TransformAssociateToMap (PointMapping.cc:755-758)
+  int rc = pm_stack(m, src, nin, full_cloud, nf);
+  if (rc != LIO_OK) return rc;
+  std::vector<size_t> valid, surround;
+  int K[2] = {0, 0}, n_ds[2] = {0, 0};
+  if ((rc = pm_locate(m, valid, &surround, K)) != LIO_OK) return rc;
+  if ((rc = pm_downsample(m, nin, n_ds)) != LIO_OK) return rc;
+  // optimisation gate (:529-544): OptimizeMap / OptimizeTransformTobeMapped end with the update behind their early return
+  // (:625-628, :1013); the skipped frames take Transform4DUpdate / TransformUpdate (:77-90)
+  const bool gate = m->odom_count % m->skip_count == 0;
+  m->last_iters = 0;
+  if (gate) {
+    const bool optimised = !(K[0] <= 10 || K[1] <= 100);
+    if (optimised && (rc = pm_optimise(m, K, n_ds, m->enable_4d ? 1 : 0)) != LIO_OK) return rc;
+    if (optimised) { m->bef = m->sum; m->aft = m->tobe; }
+  } else {
+    m->bef = m->sum; m->aft = m->tobe;
+  }
+  ++m->odom_count;
+  if ((rc = pm_update(m, valid, n_ds)) != LIO_OK) return rc;
+  // PublishMapBuilderResults: surround map every num_map_frames_ (5) frames, registered full cloud every frame
+  const bool publish = ++m->map_frame_count >= 5;
+  if (publish) {
+    m->map_frame_count = 0;
+    if ((rc = mb_surround(m, surround)) != LIO_OK) return rc;
+  }
+  if (nf > 0) k_associate<<<(nf + 255) / 256, 256, 0, st>>>(m->d_full_in, m->d_full_out, m->d_cnt + 4, m->tobe, 0);
+  m->n_full = nf;
+  if (publish) {
+    LIO_CUDA_OK(cudaMemcpyAsync(m->h_sur_n, m->d_cnt + 6, sizeof(int), cudaMemcpyDeviceToHost, st));
+    LIO_CUDA_OK(cudaStreamSynchronize(st));
+    m->n_surround = *m->h_sur_n;
+  }
+  LIO_CUDA_OK(cudaGetLastError());
+  if (transform_tobe_mapped7) twist_to_tf7(m->tobe, transform_tobe_mapped7);
+  if (transform_aft_mapped7) twist_to_tf7(m->aft, transform_aft_mapped7);
+  if (info6) { info6[0] = m->last_iters; info6[1] = gate; info6[2] = K[0]; info6[3] = K[1]; info6[4] = publish; info6[5] = m->n_surround; }
+  return LIO_OK;
+}
+
+extern "C" int lio_mb_surround_dev(lio_pm *m, const float **ptr, int *n) {
+  if (!m || !m->mb || !ptr || !n) return LIO_ERR_INVALID;
+  *ptr = (const float *)m->d_sur_ds; *n = m->n_surround;
+  return LIO_OK;
+}
+
+extern "C" int lio_mb_full_dev(lio_pm *m, const float **ptr, int *n) {
+  if (!m || !m->mb || !ptr || !n) return LIO_ERR_INVALID;
+  *ptr = (const float *)m->d_full_out; *n = m->n_full;
+  return LIO_OK;
+}
+
+static int mb_download(lio_pm *m, const float4 *src, int count, float *out, int cap, int *n) {
+  *n = count;
+  if (count > cap) return LIO_ERR_CAPACITY;
+  LIO_CUDA_OK(cudaSetDevice(m->device));
+  if (count > 0) LIO_CUDA_OK(cudaMemcpyAsync(out, src, sizeof(float4) * count, cudaMemcpyDeviceToHost, m->stream));
+  LIO_CUDA_OK(cudaStreamSynchronize(m->stream));
+  return LIO_OK;
+}
+
+extern "C" int lio_mb_surround_download(lio_pm *m, float *out_xyzi, int cap, int *n) {
+  if (!m || !m->mb || !n || (!out_xyzi && cap > 0)) return LIO_ERR_INVALID;
+  return mb_download(m, m->d_sur_ds, m->n_surround, out_xyzi, cap, n);
+}
+
+extern "C" int lio_mb_full_download(lio_pm *m, float *out_xyzi, int cap, int *n) {
+  if (!m || !m->mb || !n || (!out_xyzi && cap > 0)) return LIO_ERR_INVALID;
+  return mb_download(m, m->d_full_out, m->n_full, out_xyzi, cap, n);
 }
 
 extern "C" int lio_pm_map_centre(lio_pm *m, int centre3[3]) {

@@ -11,7 +11,7 @@ import ctypes as C
 
 import numpy as np
 
-from . import _lib
+from . import _lib, synth
 
 SUMMARY_KEYS = ["iterations", "successful", "termination", "initial_cost", "final_cost", "cost_pim", "cost_ppp", "cost_marg",
                 "turn_off", "convergence_flag", "map_size", "num_features", "odom_iters", "t_build_map", "t_features",
@@ -287,6 +287,19 @@ class Estimator:
         out = np.zeros((self.W + 1, 16))
         _lib.check(_lib.lib().lio_est_get_states(self.h, out), "lio_est_get_states")
         return out
+
+    def local_laser_odom(self):
+        """/local_laser_odom (Estimator.cc:725-742) after process_scan, as the float tf7 (qx qy qz qw px py pz) that the map
+        builder's LaserOdometryHandler (PointMapping.cc:267-282) keeps: the lidar pose of window slot W - O, i.e. of the scan
+        received O - 1 scans before the newest, rot = R q_lb^-1 and pos = P - rot p_lb.  The clouds that go with it are that
+        scan's; the caller keeps them."""
+        s = self.states()[self.W - self.c.opt_window_size]
+        ex = self.extrinsic().astype(np.float64)
+        q = s[3:7] / np.linalg.norm(s[3:7])
+        q_lb = ex[:4] / np.linalg.norm(ex[:4])
+        rot = synth.quat_to_rot(q) @ synth.quat_to_rot(q_lb).T
+        pos = s[0:3] - rot @ ex[4:7]
+        return np.concatenate([synth.rot_to_quat(rot), pos]).astype(np.float32)
 
     def summary(self):
         s = np.zeros(32)
