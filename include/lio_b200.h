@@ -195,9 +195,22 @@ int lio_mb_process_map_host(lio_pm *pm, const float *corner_last, int nc, const 
 int lio_mb_surround_download(lio_pm *pm, float *out_xyzi, int cap, int *n);
 /* full_cloud_ after PointAssociateToMap with the final transform_tobe_mapped_ (/cloud_registered, :178-185), last call. */
 int lio_mb_full_download(lio_pm *pm, float *out_xyzi, int cap, int *n);
-/* Device pointers (float4) and counts of the same clouds, valid until the next lio_mb_process_map_host; stream-ordered. */
+/* Device pointers (float4) and counts of the same clouds, valid until the next lio_mb_process_map_*; stream-ordered. */
 int lio_mb_surround_dev(lio_pm *pm, const float **ptr, int *n);
 int lio_mb_full_dev(lio_pm *pm, const float **ptr, int *n);
+/* lio_mb_process_map_host with the three clouds already in HBM, e.g. the estimator's /local/{corner,surf,full}_points publication
+ * (lio_est_local_clouds_dev): corner_dev / surf_dev / full_dev are float4 arrays, n3_dev points to their counts {corner, surf, full}
+ * on the device.  The counts are read and clamped on the device to n3_max, which is itself capped by max_points / max_full_points;
+ * n3_max also sizes the launches, so pass tight bounds.  Same semantics, outputs and host synchronisations as the host entry (which
+ * is "upload, then these steps"); the full cloud is copied with a count-guarded kernel.  A count above its bound returns
+ * LIO_ERR_CAPACITY once the down-sampling read-back sees it; by then this call's pose association and map re-centring have
+ * already been applied, so treat the handle's pose as advanced by the dropped frame.
+ * Stream rule: the inputs are read by work enqueued on the map builder's stream.  When the producer (e.g. the estimator) runs on
+ * the same stream nothing else is needed; otherwise the caller orders the two streams (an event recorded on the producer's
+ * stream and waited on by the map builder's) and keeps the inputs unchanged until this call returns. */
+int lio_mb_process_map_dev(lio_pm *pm, const float *corner_dev, const float *surf_dev, const float *full_dev, const int *n3_dev,
+                           const int n3_max[3], const float transform_sum7[7], float transform_tobe_mapped7[7],
+                           float transform_aft_mapped7[7], int info6[6]);
 
 /* ---- lio::PointOdometry: scan-to-scan odometry of the pre-initialisation phase + the /compact_data pass-through ---------
  * (src/point_processor/PointOdometry.cc; include/point_processor/PointOdometry.h).  lio_po_create mirrors the constructor
@@ -386,6 +399,58 @@ int lio_est_begin_scan(lio_est *est);
 int lio_est_process_scan_dev(lio_est *est, const float *surf_last_dev, const int *n_dev, int n_max);
 /* Device pointer to the point count of one stage-A output cloud, to chain stage A into the estimator. */
 int lio_pp_cloud_count_dev(lio_pp *pp, int which, const int **n_dev);
+/* ---- The estimator's /local/{corner,surf,full}_points publication, the input of lio::MapBuilder (launch/map_4D.launch remaps the map builder's
+ * /laser_cloud_corner_last, /laser_cloud_surf_last, /full_odom_cloud and /laser_odom_to_init to /local/corner_points,
+ * /local/surf_points, /local/full_points and /local_laser_odom).  Opt-in; while it is off nothing of the estimator changes.
+ *
+ *   lio_est_enable_local_clouds     allocates W + 1 corner and W + 1 full slots (corner_stack_ / full_stack_, rotated with the
+ *                                   surf slots), the staging buffers and the publication buffers.  Call it once, before the
+ *                                   first lio_est_init_frame; later calls return LIO_ERR_INVALID.  Not available on a sharded
+ *                                   context: it returns LIO_ERR_INVALID after lio_est_set_shard / _set_peers / _set_feature_peers,
+ *                                   and those return LIO_ERR_INVALID once local clouds are on.
+ *   lio_est_set_scan_clouds_*       stages /laser_cloud_corner_last (stage A's LIO_PP_CORNER_LESS_SHARP) and the full cloud
+ *                                   (LIO_PP_CLOUD_IN_RINGS, what the odometry pass-through carries) for the next frame push.  Each
+ *                                   staged pair is consumed by exactly one push; staging again before the push replaces it.
+ *                                   _host: counts above max_corner_points / max_full_points return LIO_ERR_CAPACITY and change
+ *                                   nothing; the clouds are copied before the call returns (it synchronises the stream), so the
+ *                                   caller's buffers may be reused at once.
+ *                                   _dev: counts are read on the device and clamped there to nc_max / nf_max (themselves capped by
+ *                                   the capacities); a count-guarded kernel copies the clouds into the estimator's staging buffers,
+ *                                   stream-ordered on the estimator's stream: the caller's buffers may be overwritten by any work
+ *                                   enqueued on that stream after this call (or after the caller has waited for it).
+ *   pushes                          lio_est_init_frame(k) stores the staged clouds verbatim as frame k's pre-initialisation stack
+ *                                   entries (the corner cloud is expected down-sampled, like surf_ds).  lio_est_process_scan_* /
+ *                                   lio_est_open_scan_* apply the INITED rules (Estimator.cc:628-693): transform_es_ is computed
+ *                                   whenever enable_deskew || cutoff_deskew; without cutoff_deskew the corner cloud goes through
+ *                                   TransformToEnd(.., 10) like the surf cloud; then VoxelGrid(corner_filter_size).  The full cloud
+ *                                   is pushed raw (:482) and de-skewed after the publication with TransformToEnd(.., 10,
+ *                                   keep_intensity) and the scan's transform_es_ (:2416, also under cutoff_deskew).  With local
+ *                                   clouds on, a push with nothing staged returns LIO_ERR_INVALID before anything advances (the
+ *                                   context is NOT poisoned).  This work does not feed the solve: it runs on a stream forked after
+ *                                   the surf push and joined back into the estimator's stream before SlideWindow.
+ *   lio_est_local_clouds_dev        after lio_est_process_scan_* / lio_est_close_scan: the clouds SolveOptimization publishes
+ *                                   (:2362-2375) - corner_stack_, surf_stack_ and full_stack_ of frame W - O + 1 before the slide,
+ *                                   i.e. of the scan received O - 1 scans before the newest.  The surf cloud is that frame's OWN
+ *                                   down-sampled cloud (not the accumulated slot lio_est_get_frame returns).  ptr[3] = device float4
+ *                                   arrays {corner, surf, full} (the argument order of lio_mb_process_map_*), *n_dev = their device
+ *                                   counts int[3], n_host[3] = their capacities (bounds to pass on as n3_max).  Pointers are stable
+ *                                   for the life of the handle; the contents are valid until the next scan entry and are written by
+ *                                   stream-ordered work on the estimator's stream (hand them to a map builder on the same stream,
+ *                                   or order the streams).
+ *   lio_est_local_clouds_download   which: 0 corner, 1 surf, 2 full; copies one of them to the host (synchronous; *n = count,
+ *                                   LIO_ERR_CAPACITY when it exceeds cap).
+ * Without lio_est_enable_local_clouds the accessors and lio_est_set_scan_clouds_* return LIO_ERR_INVALID. */
+int lio_est_enable_local_clouds(lio_est *est, float corner_filter_size, int max_corner_points, int max_full_points);
+int lio_est_set_scan_clouds_host(lio_est *est, const float *corner, int nc, const float *full, int nf);
+int lio_est_set_scan_clouds_dev(lio_est *est, const float *corner_dev, const int *nc_dev, int nc_max, const float *full_dev,
+                                const int *nf_dev, int nf_max);
+int lio_est_local_clouds_dev(lio_est *est, const float *ptr[3], const int **n_dev, int n_host[3]);
+int lio_est_local_clouds_download(lio_est *est, int which, float *out, int cap, int *n);
+/* /local_laser_odom (Estimator.cc:725-742), after lio_est_process_scan_* / lio_est_close_scan: the lidar pose of window slot W - O,
+ * rot = Quaterniond(Rs_[W-O] * transform_lb.rot.inverse()), pos = Ps_[W-O] - rot * transform_lb.pos in double with
+ * transform_lb = transform_lb_.cast<double>(), rounded to float as the map builder's LaserOdometryHandler keeps it
+ * (PointMapping.cc:267-282): tf7 = {qx,qy,qz,qw,px,py,pz}.  Works with or without local clouds. */
+int lio_est_local_laser_odom(lio_est *est, float tf7[7]);
 /* window states: (W+1) x 16 doubles (layout of state16) */
 int lio_est_get_states(lio_est *est, double *out);
 /* summary[32]: see lio_mapping_b200/estimator.py SUMMARY_KEYS */

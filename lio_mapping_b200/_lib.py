@@ -181,6 +181,13 @@ def lib():
     L.lio_est_frame_owner.argtypes = [ip, ip]
     L.lio_est_kernel_profile.argtypes = [vp, f64p, ip]
     L.lio_est_set_shard.argtypes = [vp, ip, ip, ALLREDUCE_FN, vp]
+    L.lio_est_enable_local_clouds.argtypes = [vp, C.c_float, ip, ip]
+    L.lio_est_set_scan_clouds_host.argtypes = [vp, f32p, ip, f32p, ip]
+    L.lio_est_set_scan_clouds_dev.argtypes = [vp, vp, vp, ip, vp, vp, ip]
+    L.lio_est_local_clouds_dev.argtypes = [vp, C.POINTER(vp), C.POINTER(vp), i32p]
+    L.lio_est_local_clouds_download.argtypes = [vp, ip, f32p, ip, C.POINTER(ip)]
+    L.lio_est_local_laser_odom.argtypes = [vp, f32p]
+    L.lio_mb_process_map_dev.argtypes = [vp, vp, vp, vp, vp, i32p, f32p, f32p, f32p, i32p]
     _LIB = L
     return L
 

@@ -95,6 +95,27 @@ k_scatter_to_cubes(const float4 *__restrict__ mapped, float4 *const *__restrict_
   if (d) *d = __ldg(mapped + i);
 }
 
+// Input counts of one call {corner, surf, full}, read on the device and clamped to n_max: cnt[0], cnt[1], cnt[4]; cnt[7] = 1 when
+// a count exceeded its bound (reported as LIO_ERR_CAPACITY at the down-sampling read-back)
+__global__ void k_clamp_counts(const int *__restrict__ in, int3 n_max, int *__restrict__ cnt) {
+  if (threadIdx.x != 0) return;
+  const int mx[3] = {n_max.x, n_max.y, n_max.z};
+  int v[3], over = 0;
+  for (int w = 0; w < 3; ++w) {
+    v[w] = in[w];
+    if (v[w] > mx[w]) { over = 1; v[w] = mx[w]; }
+    if (v[w] < 0) v[w] = 0;
+  }
+  cnt[0] = v[0]; cnt[1] = v[1]; cnt[4] = v[2]; cnt[7] = over;
+}
+
+// count-guarded copy of the full cloud (its count in *n_dev)
+__global__ void __launch_bounds__(256)
+k_copy_counted(const float4 *__restrict__ in, float4 *__restrict__ out, const int *__restrict__ n_dev) {
+  const int n = *n_dev;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) out[i] = __ldg(in + i);
+}
+
 struct Segment { const float4 *src; int n; int off; };
 // concatenation of cube segments (laser_cloud_*_from_map_, :1005-1011); one block range per segment
 __global__ void __launch_bounds__(256)
@@ -126,7 +147,9 @@ struct lio_pm {
   float4 *d_in[2] = {nullptr, nullptr}, *d_stack[2] = {nullptr, nullptr}, *d_ds[2] = {nullptr, nullptr}, *d_mapped = nullptr, *d_tmp = nullptr;
   float4 *d_map[2] = {nullptr, nullptr};
   int map_cap[2] = {0, 0};
-  int *d_cnt = nullptr;                // [0,1] input sizes, [2,3] down-sampled sizes, [4] full cloud, [5,6] surround map in / out
+  int *d_cnt = nullptr;                // [0,1] input sizes, [2,3] down-sampled sizes, [4] full cloud, [5,6] surround map in / out,
+                                       // [7] input count over its bound, [8..10] counts uploaded by the host entries
+  int h_cnt[8] = {};                   // read-back of d_cnt[0..7] after the down-sampling
   int *d_cube = nullptr;
   float4 **d_dst = nullptr;
   Segment *d_seg = nullptr;
@@ -197,7 +220,7 @@ extern "C" int lio_pm_create(int max_points, float corner_filter_size, float sur
     ok = ok && cudaMalloc(&m->d_ds[w], sizeof(float4) * max_points) == cudaSuccess;
   }
   ok = ok && cudaMalloc(&m->d_mapped, sizeof(float4) * max_points) == cudaSuccess;
-  ok = ok && cudaMalloc(&m->d_cnt, sizeof(int) * 8) == cudaSuccess;
+  ok = ok && cudaMalloc(&m->d_cnt, sizeof(int) * 12) == cudaSuccess;
   ok = ok && cudaMalloc(&m->d_cube, sizeof(int) * max_points) == cudaSuccess;
   ok = ok && cudaMalloc(&m->d_dst, sizeof(float4 *) * max_points) == cudaSuccess;
   ok = ok && cudaMalloc(&m->d_seg, sizeof(Segment) * 256) == cudaSuccess;
@@ -371,23 +394,33 @@ static int pm_update(lio_pm *m, const std::vector<size_t> &valid, const int n_ds
 }
 
 // ---- the steps of PointMapping::Process that MapBuilder::ProcessMap shares ------------------------------------------------
-// Stacks (:782-800, :1013-1016): the last features to the map frame with the predicted pose, and back.  In map-builder mode
-// the full-resolution cloud and its count are uploaded in the same pass.
-static int pm_stack(lio_pm *m, const float *const src[2], const int nin[2], const float *full, int nf) {
+// Host entries: the clouds and their counts go to the context's own input buffers (d_in, d_full_in, d_cnt[8..10]); the steps
+// below then run exactly as for device inputs.
+static int pm_upload(lio_pm *m, const float *const src[2], const int nin[2], const float *full, int nf) {
   cudaStream_t st = m->stream;
-  int hcnt[3] = {nin[0], nin[1], nf};
-  LIO_CUDA_OK(cudaMemcpyAsync(m->d_cnt, hcnt, sizeof(int) * 2, cudaMemcpyHostToDevice, st));
-  for (int w = 0; w < 2; ++w) {
-    if (nin[w] == 0) continue;
-    LIO_CUDA_OK(cudaMemcpyAsync(m->d_in[w], src[w], sizeof(float4) * nin[w], cudaMemcpyHostToDevice, st));
-    k_associate<<<(nin[w] + 255) / 256, 256, 0, st>>>(m->d_in[w], m->d_stack[w], m->d_cnt + w, m->tobe, 0);
-    k_associate<<<(nin[w] + 255) / 256, 256, 0, st>>>(m->d_stack[w], m->d_stack[w], m->d_cnt + w, m->tobe, 1);
-  }
-  if (m->mb) {
-    LIO_CUDA_OK(cudaMemcpyAsync(m->d_cnt + 4, hcnt + 2, sizeof(int), cudaMemcpyHostToDevice, st));
-    if (nf > 0) LIO_CUDA_OK(cudaMemcpyAsync(m->d_full_in, full, sizeof(float4) * nf, cudaMemcpyHostToDevice, st));
-  }
+  const int hcnt[3] = {nin[0], nin[1], nf};
+  LIO_CUDA_OK(cudaMemcpyAsync(m->d_cnt + 8, hcnt, sizeof(hcnt), cudaMemcpyHostToDevice, st));
+  for (int w = 0; w < 2; ++w)
+    if (nin[w] > 0) LIO_CUDA_OK(cudaMemcpyAsync(m->d_in[w], src[w], sizeof(float4) * nin[w], cudaMemcpyHostToDevice, st));
+  if (m->mb && nf > 0) LIO_CUDA_OK(cudaMemcpyAsync(m->d_full_in, full, sizeof(float4) * nf, cudaMemcpyHostToDevice, st));
   LIO_CUDA_OK(cudaStreamSynchronize(st));   // hcnt is a stack array
+  return LIO_OK;
+}
+
+// Stacks (:782-800, :1013-1016): the last features to the map frame with the predicted pose, and back.  Sources and counts
+// {corner, surf, full} are on the device; n_max bounds them (the counts are clamped on the device).  In map-builder mode the
+// full-resolution cloud is copied into d_full_in in the same pass.
+static int pm_stack(lio_pm *m, const float4 *const src[2], const float4 *full, const int *n3_dev, const int n_max[3]) {
+  cudaStream_t st = m->stream;
+  k_clamp_counts<<<1, 32, 0, st>>>(n3_dev, make_int3(n_max[0], n_max[1], n_max[2]), m->d_cnt);
+  for (int w = 0; w < 2; ++w) {
+    if (n_max[w] == 0) continue;
+    k_associate<<<(n_max[w] + 255) / 256, 256, 0, st>>>(src[w], m->d_stack[w], m->d_cnt + w, m->tobe, 0);
+    k_associate<<<(n_max[w] + 255) / 256, 256, 0, st>>>(m->d_stack[w], m->d_stack[w], m->d_cnt + w, m->tobe, 1);
+  }
+  if (m->mb && n_max[2] > 0 && full != m->d_full_in)
+    k_copy_counted<<<std::max(1, std::min(4 * m->sm, (n_max[2] + 255) / 256)), 256, 0, st>>>(full, m->d_full_in, m->d_cnt + 4);
+  LIO_CUDA_OK(cudaGetLastError());
   return LIO_OK;
 }
 
@@ -412,8 +445,11 @@ static int pm_downsample(lio_pm *m, const int nin[2], int n_ds[2]) {
     int rc = m->vg.run(m->d_stack[w], m->d_cnt + w, nin[w], m->leaf[w], m->d_ds[w], m->max_points, m->d_cnt + 2 + w, nullptr, st, nullptr);
     if (rc != LIO_OK) return rc;
   }
-  LIO_CUDA_OK(cudaMemcpyAsync(n_ds, m->d_cnt + 2, sizeof(int) * 2, cudaMemcpyDeviceToHost, st));
+  // one read-back for the down-sampled sizes, the clamped input counts and their overflow flag
+  LIO_CUDA_OK(cudaMemcpyAsync(m->h_cnt, m->d_cnt, sizeof(m->h_cnt), cudaMemcpyDeviceToHost, st));
   LIO_CUDA_OK(cudaStreamSynchronize(st));
+  n_ds[0] = m->h_cnt[2]; n_ds[1] = m->h_cnt[3];
+  if (m->h_cnt[7]) { lio_set_last_error(__FILE__, __LINE__, "input cloud count exceeds its bound n3_max"); return LIO_ERR_CAPACITY; }
   return LIO_OK;
 }
 
@@ -449,8 +485,11 @@ extern "C" int lio_pm_process_host(lio_pm *m, const float *corner_last, int nc, 
   const int nin[2] = {nc, ns};
   m->sum = tf7_to_twist(transform_sum7);
   m->tobe = twist_mul(m->tobe, twist_mul(twist_inverse(m->bef), m->sum));   // TransformAssociateToMap :753-756
-  int rc = pm_stack(m, src, nin, nullptr, 0);
+  int rc = pm_upload(m, src, nin, nullptr, 0);
   if (rc != LIO_OK) return rc;
+  const float4 *dsrc[2] = {m->d_in[0], m->d_in[1]};
+  const int n_max[3] = {nc, ns, 0};
+  if ((rc = pm_stack(m, dsrc, nullptr, m->d_cnt + 8, n_max)) != LIO_OK) return rc;
   std::vector<size_t> valid;
   int K[2] = {0, 0}, n_ds[2] = {0, 0};
   if ((rc = pm_locate(m, valid, nullptr, K)) != LIO_OK) return rc;
@@ -552,27 +591,23 @@ extern "C" int lio_mb_create(const lio_mb_config *cfg, int max_points, int max_f
   return LIO_OK;
 }
 
-// MapBuilder::ProcessMap (:220-622) for one synchronised (corner, surf, full, odometry) set + PublishMapBuilderResults (:144-218)
-extern "C" int lio_mb_process_map_host(lio_pm *m, const float *corner_last, int nc, const float *surf_last, int ns, const float *full_cloud, int nf,
-                                       const float transform_sum7[7], float transform_tobe_mapped7[7], float transform_aft_mapped7[7], int info6[6]) {
-  if (!m || !m->mb || !transform_sum7 || nc < 0 || ns < 0 || nf < 0 || (nc > 0 && !corner_last) || (ns > 0 && !surf_last) ||
-      (nf > 0 && !full_cloud))
-    return LIO_ERR_INVALID;
-  if (nc > m->max_points || ns > m->max_points || nf > m->max_full) return LIO_ERR_CAPACITY;
-  LIO_CUDA_OK(cudaSetDevice(m->device));
+// MapBuilder::ProcessMap (:220-622) for one synchronised (corner, surf, full, odometry) set + PublishMapBuilderResults (:144-218).
+// Device sources, device counts {corner, surf, full}, host bounds n_max (already capped by the capacities).
+static int mb_process_map(lio_pm *m, const float4 *const src[2], const float4 *full, const int *n3_dev, const int n_max[3],
+                          const float transform_sum7[7], float transform_tobe_mapped7[7], float transform_aft_mapped7[7], int info6[6]) {
   cudaStream_t st = m->stream;
-  const float *src[2] = {corner_last, surf_last};
-  const int nin[2] = {nc, ns};
+  const int nin[2] = {n_max[0], n_max[1]};
   m->sum = tf7_to_twist(transform_sum7);
   if (!m->system_init) { m->system_init = true; m->bef = m->sum; m->tobe = m->sum; m->aft = m->tobe; }   // :227-232
   if (m->enable_4d) m->tobe = transform_4d_associate(m->tobe, m->bef, m->sum);
   else m->tobe = twist_mul(m->tobe, twist_mul(twist_inverse(m->bef), m->sum));   // TransformAssociateToMap (PointMapping.cc:755-758)
-  int rc = pm_stack(m, src, nin, full_cloud, nf);
+  int rc = pm_stack(m, src, full, n3_dev, n_max);
   if (rc != LIO_OK) return rc;
   std::vector<size_t> valid, surround;
   int K[2] = {0, 0}, n_ds[2] = {0, 0};
   if ((rc = pm_locate(m, valid, &surround, K)) != LIO_OK) return rc;
   if ((rc = pm_downsample(m, nin, n_ds)) != LIO_OK) return rc;
+  const int nf = n_max[2] > 0 ? m->h_cnt[4] : 0;
   // optimisation gate (:529-544): OptimizeMap / OptimizeTransformTobeMapped end with the update behind their early return
   // (:625-628, :1013); the skipped frames take Transform4DUpdate / TransformUpdate (:77-90)
   const bool gate = m->odom_count % m->skip_count == 0;
@@ -604,6 +639,35 @@ extern "C" int lio_mb_process_map_host(lio_pm *m, const float *corner_last, int 
   if (transform_aft_mapped7) twist_to_tf7(m->aft, transform_aft_mapped7);
   if (info6) { info6[0] = m->last_iters; info6[1] = gate; info6[2] = K[0]; info6[3] = K[1]; info6[4] = publish; info6[5] = m->n_surround; }
   return LIO_OK;
+}
+
+extern "C" int lio_mb_process_map_host(lio_pm *m, const float *corner_last, int nc, const float *surf_last, int ns, const float *full_cloud, int nf,
+                                       const float transform_sum7[7], float transform_tobe_mapped7[7], float transform_aft_mapped7[7], int info6[6]) {
+  if (!m || !m->mb || !transform_sum7 || nc < 0 || ns < 0 || nf < 0 || (nc > 0 && !corner_last) || (ns > 0 && !surf_last) ||
+      (nf > 0 && !full_cloud))
+    return LIO_ERR_INVALID;
+  if (nc > m->max_points || ns > m->max_points || nf > m->max_full) return LIO_ERR_CAPACITY;
+  LIO_CUDA_OK(cudaSetDevice(m->device));
+  const float *src[2] = {corner_last, surf_last};
+  const int nin[2] = {nc, ns};
+  int rc = pm_upload(m, src, nin, full_cloud, nf);
+  if (rc != LIO_OK) return rc;
+  const float4 *dsrc[2] = {m->d_in[0], m->d_in[1]};
+  const int n_max[3] = {nc, ns, nf};
+  return mb_process_map(m, dsrc, m->d_full_in, m->d_cnt + 8, n_max, transform_sum7, transform_tobe_mapped7, transform_aft_mapped7, info6);
+}
+
+extern "C" int lio_mb_process_map_dev(lio_pm *m, const float *corner_dev, const float *surf_dev, const float *full_dev, const int *n3_dev,
+                                      const int n3_max[3], const float transform_sum7[7], float transform_tobe_mapped7[7],
+                                      float transform_aft_mapped7[7], int info6[6]) {
+  if (!m || !m->mb || !transform_sum7 || !n3_dev || !n3_max || n3_max[0] < 0 || n3_max[1] < 0 || n3_max[2] < 0 ||
+      (n3_max[0] > 0 && !corner_dev) || (n3_max[1] > 0 && !surf_dev) || (n3_max[2] > 0 && !full_dev))
+    return LIO_ERR_INVALID;
+  LIO_CUDA_OK(cudaSetDevice(m->device));
+  const float4 *dsrc[2] = {reinterpret_cast<const float4 *>(corner_dev), reinterpret_cast<const float4 *>(surf_dev)};
+  const int n_max[3] = {std::min(n3_max[0], m->max_points), std::min(n3_max[1], m->max_points), std::min(n3_max[2], m->max_full)};
+  return mb_process_map(m, dsrc, reinterpret_cast<const float4 *>(full_dev), n3_dev, n_max, transform_sum7, transform_tobe_mapped7,
+                        transform_aft_mapped7, info6);
 }
 
 extern "C" int lio_mb_surround_dev(lio_pm *m, const float **ptr, int *n) {

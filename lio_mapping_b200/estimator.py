@@ -11,7 +11,7 @@ import ctypes as C
 
 import numpy as np
 
-from . import _lib, synth
+from . import _lib
 
 SUMMARY_KEYS = ["iterations", "successful", "termination", "initial_cost", "final_cost", "cost_pim", "cost_ppp", "cost_marg",
                 "turn_off", "convergence_flag", "map_size", "num_features", "odom_iters", "t_build_map", "t_features",
@@ -292,14 +292,50 @@ class Estimator:
         """/local_laser_odom (Estimator.cc:725-742) after process_scan, as the float tf7 (qx qy qz qw px py pz) that the map
         builder's LaserOdometryHandler (PointMapping.cc:267-282) keeps: the lidar pose of window slot W - O, i.e. of the scan
         received O - 1 scans before the newest, rot = R q_lb^-1 and pos = P - rot p_lb.  The clouds that go with it are that
-        scan's; the caller keeps them."""
-        s = self.states()[self.W - self.c.opt_window_size]
-        ex = self.extrinsic().astype(np.float64)
-        q = s[3:7] / np.linalg.norm(s[3:7])
-        q_lb = ex[:4] / np.linalg.norm(ex[:4])
-        rot = synth.quat_to_rot(q) @ synth.quat_to_rot(q_lb).T
-        pos = s[0:3] - rot @ ex[4:7]
-        return np.concatenate([synth.rot_to_quat(rot), pos]).astype(np.float32)
+        scan's: local_clouds() / local_clouds_dev() once enable_local_clouds() is on."""
+        t = np.zeros(7, np.float32)
+        _lib.check(_lib.lib().lio_est_local_laser_odom(self.h, t), "lio_est_local_laser_odom")
+        return t
+
+    # ---- /local/* publication (lio_est_enable_local_clouds): the map builder's input
+    LOCAL_CLOUDS = ("corner", "surf", "full")
+
+    def enable_local_clouds(self, corner_filter_size=0.2, max_corner_points=1 << 16, max_full_points=1 << 18):
+        """Keep corner_stack_ / full_stack_ and publish /local/* (call before the first init_frame)."""
+        _lib.check(_lib.lib().lio_est_enable_local_clouds(self.h, float(corner_filter_size), int(max_corner_points), int(max_full_points)),
+                   "lio_est_enable_local_clouds")
+
+    def set_scan_clouds(self, corner, full):
+        """Stage /laser_cloud_corner_last and the full cloud of the next pushed frame (host arrays, copied before return)."""
+        c = np.ascontiguousarray(corner, np.float32).reshape(-1, 4)
+        f = np.ascontiguousarray(full, np.float32).reshape(-1, 4)
+        nc, nf = c.shape[0], f.shape[0]
+        c = c if nc else np.zeros((1, 4), np.float32)
+        f = f if nf else np.zeros((1, 4), np.float32)
+        _lib.check(_lib.lib().lio_est_set_scan_clouds_host(self.h, c, nc, f, nf), "lio_est_set_scan_clouds_host")
+
+    def set_scan_clouds_dev(self, corner_ptr: int, nc_dev_ptr: int, nc_max: int, full_ptr: int, nf_dev_ptr: int, nf_max: int):
+        """The same from device float4 arrays and device counts (stream-ordered on the estimator's stream)."""
+        _lib.check(_lib.lib().lio_est_set_scan_clouds_dev(self.h, C.c_void_p(corner_ptr), C.c_void_p(nc_dev_ptr), int(nc_max),
+                                                          C.c_void_p(full_ptr), C.c_void_p(nf_dev_ptr), int(nf_max)),
+                   "lio_est_set_scan_clouds_dev")
+
+    def local_clouds_dev(self):
+        """(ptrs {corner, surf, full} as ints, device pointer of their int[3] counts, their capacities as n_max) of /local/*:
+        valid until the next scan entry, stream-ordered on the estimator's stream."""
+        ptrs = (C.c_void_p * 3)(); n_dev = C.c_void_p(); n_max = np.zeros(3, np.int32)
+        _lib.check(_lib.lib().lio_est_local_clouds_dev(self.h, ptrs, C.byref(n_dev), n_max), "lio_est_local_clouds_dev")
+        return [int(p or 0) for p in ptrs], n_dev.value, n_max
+
+    def local_clouds(self):
+        """/local/corner_points, /local/surf_points and /local/full_points of the last scan as a dict of (n, 4) float32 arrays."""
+        _, _, cap = self.local_clouds_dev()
+        out = {}
+        for w, name in enumerate(self.LOCAL_CLOUDS):
+            a = np.zeros((max(int(cap[w]), 1), 4), np.float32); n = C.c_int()
+            _lib.check(_lib.lib().lio_est_local_clouds_download(self.h, w, a, a.shape[0], C.byref(n)), "lio_est_local_clouds_download")
+            out[name] = a[:n.value].copy()
+        return out
 
     def summary(self):
         s = np.zeros(32)

@@ -56,6 +56,19 @@ class MapBuilder(PointMapping):
         return tobe, dict(iterations=int(info[0]), optimised=bool(info[1]), corner_from_map=int(info[2]), surf_from_map=int(info[3]),
                           surround_published=bool(info[4]), surround_size=int(info[5]))
 
+    def ProcessMapDev(self, ptrs, n_dev_ptr: int, n_max, transform_sum7):
+        """ProcessMap with the clouds in HBM: ptrs = device pointers {corner, surf, full} of float4 arrays, n_dev_ptr = device pointer
+        of their int[3] counts, n_max = host bounds of the counts - exactly what Estimator.local_clouds_dev() returns.  Stream rule:
+        share the producer's stream or order the two streams."""
+        tobe = np.zeros(7, np.float32); aft = np.zeros(7, np.float32); info = np.zeros(6, np.int32)
+        _lib.check(_lib.lib().lio_mb_process_map_dev(self.h, C.c_void_p(ptrs[0]), C.c_void_p(ptrs[1]), C.c_void_p(ptrs[2]),
+                                                     C.c_void_p(n_dev_ptr), np.ascontiguousarray(n_max, np.int32),
+                                                     np.ascontiguousarray(transform_sum7, np.float32), tobe, aft, info),
+                   "lio_mb_process_map_dev")
+        self.transform_aft_mapped = aft
+        return tobe, dict(iterations=int(info[0]), optimised=bool(info[1]), corner_from_map=int(info[2]), surf_from_map=int(info[3]),
+                          surround_published=bool(info[4]), surround_size=int(info[5]))
+
     def _download(self, fn, count):
         n = C.c_int()
         out = np.zeros((max(count, 1), 4), np.float32)
