@@ -512,6 +512,7 @@ struct lio_est {
   double *d_Rt = nullptr;
   double *h_S = nullptr;    // pinned kMaxOpt*kAsmStride
   int *h_counts = nullptr;  // pinned
+  int *h_xerr = nullptr;    // h_counts + W + 10: the rows exchange's bounded-wait error word (the feature exchange's is W + 9)
   OdomState *d_odom = nullptr;
   double *d_odom_partial = nullptr;
   // ---- sharding
@@ -780,11 +781,11 @@ extern "C" int lio_est_create(const lio_est_config *cfg, int device, void *cuda_
   ok = ok && cudaMalloc(&e->d_odom, sizeof(OdomState)) == cudaSuccess;
   ok = ok && cudaMalloc(&e->d_odom_partial, sizeof(double) * 32 * 1024) == cudaSuccess;
   ok = ok && cudaMallocHost((void **)&e->h_tf, sizeof(TransformF) * (W + 1)) == cudaSuccess;
-  ok = ok && cudaMallocHost((void **)&e->h_S, sizeof(double) * (kMaxOpt * kAsmStride + 2)) == cudaSuccess;  // + exchange error flag
-  if (ok) std::memset(e->h_S, 0, sizeof(double) * (kMaxOpt * kAsmStride + 2));
+  ok = ok && cudaMallocHost((void **)&e->h_S, sizeof(double) * kMaxOpt * kAsmStride) == cudaSuccess;
   ok = ok && cudaMallocHost((void **)&e->h_Rt, sizeof(double) * kMaxOpt * kAsmRtStride) == cudaSuccess;
   ok = ok && cudaMalloc(&e->d_Rt, sizeof(double) * kMaxOpt * kAsmRtStride) == cudaSuccess;
   ok = ok && cudaMallocHost((void **)&e->h_counts, sizeof(int) * (W + 16)) == cudaSuccess;
+  if (ok) { std::memset(e->h_counts, 0, sizeof(int) * (W + 16)); e->h_xerr = e->h_counts + W + 10; }
   int vg_cap = std::max(e->local_cap, cfg->max_scan_points);
   ok = ok && e->vg.init(vg_cap) == 0;
   ok = ok && e->hash.init(e->local_cap) == 0;
@@ -1104,14 +1105,35 @@ static void double_to_vector(lio_est *e) {  // Estimator.cc:2479-2568
 
 // ---- stage B orchestration -----------------------------------------------------------------------
 extern "C" int lio_est_frame_owner(int frame_rel, int world);
-// ranks the lidar reduction of a solve is sharded over: 1 when the features themselves were exchanged (every rank holds all of them)
-static int solve_world(const lio_est *e) { return e->fpeers ? 1 : e->world; }
+// How a sharded context completes the lidar reduction of a solve.  features: the features themselves were exchanged, so every rank
+// holds all of them and solves like a single GPU (this wins even when the rows exchange was also set up); rows: the peer-memory
+// exchange of the S rows (lio_est_set_peers), which wins over the allreduce callback; missing: a sharded context with neither.
+enum class Exchange { none, features, rows, callback, missing };
+static Exchange exchange_of(const lio_est *e) {
+  if (e->world == 1) return Exchange::none;
+  if (e->fpeers) return Exchange::features;
+  if (e->npeers == e->world) return Exchange::rows;
+  return e->allreduce ? Exchange::callback : Exchange::missing;
+}
 static bool owns_frame(const lio_est *e, int idx) {  // idx: logical frame > pivot
   const int pivot = e->W - e->O;
   return lio_est_frame_owner(idx - pivot, e->world) == e->rank;
 }
 
 __global__ void k_xwait(const unsigned *__restrict__ flags, int npeers, unsigned epoch, int *__restrict__ err, const int *__restrict__ skip);
+
+// Reports a bounded peer wait (k_xwait) of the feature or rows exchange that gave up, after its error word was read back.  The word
+// is one-shot: its device and host copies are cleared with the report.
+static int xwait_report(lio_est *e, Exchange x, cudaStream_t st) {
+  const bool features = x == Exchange::features;
+  int *h = features ? e->h_counts + e->W + 9 : e->h_xerr;
+  if (!*h) return LIO_OK;
+  cudaMemsetAsync(features ? e->fslab + e->foff_flags + 128 : e->xbuf + kXErrOff, 0, sizeof(int), st);
+  *h = 0;
+  lio_set_last_error(__FILE__, __LINE__, features ? "feature exchange timed out (a rank did not publish its frames)"
+                                                  : "peer exchange timed out (a rank did not publish its rows)");
+  return LIO_ERR_CUDA;
+}
 
 static int build_local_map(lio_est *e, const std::function<int()> &before_sync = nullptr) {
   const int W = e->W, O = e->O, pivot = W - O;
@@ -1309,11 +1331,7 @@ static int build_local_map(lio_est *e, const std::function<int()> &before_sync =
     rc = readback();
     if (rc != LIO_OK) return rc;
   }
-  if (e->fpeers && e->h_counts[W + 9]) {
-    cudaMemsetAsync(e->fslab + e->foff_flags + 128, 0, sizeof(int), st);
-    lio_set_last_error(__FILE__, __LINE__, "feature exchange timed out (a rank did not publish its frames)");
-    return LIO_ERR_CUDA;
-  }
+  if (e->fpeers && (rc = xwait_report(e, Exchange::features, st)) != LIO_OK) return rc;
   if (e->h_counts[W + 6] > e->cfg.max_frame_points) {   // vg_emit stopped storing at the capacity but kept counting
     lio_set_last_error(__FILE__, __LINE__, "down-sampled scan exceeds max_frame_points");
     return LIO_ERR_CAPACITY;
@@ -1364,60 +1382,97 @@ __global__ void k_xwait(const unsigned *__restrict__ flags, int npeers, unsigned
 }
 
 // ---- stage C: lidar reduction at the current parameter values ------------------------------------
-struct FrameTerms { double R[9], t[3], M[6 * 18]; };
+struct FrameTerms { double M[6 * 18]; };
 
-static int eval_lidar_wait(lio_est *e);
-// Enqueues the fused lidar reduction at the current parameters (no host synchronisation); eval_lidar_wait() completes it.
-static int eval_lidar_launch(lio_est *e, std::vector<FrameTerms> &ft) {
-  const int O = e->O, pivot = e->W - O;
-  ft.resize(O + 1);
-  AsmParams ap;
-  std::memset(&ap, 0, sizeof(ap));
-  ap.nframes = O;
-  for (int i = 1; i <= O; ++i) {
-    ppp_frame_terms(e->para_pose[0].data(), e->para_pose[i].data(), e->para_ex, ft[i].R, ft[i].t, ft[i].M);
-    AsmFrame &f = ap.f[i - 1];
-    const FeatureOut &fo = e->feats[pivot + i];
-    f.pts = fo.pts; f.coef = fo.coef;
-    f.n = (e->cfg.point_distance_factor && (e->fpeers || owns_frame(e, pivot + i))) ? e->h_feat_n[pivot + i] : 0;
-    std::memcpy(e->h_Rt + (i - 1) * kAsmRtStride, ft[i].R, sizeof(double) * 9);
-    std::memcpy(e->h_Rt + (i - 1) * kAsmRtStride + 9, ft[i].t, sizeof(double) * 3);
+// Frame terms at the current parameters: R, t of every window frame into h_Rt (the input of asm_ppp) and, when ft is given, the
+// M blocks that expand the frame's reduced rows into the normal equations.
+static void write_frame_terms(lio_est *e, std::vector<FrameTerms> *ft) {
+  if (ft) ft->resize(e->O + 1);
+  for (int i = 1; i <= e->O; ++i) {
+    double *Rt = e->h_Rt + (i - 1) * kAsmRtStride, M[6 * 18];
+    ppp_frame_terms(e->para_pose[0].data(), e->para_pose[i].data(), e->para_ex, Rt, Rt + 9, ft ? (*ft)[i].M : M);
   }
-  if (e->S_valid) return LIO_OK;
-  EST_CUDA(cudaMemcpyAsync(e->d_Rt, e->h_Rt, sizeof(double) * O * kAsmRtStride, cudaMemcpyHostToDevice, e->stream));
-  asm_plan(ap, e->sm_count);
-  long long nfeat = 0;
-  for (int k = 0; k < ap.nframes; ++k) nfeat += ap.f[k].n;
-  const bool peers = solve_world(e) > 1 && e->npeers == e->world;
-  if (solve_world(e) > 1 && !peers && !e->allreduce) {
+}
+
+// The frames and tile plan of the fused lidar reduction.  A frame counts when this rank holds its features: every frame after a
+// feature exchange, its own frames otherwise.  Fails before anything is enqueued when a sharded context has no exchange.
+static int lidar_setup(const lio_est *e, Exchange x, AsmParams &ap, long long &nfeat) {
+  if (x == Exchange::missing) {
     lio_set_last_error(__FILE__, __LINE__, "sharded context without an exchange: call lio_est_set_peers or pass an allreduce callback");
     return LIO_ERR_INVALID;
   }
-  const double *result = e->asmw.out;
-  if (peers) {  // the kernel's tail scatters the owned rows to every rank and publishes the epoch
-    ap.npeers = e->npeers; ap.self = e->rank; ap.epoch = ++e->xepoch;
-    const size_t par = (size_t)(ap.epoch & 1u) * kXRowBytes;
-    for (int i = 1; i <= O; ++i) if (owns_frame(e, pivot + i)) ap.owned_mask |= 1u << (i - 1);
-    for (int r = 0; r < e->npeers; ++r) {
-      ap.peer_out[r] = reinterpret_cast<double *>(e->peer_base[r] + par);
-      ap.peer_flag[r] = reinterpret_cast<unsigned *>(e->peer_base[r] + kXFlagOff);
-    }
-    result = reinterpret_cast<const double *>(e->xbuf + par);
+  const int O = e->O, pivot = e->W - O;
+  std::memset(&ap, 0, sizeof(ap));
+  ap.nframes = O;
+  nfeat = 0;
+  for (int i = 1; i <= O; ++i) {
+    AsmFrame &f = ap.f[i - 1];
+    const FeatureOut &fo = e->feats[pivot + i];
+    f.pts = fo.pts; f.coef = fo.coef;
+    f.n = (e->cfg.point_distance_factor && (x == Exchange::features || owns_frame(e, pivot + i))) ? e->h_feat_n[pivot + i] : 0;
+    nfeat += f.n;
   }
+  asm_plan(ap, e->sm_count);
+  return LIO_OK;
+}
+
+// Rows exchange, before each asm_ppp launch: a new epoch, and the kernel's tail scatters the owned rows into the epoch's parity of
+// every rank's buffer and publishes the epoch.  Returns where all rows of the evaluation land on this rank.
+static const double *exchange_targets(lio_est *e, Exchange x, AsmParams &ap) {
+  if (x != Exchange::rows) return e->asmw.out;
+  const int pivot = e->W - e->O;
+  ap.npeers = e->npeers; ap.self = e->rank; ap.epoch = ++e->xepoch;
+  ap.owned_mask = 0;
+  for (int i = 1; i <= e->O; ++i) if (owns_frame(e, pivot + i)) ap.owned_mask |= 1u << (i - 1);
+  const size_t par = (size_t)(ap.epoch & 1u) * kXRowBytes;
+  for (int r = 0; r < e->npeers; ++r) {
+    ap.peer_out[r] = reinterpret_cast<double *>(e->peer_base[r] + par);
+    ap.peer_flag[r] = reinterpret_cast<unsigned *>(e->peer_base[r] + kXFlagOff);
+  }
+  return reinterpret_cast<const double *>(e->xbuf + par);
+}
+
+// After each asm_ppp launch: the rows exchange waits on q for every rank's epoch (skipped on the device once `*skip` is set), the
+// callback exchange sums the partial rows of all ranks.
+static int exchange_rows(lio_est *e, Exchange x, const AsmParams &ap, cudaStream_t q, const int *skip) {
+  if (x == Exchange::rows) {
+    k_xwait<<<1, 32, 0, q>>>(reinterpret_cast<const unsigned *>(e->xbuf + kXFlagOff), e->npeers, ap.epoch,
+                             reinterpret_cast<int *>(e->xbuf + kXErrOff), skip);
+    ++e->launches;
+  } else if (x == Exchange::callback && e->allreduce(e->allreduce_user, e->asmw.out, e->O * kAsmStride) != 0) {
+    lio_set_last_error(__FILE__, __LINE__, "allreduce callback failed");
+    return LIO_ERR_CUDA;
+  }
+  return LIO_OK;
+}
+
+// One completed asm_ppp launch into lio_est_kernel_profile's totals.  A failed timing query is dropped and cleared, so that it does
+// not surface as the next launch's error.
+static void asm_time_add(lio_est *e, cudaEvent_t a, cudaEvent_t b, long long nfeat) {
+  float ms = 0.f;
+  if (cudaEventElapsedTime(&ms, a, b) == cudaSuccess) { e->asm_ms_sum += ms; e->asm_launch_count += 1; e->asm_feat_sum += nfeat; }
+  else (void)cudaGetLastError();
+}
+
+// Enqueues the fused lidar reduction at the current parameters (no host synchronisation); eval_lidar_wait() completes it.
+static int eval_lidar_launch(lio_est *e, std::vector<FrameTerms> &ft) {
+  write_frame_terms(e, &ft);
+  if (e->S_valid) return LIO_OK;
+  const Exchange x = exchange_of(e);
+  AsmParams ap;
+  long long nfeat;
+  int rc = lidar_setup(e, x, ap, nfeat);
+  if (rc != LIO_OK) return rc;
+  EST_CUDA(cudaMemcpyAsync(e->d_Rt, e->h_Rt, sizeof(double) * e->O * kAsmRtStride, cudaMemcpyHostToDevice, e->stream));
+  const double *result = exchange_targets(e, x, ap);
   if (e->ev0) cudaEventRecord(e->ev0, e->stream);
-  int rc = asm_launch(ap, e->d_Rt, e->asmw, e->stream, &e->launches);
+  rc = asm_launch(ap, e->d_Rt, e->asmw, e->stream, &e->launches);
   if (rc != LIO_OK) return rc;
   if (e->ev1) cudaEventRecord(e->ev1, e->stream);
-  if (peers) {
-    k_xwait<<<1, 32, 0, e->stream>>>(reinterpret_cast<const unsigned *>(e->xbuf + kXFlagOff), e->npeers, ap.epoch,
-                                     reinterpret_cast<int *>(e->xbuf + kXErrOff), nullptr);
-    ++e->launches;
-    EST_CUDA(cudaMemcpyAsync(e->h_S + kMaxOpt * kAsmStride, e->xbuf + kXErrOff, sizeof(int), cudaMemcpyDeviceToHost, e->stream));
-  } else if (solve_world(e) > 1 && e->allreduce) {
-    rc = e->allreduce(e->allreduce_user, e->asmw.out, O * kAsmStride);
-    if (rc != 0) { lio_set_last_error(__FILE__, __LINE__, "allreduce callback failed"); return LIO_ERR_CUDA; }
-  }
-  EST_CUDA(cudaMemcpyAsync(e->h_S, result, sizeof(double) * O * kAsmStride, cudaMemcpyDeviceToHost, e->stream));
+  rc = exchange_rows(e, x, ap, e->stream, nullptr);
+  if (rc != LIO_OK) return rc;
+  if (x == Exchange::rows) EST_CUDA(cudaMemcpyAsync(e->h_xerr, e->xbuf + kXErrOff, sizeof(int), cudaMemcpyDeviceToHost, e->stream));
+  EST_CUDA(cudaMemcpyAsync(e->h_S, result, sizeof(double) * e->O * kAsmStride, cudaMemcpyDeviceToHost, e->stream));
   e->S_pending = true;
   e->S_pending_feats = nfeat;
   return LIO_OK;
@@ -1429,16 +1484,9 @@ static int eval_lidar_wait(lio_est *e) {
   EST_CUDA(cudaStreamSynchronize(e->stream));
   e->t_lin_wait += now_s() - t0;
   e->S_pending = false;
-  if (*reinterpret_cast<const int *>(e->h_S + kMaxOpt * kAsmStride)) {
-    cudaMemsetAsync(e->xbuf + kXErrOff, 0, sizeof(int), e->stream);   // the flag is one-shot: clear it with the report
-    *reinterpret_cast<int *>(e->h_S + kMaxOpt * kAsmStride) = 0;
-    lio_set_last_error(__FILE__, __LINE__, "peer exchange timed out (a rank did not publish its rows)");
-    return LIO_ERR_CUDA;
-  }
-  if (e->ev0 && e->ev1) {
-    float ms = 0.f;
-    if (cudaEventElapsedTime(&ms, e->ev0, e->ev1) == cudaSuccess) { e->asm_ms_sum += ms; e->asm_launch_count += 1; e->asm_feat_sum += e->S_pending_feats; }
-  }
+  const int rc = xwait_report(e, Exchange::rows, e->stream);
+  if (rc != LIO_OK) return rc;
+  asm_time_add(e, e->ev0, e->ev1, e->S_pending_feats);
   e->S_valid = true;
   return LIO_OK;
 }
@@ -1520,14 +1568,16 @@ static void imu_pool_run(lio_est *e, int O, int pivot) {
   }
 }
 
-// Full linearisation at the current parameter values.  n_t = tangent dim (ex block present iff !ex_constant).
-static bool linearize(lio_est *e, Mat &H, Vec &g, double &cost, double *c_pim, double *c_ppp, double *c_marg) {
+// Full linearisation at the current parameter values.  n_t = tangent dim (ex block present iff !ex_constant).  Returns the lidar
+// evaluation's error, or LIO_ERR_NUMERIC for a non-finite cost.
+static int linearize(lio_est *e, Mat &H, Vec &g, double &cost, double *c_pim, double *c_ppp, double *c_marg) {
   const int O = e->O, pivot = e->W - O;
   const bool ex_free = !e->ex_constant;
   const int n = 15 * (O + 1) + (ex_free ? 6 : 0);
   const int oe = ex_free ? 15 * (O + 1) : -1;
   std::vector<FrameTerms> ft;
-  if (eval_lidar_launch(e, ft) != LIO_OK) return false;  // the device reduces the lidar factors while the host does the rest
+  int rc = eval_lidar_launch(e, ft);  // the device reduces the lidar factors while the host does the rest
+  if (rc != LIO_OK) return rc;
   // H starts as the prior's information matrix scattered into the tangent layout (constant over a solve: cached), or zero
   const bool use_prior = e->cfg.marginalization_factor && e->prior.valid;
   if (use_prior) {
@@ -1625,7 +1675,8 @@ static bool linearize(lio_est *e, Mat &H, Vec &g, double &cost, double *c_pim, d
     for (int k = 0; k < 6; ++k) cprior += 0.5 * r[k] * r[k];
   }
   e->t_lin_host += now_s() - th0;
-  if (eval_lidar_wait(e) != LIO_OK) return false;
+  rc = eval_lidar_wait(e);
+  if (rc != LIO_OK) return rc;
   if (e->cfg.point_distance_factor) {
     const double tl0 = now_s();
     for (int i = 1; i <= O; ++i) {
@@ -1639,7 +1690,7 @@ static bool linearize(lio_est *e, Mat &H, Vec &g, double &cost, double *c_pim, d
   if (c_pim) *c_pim = ci;
   if (c_ppp) *c_ppp = cp;
   if (c_marg) *c_marg = cm;
-  return std::isfinite(cost);
+  return std::isfinite(cost) ? LIO_OK : LIO_ERR_NUMERIC;
 }
 
 static void prior_join(lio_est *e);
@@ -1828,7 +1879,9 @@ static int solve_host(lio_est *e, int max_it) {
   Mat H;
   Vec g;
   double cost;
-  if (!linearize(e, H, g, cost, &e->cost_pim, &e->cost_ppp, &e->cost_marg)) { lio_set_last_error(__FILE__, __LINE__, "non-finite cost at the initial point"); return LIO_ERR_NUMERIC; }
+  int rc = linearize(e, H, g, cost, &e->cost_pim, &e->cost_ppp, &e->cost_marg);
+  if (rc == LIO_ERR_NUMERIC) lio_set_last_error(__FILE__, __LINE__, "non-finite cost at the initial point");
+  if (rc != LIO_OK) return rc;
   if (e->cfg.imu_factor) e->turn_off = e->cost_pim > 1e3;
   const bool ex_constant_before = e->ex_constant, prior_before = e->prior.valid;
   {
@@ -1845,12 +1898,17 @@ static int solve_host(lio_est *e, int max_it) {
   bool first = true;
   // the gate evaluation above is the solver's first linearisation when the gates left the problem structure unchanged
   bool reuse_gate = (ex_constant_before == e->ex_constant && prior_before == e->prior.valid);
+  // A non-finite cost is a rejected step.  Any other failed evaluation ends the solve with its error: the remaining iterations of
+  // dogleg_solve evaluate nothing.
+  int eval_rc = LIO_OK;
   P.linearize = [&](Mat &Hh, Vec &gg, double &c) {
-    bool ok = true;
+    if (eval_rc != LIO_OK) return false;
+    int r2 = LIO_OK;
     if (reuse_gate && first) { Hh.d.swap(H.d); Hh.r = H.r; Hh.c = H.c; gg.swap(g); c = cost; }
-    else ok = linearize(e, Hh, gg, c, nullptr, nullptr, nullptr);
-    if (ok && first) { e->H0 = Hh; e->g0 = gg; e->cost0 = c; e->have_H0 = true; first = false; }
-    return ok;
+    else r2 = linearize(e, Hh, gg, c, nullptr, nullptr, nullptr);
+    if (r2 != LIO_OK && r2 != LIO_ERR_NUMERIC) eval_rc = r2;
+    if (r2 == LIO_OK && first) { e->H0 = Hh; e->g0 = gg; e->cost0 = c; e->have_H0 = true; first = false; }
+    return r2 == LIO_OK;
   };
   P.get_state = [&](Vec &x) {
     x.clear();
@@ -1873,6 +1931,7 @@ static int solve_host(lio_est *e, int max_it) {
   DoglegOptions opt;
   opt.max_num_iterations = max_it;
   dogleg_solve(opt, P, &e->summary);
+  if (eval_rc != LIO_OK) return eval_rc;
   if (e->summary.termination == 2 && !std::isfinite(e->summary.final_cost)) { lio_set_last_error(__FILE__, __LINE__, "solver breakdown"); return LIO_ERR_NUMERIC; }
   e->t_solve = now_s() - t0;
   return LIO_OK;
@@ -1937,18 +1996,14 @@ static int solve_dev_prepare(lio_est *e, int max_it, bool assemble_only) {
     }
   }
   EST_CUDA(cudaMemcpyAsync(e->ds.st, &S, sizeof(DevSolveState), cudaMemcpyHostToDevice, st));
-  for (int i = 1; i <= O; ++i) {
-    double Mtmp[108];   // frame terms of the initial point; the solver writes the candidates' terms itself
-    ppp_frame_terms(e->para_pose[0].data(), e->para_pose[i].data(), e->para_ex, e->h_Rt + (i - 1) * kAsmRtStride,
-                    e->h_Rt + (i - 1) * kAsmRtStride + 9, Mtmp);
-  }
+  write_frame_terms(e, nullptr);   // frame terms of the initial point; the solver writes the candidates' terms itself
   EST_CUDA(cudaMemcpyAsync(e->d_Rt, e->h_Rt, sizeof(double) * O * kAsmRtStride, cudaMemcpyHostToDevice, st));
   e->ds_prepared = true; e->ds_prepared_it = max_it; e->ds_prepared_asm = assemble_only;
   return LIO_OK;
 }
 
 static int solve_dev(lio_est *e, int max_it, bool assemble_only) {
-  const int O = e->O, pivot = e->W - O;
+  const int O = e->O;
   cudaStream_t st = e->stream;
   int rc = LIO_OK;
   const double t0 = now_s();
@@ -1958,29 +2013,15 @@ static int solve_dev(lio_est *e, int max_it, bool assemble_only) {
   }
   e->ds_prepared = false;
   DevSolveState &S = *e->ds.h_st;
+  const Exchange x = exchange_of(e);
   AsmParams ap;
-  std::memset(&ap, 0, sizeof(ap));
-  ap.nframes = O;
-  long long nfeat = 0;
-  for (int i = 1; i <= O; ++i) {
-    AsmFrame &f = ap.f[i - 1];
-    const FeatureOut &fo = e->feats[pivot + i];
-    f.pts = fo.pts; f.coef = fo.coef;
-    f.n = (e->cfg.point_distance_factor && (e->fpeers || owns_frame(e, pivot + i))) ? e->h_feat_n[pivot + i] : 0;
-    nfeat += f.n;
-  }
-  asm_plan(ap, e->sm_count);
+  long long nfeat;
+  rc = lidar_setup(e, x, ap, nfeat);
+  if (rc != LIO_OK) return rc;
   ap.skip_flag = &e->ds.st->sc.done;
   ap.stamps = &e->ds.st->dbg[12][0];   // rows 12..14 of the trace: asm_ppp entry / exit stamps per evaluation
-  const bool peers = solve_world(e) > 1 && e->npeers == e->world;
-  if (solve_world(e) > 1 && !peers && !e->allreduce) {
-    lio_set_last_error(__FILE__, __LINE__, "sharded context without an exchange: call lio_est_set_peers or pass an allreduce callback");
-    return LIO_ERR_INVALID;
-  }
-  if (peers) {
-    ap.npeers = e->npeers; ap.self = e->rank;
-    for (int i = 1; i <= O; ++i) if (owns_frame(e, pivot + i)) ap.owned_mask |= 1u << (i - 1);
-  }
+  const bool sharded = x == Exchange::rows || x == Exchange::callback;
+  const bool use_graph = e->gstream && !sharded && !assemble_only && max_it == e->cfg.max_num_iterations;
   const int nevals = (assemble_only ? 0 : max_it) + 1;
   auto enqueue = [&](cudaStream_t q, bool capturing) -> int {
     // timing events inside a capture must be EXTERNAL event nodes to stay usable with cudaEventElapsedTime
@@ -1988,36 +2029,22 @@ static int solve_dev(lio_est *e, int max_it, bool assemble_only) {
     for (int ev = 0; ev < nevals; ++ev) {
       int r2 = dev_solver_factors(e->ds, ev, q, &e->launches);   // ImuFactors / prior / M_i on the second stream, beside asm_ppp
       if (r2 != LIO_OK) return r2;
-      const double *result = e->asmw.out;
-      if (peers) {
-        ap.epoch = ++e->xepoch;
-        const size_t par = (size_t)(ap.epoch & 1u) * kXRowBytes;
-        for (int r = 0; r < e->npeers; ++r) {
-          ap.peer_out[r] = reinterpret_cast<double *>(e->peer_base[r] + par);
-          ap.peer_flag[r] = reinterpret_cast<unsigned *>(e->peer_base[r] + kXFlagOff);
-        }
-        result = reinterpret_cast<const double *>(e->xbuf + par);
-      }
+      const double *result = exchange_targets(e, x, ap);
       // asm_ppp is timed on the first evaluation only: inside the captured graph every event record is a node on the critical path
       // between two k_step launches (measured: the launch behind it starts ~4 us later)
-      const bool timed = ev == 0 || (!capturing && solve_world(e) == 1);   // sharded runs: first evaluation only, like the graph
+      const bool timed = ev == 0 || (!capturing && !sharded);   // sharded runs: first evaluation only, like the graph
       if (timed) cudaEventRecordWithFlags(e->evp[2 * ev], q, evflag);
       r2 = asm_launch(ap, e->d_Rt, e->asmw, q, &e->launches);
       if (r2 != LIO_OK) return r2;
       if (timed) cudaEventRecordWithFlags(e->evp[2 * ev + 1], q, evflag);
-      if (peers) {
-        k_xwait<<<1, 32, 0, q>>>(reinterpret_cast<const unsigned *>(e->xbuf + kXFlagOff), e->npeers, ap.epoch,
-                                 reinterpret_cast<int *>(e->xbuf + kXErrOff), &e->ds.st->sc.done);
-        ++e->launches;
-      } else if (solve_world(e) > 1 && e->allreduce) {
-        if (e->allreduce(e->allreduce_user, e->asmw.out, O * kAsmStride) != 0) { lio_set_last_error(__FILE__, __LINE__, "allreduce callback failed"); return LIO_ERR_CUDA; }
-      }
+      r2 = exchange_rows(e, x, ap, q, &e->ds.st->sc.done);
+      if (r2 != LIO_OK) return r2;
       r2 = dev_solver_step(e->ds, result, e->d_Rt, ev, q, &e->launches);
       if (r2 != LIO_OK) return r2;
     }
     return LIO_OK;
   };
-  if (e->gstream && solve_world(e) == 1 && !assemble_only && max_it == e->cfg.max_num_iterations) {
+  if (use_graph) {
     // One graph per solve: the launch sequence (and the fork / join with the factor stream) is captured the first time and
     // replayed afterwards; only the asm_ppp nodes are re-parameterised with this scan's feature counts and tile plan.
     cudaStream_t gs = e->gstream;
@@ -2059,21 +2086,13 @@ static int solve_dev(lio_est *e, int max_it, bool assemble_only) {
     rc = enqueue(st, false);
     if (rc != LIO_OK) return rc;
   }
-  if (peers) EST_CUDA(cudaMemcpyAsync(e->h_S + kMaxOpt * kAsmStride, e->xbuf + kXErrOff, sizeof(int), cudaMemcpyDeviceToHost, st));
+  if (x == Exchange::rows) EST_CUDA(cudaMemcpyAsync(e->h_xerr, e->xbuf + kXErrOff, sizeof(int), cudaMemcpyDeviceToHost, st));
   EST_CUDA(cudaMemcpyAsync(&S, e->ds.st, offsetof(DevSolveState, scale), cudaMemcpyDeviceToHost, st));
   EST_CUDA(cudaStreamSynchronize(st));
-  if (peers && *reinterpret_cast<const int *>(e->h_S + kMaxOpt * kAsmStride)) {
-    cudaMemsetAsync(e->xbuf + kXErrOff, 0, sizeof(int), st);
-    *reinterpret_cast<int *>(e->h_S + kMaxOpt * kAsmStride) = 0;
-    lio_set_last_error(__FILE__, __LINE__, "peer exchange timed out (a rank did not publish its rows)");
-    return LIO_ERR_CUDA;
-  }
-  const bool graph_replayed = e->sexec && e->gstream && solve_world(e) == 1 && !assemble_only && max_it == e->cfg.max_num_iterations;
-  for (int ev = 0; ev < std::min((graph_replayed || solve_world(e) > 1) ? 1 : nevals, S.sc.evaluations); ++ev) {
-    float ms = 0.f;
-    if (cudaEventElapsedTime(&ms, e->evp[2 * ev], e->evp[2 * ev + 1]) == cudaSuccess) { e->asm_ms_sum += ms; e->asm_launch_count += 1; e->asm_feat_sum += nfeat; }
-    else (void)cudaGetLastError();   // a failed timing query must not surface as the next launch's error
-  }
+  rc = xwait_report(e, Exchange::rows, st);
+  if (rc != LIO_OK) return rc;
+  for (int ev = 0; ev < std::min((use_graph || sharded) ? 1 : nevals, S.sc.evaluations); ++ev)
+    asm_time_add(e, e->evp[2 * ev], e->evp[2 * ev + 1], nfeat);
   e->have_H0 = true; e->H0 = Mat(); e->cost0 = S.sc.initial_cost;
   if (assemble_only) return LIO_OK;
   for (int k = 0; k <= O; ++k) { std::memcpy(e->para_pose[k].data(), S.x + 16 * k, 7 * sizeof(double)); std::memcpy(e->para_sb[k].data(), S.x + 16 * k + 7, 9 * sizeof(double)); }
@@ -2307,8 +2326,9 @@ extern "C" int lio_est_assemble(lio_est *e, const double *pose, const double *sp
     Mat Hh;
     Vec gg;
     double c = 0;
-    if (!linearize(e, Hh, gg, c, nullptr, nullptr, nullptr)) { lio_set_last_error(__FILE__, __LINE__, "non-finite cost"); rc = LIO_ERR_NUMERIC; }
-    else {
+    rc = linearize(e, Hh, gg, c, nullptr, nullptr, nullptr);
+    if (rc == LIO_ERR_NUMERIC) lio_set_last_error(__FILE__, __LINE__, "non-finite cost");
+    if (rc == LIO_OK) {
       *n = Hh.r;
       if (H) std::memcpy(H, Hh.d.data(), sizeof(double) * Hh.r * Hh.r);
       if (g) std::memcpy(g, gg.data(), sizeof(double) * Hh.r);

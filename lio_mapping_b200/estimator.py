@@ -228,18 +228,8 @@ class Estimator:
         """Switch the sharded solve to the fused peer-memory exchange.  ptrs: device pointers of every rank's exchange
         buffer valid in this process (same-process contexts), or handles: (world, 64) uint8 IPC handles (one per rank)."""
         self.set_shard(rank, world, None)
-        arr = (C.c_void_p * world)()
         self._peer_open = []
-        for r in range(world):
-            if r == rank:
-                arr[r] = self.exchange_buffer()
-            elif ptrs is not None:
-                arr[r] = int(ptrs[r])
-            else:
-                p = C.c_void_p()
-                _lib.check(_lib.lib().lio_ipc_open(np.ascontiguousarray(handles[r], np.uint8), C.byref(p)), "lio_ipc_open")
-                self._peer_open.append(p.value)
-                arr[r] = p.value
+        arr = self._peer_array(rank, world, self.exchange_buffer(), ptrs, handles, self._peer_open)
         _lib.check(_lib.lib().lio_est_set_peers(self.h, world, arr), "lio_est_set_peers")
 
     def feature_slab(self):
@@ -256,19 +246,26 @@ class Estimator:
         """Sharded matching with a per-scan exchange of the features themselves (lio_est_set_feature_peers): ptrs = every rank's
         feature slab as a device pointer valid in this process, or handles = (world, 64) uint8 IPC handles."""
         self.set_shard(rank, world, None)
-        arr = (C.c_void_p * world)()
         self._fpeer_open = []
+        arr = self._peer_array(rank, world, self.feature_slab(), ptrs, handles, self._fpeer_open)
+        _lib.check(_lib.lib().lio_est_set_feature_peers(self.h, world, arr), "lio_est_set_feature_peers")
+
+    @staticmethod
+    def _peer_array(rank, world, own, ptrs, handles, opened):
+        """Every rank's buffer as a device pointer valid in this process: `own` for this rank, ptrs[r] or the IPC handle
+        handles[r] opened here (its pointer appended to `opened`) for the others."""
+        arr = (C.c_void_p * world)()
         for r in range(world):
             if r == rank:
-                arr[r] = self.feature_slab()
+                arr[r] = own
             elif ptrs is not None:
                 arr[r] = int(ptrs[r])
             else:
                 p = C.c_void_p()
                 _lib.check(_lib.lib().lio_ipc_open(np.ascontiguousarray(handles[r], np.uint8), C.byref(p)), "lio_ipc_open")
-                self._fpeer_open.append(p.value)
+                opened.append(p.value)
                 arr[r] = p.value
-        _lib.check(_lib.lib().lio_est_set_feature_peers(self.h, world, arr), "lio_est_set_feature_peers")
+        return arr
 
     def kernel_profile(self, reset=False):
         o = np.zeros(8)

@@ -163,14 +163,14 @@ def test_window_solve_parity_full_odom(oracle, vlp_seq):
         assert np.abs(xg[:, 3:7] - xo[:, 3:7]).max() <= 1e-4
 
 
-def test_two_rank_shard_equals_single(oracle, vlp_seq):
+def test_two_rank_shard_equals_single(oracle, vlp_seq, device_solver=1):
     """Frame sharding with an allreduce of the S blocks reproduces the single-rank solve (two estimator instances on
     one GPU, driven by two threads; the callback sums through the host with a barrier)."""
     import ctypes as C
     import threading
     from lio_mapping_b200 import estimator
     W = 5
-    cfg = dict(odom_max_iterations=1, prior_factor=1)
+    cfg = dict(odom_max_iterations=1, prior_factor=1, device_solver=device_solver)
     ref = estimator.Estimator(window_size=W, opt_window_size=W, max_frame_points=1 << 15, max_scan_points=1 << 17, **cfg)
     ranks = [estimator.Estimator(window_size=W, opt_window_size=W, max_frame_points=1 << 15, max_scan_points=1 << 17, **cfg)
              for _ in range(2)]
@@ -219,14 +219,19 @@ def test_two_rank_shard_equals_single(oracle, vlp_seq):
         assert np.abs(e.states() - x).max() <= 1e-9 * max(1.0, np.abs(x).max())
 
 
-def test_two_rank_peer_exchange_equals_single(oracle, vlp_seq):
+def test_two_rank_shard_equals_single_host_controller(oracle, vlp_seq):
+    """The same with the host dogleg controller."""
+    test_two_rank_shard_equals_single(oracle, vlp_seq, device_solver=0)
+
+
+def test_two_rank_peer_exchange_equals_single(oracle, vlp_seq, device_solver=1):
     """The fused peer-memory exchange (owned S rows stored into every rank's buffer by the stage-C kernel tail, epoch
     flags with system-scope release / acquire): two estimator contexts of one process exchange through raw device
     pointers on one GPU and reproduce the single-rank solve."""
     import threading
     from lio_mapping_b200 import estimator
     W = 5
-    cfg = dict(odom_max_iterations=1, prior_factor=1)
+    cfg = dict(odom_max_iterations=1, prior_factor=1, device_solver=device_solver)
     import torch
     ref = estimator.Estimator(window_size=W, opt_window_size=W, max_frame_points=1 << 15, max_scan_points=1 << 17, **cfg)
     # each rank on its own non-blocking stream: a rank's flag-wait kernel must not serialise with its peer's kernels
@@ -261,15 +266,20 @@ def test_two_rank_peer_exchange_equals_single(oracle, vlp_seq):
         assert np.abs(e.states() - x).max() <= 1e-9 * max(1.0, np.abs(x).max())
 
 
-def test_two_rank_feature_exchange_equals_single(oracle, vlp_seq):
+def test_two_rank_peer_exchange_equals_single_host_controller(oracle, vlp_seq):
+    """The same with the host dogleg controller."""
+    test_two_rank_peer_exchange_equals_single(oracle, vlp_seq, device_solver=0)
+
+
+def test_two_rank_feature_exchange_equals_single(oracle, vlp_seq, device_solver=1):
     """Sharded matching with the per-scan exchange of the features themselves (lio_est_set_feature_peers): each of two contexts
     matches half of the frames, copies its features into the peer's slab and then runs the complete single-GPU solve (graph
-    included) - the window states are those of an unsharded context, bit for bit."""
+    included with the device solver) - the window states are those of an unsharded context, bit for bit."""
     import threading
     import torch
     from lio_mapping_b200 import estimator
     W = 5
-    cfg = dict(odom_max_iterations=3, prior_factor=1)
+    cfg = dict(odom_max_iterations=3, prior_factor=1, device_solver=device_solver)
     ref = estimator.Estimator(window_size=W, opt_window_size=W, max_frame_points=1 << 15, max_scan_points=1 << 17, **cfg)
     streams = [torch.cuda.Stream() for _ in range(2)]
     ranks = [estimator.Estimator(stream=streams[r].cuda_stream, window_size=W, opt_window_size=W, max_frame_points=1 << 15,
@@ -301,6 +311,48 @@ def test_two_rank_feature_exchange_equals_single(oracle, vlp_seq):
     for e in ranks:
         assert np.array_equal(e.states(), x)
         assert e.summary()["iterations"] == ref.summary()["iterations"]
+
+
+def test_two_rank_feature_exchange_equals_single_host_controller(oracle, vlp_seq):
+    """The same with the host dogleg controller."""
+    test_two_rank_feature_exchange_equals_single(oracle, vlp_seq, device_solver=0)
+
+
+def _sharded_after_warm_start(oracle, vlp_seq, device_solver, fn):
+    """One context of a two-rank shard (rank 0) after warm start, with the allreduce callback fn (None: no exchange)."""
+    from lio_mapping_b200 import estimator
+    W = 5
+    e = estimator.Estimator(window_size=W, opt_window_size=W, max_frame_points=1 << 15, max_scan_points=1 << 17,
+                            odom_max_iterations=1, device_solver=device_solver)
+    helpers.warm_start(e, vlp_seq, oracle, W, pose_noise=0.01, seed=1,
+                       make_pim=lambda a, g: estimator.Pim(a, g, np.zeros(3), np.zeros(3), acc_n=0.2, gyr_n=0.02))
+    e.set_shard(0, 2, fn)
+    return e, W
+
+
+@pytest.mark.parametrize("device_solver", [1, 0])
+def test_sharded_context_without_exchange_is_invalid(oracle, vlp_seq, device_solver):
+    """A sharded context with neither a peer exchange nor a callback fails its scan with LIO_ERR_INVALID in both controllers."""
+    from lio_mapping_b200 import _lib
+    e, W = _sharded_after_warm_start(oracle, vlp_seq, device_solver, None)
+    with pytest.raises(_lib.LioError, match="LIO_ERR_INVALID.*without an exchange"):
+        helpers.feed_scan(e, vlp_seq, W)
+
+
+@pytest.mark.parametrize("device_solver", [1, 0])
+def test_allreduce_failure_inside_the_solve_fails_the_scan(oracle, vlp_seq, device_solver):
+    """The callback fails once, on the scan's second call (the first candidate evaluation of the dogleg loop): the scan fails
+    with that error in both controllers (not as a rejected step), and nothing is evaluated after it."""
+    from lio_mapping_b200 import _lib
+    calls = []
+
+    def cb(ptr, count):
+        calls.append(count)
+        return 1 if len(calls) == 2 else 0
+    e, W = _sharded_after_warm_start(oracle, vlp_seq, device_solver, cb)
+    with pytest.raises(_lib.LioError, match="LIO_ERR_CUDA.*allreduce callback failed"):
+        helpers.feed_scan(e, vlp_seq, W)
+    assert len(calls) == 2
 
 
 def test_device_solver_equals_host_solver(oracle, vlp_seq):
