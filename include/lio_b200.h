@@ -159,6 +159,35 @@ int lio_pm_process_host(lio_pm *pm, const float *corner_last, int nc, const floa
 int lio_pm_map_centre(lio_pm *pm, int centre3[3]);                 /* laser_cloud_cen_length_ / width_ / height_ */
 int lio_pm_cube_size(lio_pm *pm, int cube_index, int which, int *n);  /* which: 0 corner, 1 surf */
 int lio_pm_cube_download(lio_pm *pm, int cube_index, int which, float *out_xyzi, int cap);
+/* lio_pm_process_host with the clouds already in HBM, e.g. the odometry's published clouds (lio_po_clouds_dev): corner_dev / surf_dev
+ * / full_dev are float4 arrays (/laser_cloud_corner_last, /laser_cloud_surf_last, /full_odom_cloud), n3_dev points to their device
+ * counts int[3] {corner, surf, full}.  The counts are read and clamped on the device to n3_max, which is itself capped by max_points /
+ * max_full_points; n3_max also sizes the launches, so pass tight bounds.  Same steps, outputs and host synchronisations as the host
+ * entry (which is "upload, then these steps"), bit for bit.  A count above its bound returns LIO_ERR_CAPACITY once the down-sampling
+ * read-back sees it; by then this call's pose association and map re-centring have already been applied, so treat the handle's pose
+ * as advanced by the dropped frame.  On a handle that does not publish the full cloud is not read and its count has no bound:
+ * full_dev may be NULL.  Outputs (any may be NULL): transform_tobe_mapped_, transform_aft_mapped_ (/aft_mapped_to_init; it takes
+ * tobe on calls that optimised, TransformUpdate :716, and is held otherwise) and info5 = {iterations, corner_from_map size,
+ * surf_from_map size, surround map published by this call, size of the last published surround map} (the last two 0 without
+ * publishing).  An lio_mb handle returns LIO_ERR_INVALID.
+ * Stream rule: the inputs are read by work enqueued on the mapping stream.  When the producer (e.g. lio_po_process_dev) runs on the
+ * same stream nothing else is needed; otherwise the caller records an event on the producer's stream, makes the mapping stream wait
+ * for it and keeps the inputs unchanged until this call returns. */
+int lio_pm_process_dev(lio_pm *pm, const float *corner_dev, const float *surf_dev, const float *full_dev, const int *n3_dev,
+                       const int n3_max[3], const float transform_sum7[7], float transform_tobe_mapped7[7], float transform_aft_mapped7[7],
+                       int info5[5]);
+/* PointMapping::PublishResults (:1210-1270) on a plain PointMapping handle: after this, every lio_pm_process_dev also publishes
+ *   /laser_cloud_surround   on the first call and every num_map_frames_ (5)-th call after it (calls 1, 6, 11, ...; map_frame_count_
+ *                           starts at num_map_frames_ - 1, :104): every surround cube's corner then surf cloud through
+ *                           VoxelGrid(map_filter_size) (0.6, :123) - lio_mb_surround_download / lio_mb_surround_dev;
+ *   /cloud_registered       the call's full cloud through PointAssociateToMap with the final transform_tobe_mapped_ (:1245-1251) -
+ *                           lio_mb_full_download / lio_mb_full_dev;
+ *   /aft_mapped_to_init     transform_aft_mapped_ (:1254-1262), the aft output of lio_pm_process_dev.
+ * It allocates the full cloud in / registered (max_full_points float4 each) and the surround buffers of the map-builder mode, and
+ * adds one synchronisation on calls that publish the surround map (its size).  Call it once, before the first process call; a later
+ * call, a second call or an lio_mb handle returns LIO_ERR_INVALID.  A publishing handle rejects lio_pm_process_host (it has no full
+ * cloud) with LIO_ERR_INVALID.  Without it the handle behaves as before and the lio_mb_* accessors return LIO_ERR_INVALID. */
+int lio_pm_enable_publish(lio_pm *pm, float map_filter_size, int max_full_points);
 
 /* ---- lio::MapBuilder, the global 4-D mapper (src/map_builder/MapBuilder.cc, src/map_builder_node.cc) ---------------------
  * MapBuilder derives from PointMapping; here a map-builder context is an lio_pm handle created by lio_mb_create, so
@@ -195,7 +224,8 @@ int lio_mb_process_map_host(lio_pm *pm, const float *corner_last, int nc, const 
 int lio_mb_surround_download(lio_pm *pm, float *out_xyzi, int cap, int *n);
 /* full_cloud_ after PointAssociateToMap with the final transform_tobe_mapped_ (/cloud_registered, :178-185), last call. */
 int lio_mb_full_download(lio_pm *pm, float *out_xyzi, int cap, int *n);
-/* Device pointers (float4) and counts of the same clouds, valid until the next lio_mb_process_map_*; stream-ordered. */
+/* Device pointers (float4) and counts of the same clouds, valid until the next lio_mb_process_map_*; stream-ordered.  The four
+ * accessors also serve a publishing PointMapping handle (lio_pm_enable_publish), valid until its next lio_pm_process_dev. */
 int lio_mb_surround_dev(lio_pm *pm, const float **ptr, int *n);
 int lio_mb_full_dev(lio_pm *pm, const float **ptr, int *n);
 /* lio_mb_process_map_host with the three clouds already in HBM, e.g. the estimator's /local/{corner,surf,full}_points publication
@@ -241,6 +271,27 @@ int lio_po_cloud_download(lio_po *po, int which, float *out_xyzi, int cap);
 int lio_po_compact_data(lio_po *po, float *out_xyzi, int cap_points, int *n_points);
 int lio_po_last_launches(lio_po *po);
 int lio_po_matches(lio_po *po, int kind, int32_t *out, int cap_queries);   /* test aid: indices of the last search, 2 (corner) / 3 (surf) per query */
+/* lio_po_process_host with the five clouds already in HBM, e.g. stage A's outputs (lio_pp_cloud_dev / lio_pp_cloud_count_dev):
+ * clouds_dev = float4 arrays {sharp, less_sharp, flat, less_flat, full} (LIO_PP_CORNER_SHARP, LIO_PP_CORNER_LESS_SHARP,
+ * LIO_PP_SURF_FLAT, LIO_PP_SURF_LESS_FLAT, LIO_PP_CLOUD_IN_RINGS), n_dev = one device int per cloud with its count, n_max = host
+ * bounds of the counts.  A bound above the capacities given to lio_po_create returns LIO_ERR_CAPACITY; so does a device count above
+ * its bound, before anything of the handle changes (no swap, no frame_count_ increment: the call can be repeated with a correct
+ * bound).  less_sharp, less_flat and full are copied into the handle by a count-guarded kernel (they are de-skewed in place and kept
+ * as the last clouds), sharp and flat are read where they are during the call.  Then one read-back of the clamped counts and the
+ * overflow flag, and the host entry's steps; the outputs are bit-identical to lio_po_process_host on the same clouds.  The call
+ * synchronises the stream at most twice (the count read-back; the pose after the iterations when odometry runs) and not at its
+ * end: what it enqueues last (the de-skew kernels) is ordered before later work on the same stream.
+ * Stream rule: the inputs are read by work enqueued on the odometry's stream; share the producer's stream, or record an event on
+ * the producer's stream and make the odometry's stream wait for it, and keep sharp / flat unchanged until that stream has passed
+ * this call's work. */
+int lio_po_process_dev(lio_po *po, const float *const clouds_dev[5], const int *const n_dev[5], const int n_max[5], float transform_sum7[7],
+                       float transform_es7[7], int info4[4]);
+/* The published clouds in HBM: ptr = {last_corner_cloud_, last_surf_cloud_, full_cloud_} (/laser_cloud_corner_last,
+ * /laser_cloud_surf_last and the full cloud of /compact_data, the argument order of lio_pm_process_dev), *n_dev = a device int[3]
+ * with their counts (stable for the life of the handle, written stream-ordered by every process call), n_host = the same counts as
+ * the host knows them after the last call (exact, so tight bounds for n3_max).  The two last clouds swap buffers with the incoming
+ * less_sharp / less_flat clouds, so the pointers are valid until the next process call only: fetch them after every call. */
+int lio_po_clouds_dev(lio_po *po, const float *ptr[3], const int **n_dev, int n_host[3]);
 
 /* PointMapping::OptimizeTransformTobeMapped (PointMapping.cc:325-753): scan-to-map 6-DoF float Gauss-Newton of
  * transform_tobe_mapped_ (tf7, in/out) against explicit corner / surf maps (laser_cloud_corner_from_map_ /

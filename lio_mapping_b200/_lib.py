@@ -188,6 +188,10 @@ def lib():
     L.lio_est_local_clouds_download.argtypes = [vp, ip, f32p, ip, C.POINTER(ip)]
     L.lio_est_local_laser_odom.argtypes = [vp, f32p]
     L.lio_mb_process_map_dev.argtypes = [vp, vp, vp, vp, vp, i32p, f32p, f32p, f32p, i32p]
+    L.lio_po_process_dev.argtypes = [vp, C.POINTER(vp), C.POINTER(vp), i32p, f32p, f32p, i32p]
+    L.lio_po_clouds_dev.argtypes = [vp, C.POINTER(vp), C.POINTER(vp), i32p]
+    L.lio_pm_process_dev.argtypes = [vp, vp, vp, vp, vp, i32p, f32p, f32p, f32p, i32p]
+    L.lio_pm_enable_publish.argtypes = [vp, C.c_float, ip]
     _LIB = L
     return L
 

@@ -7,6 +7,10 @@
 //   Process                    :765-1052     PointAssociateToMap / TobeMapped kernels, VoxelGrid of the stacks,
 //                                            OptimizeTransformTobeMapped (scan_to_map_run: voxel-hash k-NN + 6 x 6 float GN)
 //   UpdateMapDatabase          :1112-1208    order-preserving insert into the cubes + VoxelGrid of every touched valid cube
+//   PublishResults             :1210-1270    after lio_pm_enable_publish: the map-builder mode's surround map (every 5th call) and
+//                                            registered full cloud, shared with PublishMapBuilderResults (pm_publish)
+// Host entries upload into the context's own buffers and run the same steps as the device entries (lio_pm_process_dev,
+// lio_mb_process_map_dev), whose clouds and counts stay in HBM.
 // lio::MapBuilder::ProcessMap (src/map_builder/MapBuilder.cc:220-622) is the same context in map-builder mode (lio_mb_*):
 //   Transform4DAssociateToMap  :55-75       yaw-only correction of the odometry rotation (host, once per frame)
 //   optimisation gate          :529-544     OptimizeMap = scan_to_map_run variant 1 on every skip_count-th frame
@@ -16,6 +20,7 @@
 // the only thing the control logic touches.  Compiled with -fmad=false: the float expressions follow the reference's order,
 // clouds, cube contents and the mapped pose are compared with the oracle (oracle/o_cubemap.cc; the map-builder mode with oracle/o_mapbuilder.cc).
 #include <algorithm>
+#include <climits>
 #include <cmath>
 #include <cstring>
 #include <new>
@@ -161,11 +166,13 @@ struct lio_pm {
   int last_iters = 0, last_from_map[2] = {0, 0};
   std::vector<int> h_cube;
   std::vector<float4 *> h_dst;
+  bool started = false;                // a process call has run (lio_pm_enable_publish must come before it)
+  bool publish = false;                // lio_pm_enable_publish: PointMapping::PublishResults on every lio_pm_process_dev
   // map-builder mode (lio_mb_*: MapBuilder : PointMapping, src/map_builder/MapBuilder.cc)
   bool mb = false, enable_4d = true, system_init = false;
   int skip_count = 2, odom_count = 0;
   int map_frame_count = 4;             // num_map_frames_ - 1 (PointMapping.cc:104): the first frame publishes
-  float map_leaf = 0.2f;
+  float map_leaf = 0.2f;               // down_size_filter_map_ (PointMapping.cc:123 0.6, map_builder_node 0.2)
   int max_full = 0, n_full = 0, n_surround = 0, sur_cap = 0;
   float4 *d_full_in = nullptr, *d_full_out = nullptr, *d_sur = nullptr, *d_sur_ds = nullptr;
   Segment *d_sur_seg = nullptr, *h_sur_seg = nullptr;   // h_sur_seg / h_sur_n: pinned, so their uploads need no sync
@@ -408,8 +415,8 @@ static int pm_upload(lio_pm *m, const float *const src[2], const int nin[2], con
 }
 
 // Stacks (:782-800, :1013-1016): the last features to the map frame with the predicted pose, and back.  Sources and counts
-// {corner, surf, full} are on the device; n_max bounds them (the counts are clamped on the device).  In map-builder mode the
-// full-resolution cloud is copied into d_full_in in the same pass.
+// {corner, surf, full} are on the device; n_max bounds them (the counts are clamped on the device).  In map-builder mode and on a
+// publishing PointMapping the full-resolution cloud is copied into d_full_in in the same pass.
 static int pm_stack(lio_pm *m, const float4 *const src[2], const float4 *full, const int *n3_dev, const int n_max[3]) {
   cudaStream_t st = m->stream;
   k_clamp_counts<<<1, 32, 0, st>>>(n3_dev, make_int3(n_max[0], n_max[1], n_max[2]), m->d_cnt);
@@ -418,7 +425,7 @@ static int pm_stack(lio_pm *m, const float4 *const src[2], const float4 *full, c
     k_associate<<<(n_max[w] + 255) / 256, 256, 0, st>>>(src[w], m->d_stack[w], m->d_cnt + w, m->tobe, 0);
     k_associate<<<(n_max[w] + 255) / 256, 256, 0, st>>>(m->d_stack[w], m->d_stack[w], m->d_cnt + w, m->tobe, 1);
   }
-  if (m->mb && n_max[2] > 0 && full != m->d_full_in)
+  if ((m->mb || m->publish) && n_max[2] > 0 && full != m->d_full_in)
     k_copy_counted<<<std::max(1, std::min(4 * m->sm, (n_max[2] + 255) / 256)), 256, 0, st>>>(full, m->d_full_in, m->d_cnt + 4);
   LIO_CUDA_OK(cudaGetLastError());
   return LIO_OK;
@@ -475,33 +482,85 @@ static int pm_optimise(lio_pm *m, const int K[2], const int n_ds[2], int variant
 static TwistF tf7_to_twist(const float t[7]) { return TwistF{t[0], t[1], t[2], t[3], t[4], t[5], t[6]}; }
 static void twist_to_tf7(const TwistF &t, float o[7]) { o[0] = t.qx; o[1] = t.qy; o[2] = t.qz; o[3] = t.qw; o[4] = t.px; o[5] = t.py; o[6] = t.pz; }
 
-// PointMapping::Process (:765-1052), imu_inited_ == false, num_stack_frames_ == 1.  Clouds: HOST arrays of n x 4 floats.
-extern "C" int lio_pm_process_host(lio_pm *m, const float *corner_last, int nc, const float *surf_last, int ns, const float transform_sum7[7],
-                                   float transform_tobe_mapped7[7], int info3[3]) {
-  if (!m || m->mb || !transform_sum7 || nc < 0 || ns < 0 || (nc > 0 && !corner_last) || (ns > 0 && !surf_last)) return LIO_ERR_INVALID;
-  if (nc > m->max_points || ns > m->max_points) return LIO_ERR_CAPACITY;
-  LIO_CUDA_OK(cudaSetDevice(m->device));
-  const float *src[2] = {corner_last, surf_last};
-  const int nin[2] = {nc, ns};
+static int mb_surround(lio_pm *m, const std::vector<size_t> &surround);
+
+// PublishResults (PointMapping.cc:1210-1270) / PublishMapBuilderResults (MapBuilder.cc:144-218): the surround map every
+// num_map_frames_ (5) calls, the first call included, and the nf-point full cloud in d_full_in to the map frame with the final
+// tobe every call.  The only synchronisation is the read of the surround size on calls that publish it.
+static int pm_publish(lio_pm *m, const std::vector<size_t> &surround, int nf, bool &published) {
+  cudaStream_t st = m->stream;
+  published = ++m->map_frame_count >= 5;
+  if (published) {
+    m->map_frame_count = 0;
+    int rc = mb_surround(m, surround);
+    if (rc != LIO_OK) return rc;
+  }
+  if (nf > 0) k_associate<<<(nf + 255) / 256, 256, 0, st>>>(m->d_full_in, m->d_full_out, m->d_cnt + 4, m->tobe, 0);
+  m->n_full = nf;
+  if (published) {
+    LIO_CUDA_OK(cudaMemcpyAsync(m->h_sur_n, m->d_cnt + 6, sizeof(int), cudaMemcpyDeviceToHost, st));
+    LIO_CUDA_OK(cudaStreamSynchronize(st));
+    m->n_surround = *m->h_sur_n;
+  }
+  LIO_CUDA_OK(cudaGetLastError());
+  return LIO_OK;
+}
+
+// PointMapping::Process (:765-1052), imu_inited_ == false, num_stack_frames_ == 1, followed on a publishing handle by
+// PublishResults (:1210-1270).  Device sources, device counts {corner, surf, full}, host bounds n_max (already capped).
+static int pm_process(lio_pm *m, const float4 *const src[2], const float4 *full, const int *n3_dev, const int n_max[3], const float transform_sum7[7],
+                      float transform_tobe_mapped7[7], float transform_aft_mapped7[7], int *info, int n_info) {
+  const int nin[2] = {n_max[0], n_max[1]};
+  m->started = true;
   m->sum = tf7_to_twist(transform_sum7);
   m->tobe = twist_mul(m->tobe, twist_mul(twist_inverse(m->bef), m->sum));   // TransformAssociateToMap :753-756
-  int rc = pm_upload(m, src, nin, nullptr, 0);
+  int rc = pm_stack(m, src, full, n3_dev, n_max);
   if (rc != LIO_OK) return rc;
-  const float4 *dsrc[2] = {m->d_in[0], m->d_in[1]};
-  const int n_max[3] = {nc, ns, 0};
-  if ((rc = pm_stack(m, dsrc, nullptr, m->d_cnt + 8, n_max)) != LIO_OK) return rc;
-  std::vector<size_t> valid;
+  std::vector<size_t> valid, surround;
   int K[2] = {0, 0}, n_ds[2] = {0, 0};
-  if ((rc = pm_locate(m, valid, nullptr, K)) != LIO_OK) return rc;
+  if ((rc = pm_locate(m, valid, m->publish ? &surround : nullptr, K)) != LIO_OK) return rc;
   if ((rc = pm_downsample(m, nin, n_ds)) != LIO_OK) return rc;
   const bool optimised = !(K[0] <= 10 || K[1] <= 100);
   m->last_iters = 0;
   if (optimised && (rc = pm_optimise(m, K, n_ds, 0)) != LIO_OK) return rc;
   if (optimised) { m->bef = m->sum; m->aft = m->tobe; }   // TransformUpdate sits behind the optimiser's early return (:327-329, :716)
   if ((rc = pm_update(m, valid, n_ds)) != LIO_OK) return rc;
+  bool published = false;
+  if (m->publish && (rc = pm_publish(m, surround, n_max[2] > 0 ? m->h_cnt[4] : 0, published)) != LIO_OK) return rc;
   if (transform_tobe_mapped7) twist_to_tf7(m->tobe, transform_tobe_mapped7);
-  if (info3) { info3[0] = m->last_iters; info3[1] = K[0]; info3[2] = K[1]; }
+  if (transform_aft_mapped7) twist_to_tf7(m->aft, transform_aft_mapped7);
+  const int out[5] = {m->last_iters, K[0], K[1], published ? 1 : 0, m->publish ? m->n_surround : 0};
+  if (info) for (int k = 0; k < n_info; ++k) info[k] = out[k];
   return LIO_OK;
+}
+
+// Clouds: HOST arrays of n x 4 floats.
+extern "C" int lio_pm_process_host(lio_pm *m, const float *corner_last, int nc, const float *surf_last, int ns, const float transform_sum7[7],
+                                   float transform_tobe_mapped7[7], int info3[3]) {
+  if (!m || m->mb || m->publish || !transform_sum7 || nc < 0 || ns < 0 || (nc > 0 && !corner_last) || (ns > 0 && !surf_last)) return LIO_ERR_INVALID;
+  if (nc > m->max_points || ns > m->max_points) return LIO_ERR_CAPACITY;
+  LIO_CUDA_OK(cudaSetDevice(m->device));
+  const float *src[2] = {corner_last, surf_last};
+  const int nin[2] = {nc, ns};
+  int rc = pm_upload(m, src, nin, nullptr, 0);
+  if (rc != LIO_OK) return rc;
+  const float4 *dsrc[2] = {m->d_in[0], m->d_in[1]};
+  const int n_max[3] = {nc, ns, 0};
+  return pm_process(m, dsrc, nullptr, m->d_cnt + 8, n_max, transform_sum7, transform_tobe_mapped7, nullptr, info3, 3);
+}
+
+extern "C" int lio_pm_process_dev(lio_pm *m, const float *corner_dev, const float *surf_dev, const float *full_dev, const int *n3_dev,
+                                  const int n3_max[3], const float transform_sum7[7], float transform_tobe_mapped7[7], float transform_aft_mapped7[7],
+                                  int info5[5]) {
+  if (!m || m->mb || !transform_sum7 || !n3_dev || !n3_max || n3_max[0] < 0 || n3_max[1] < 0 || n3_max[2] < 0 || (n3_max[0] > 0 && !corner_dev) ||
+      (n3_max[1] > 0 && !surf_dev) || (m->publish && n3_max[2] > 0 && !full_dev))
+    return LIO_ERR_INVALID;
+  LIO_CUDA_OK(cudaSetDevice(m->device));
+  const float4 *dsrc[2] = {reinterpret_cast<const float4 *>(corner_dev), reinterpret_cast<const float4 *>(surf_dev)};
+  // without publishing the full cloud is not read: its count gets no bound, so it never reports an overflow
+  const int n_max[3] = {std::min(n3_max[0], m->max_points), std::min(n3_max[1], m->max_points), m->publish ? std::min(n3_max[2], m->max_full) : INT_MAX};
+  return pm_process(m, dsrc, m->publish ? reinterpret_cast<const float4 *>(full_dev) : nullptr, n3_dev, n_max, transform_sum7, transform_tobe_mapped7,
+                    transform_aft_mapped7, info5, 5);
 }
 
 // ---- lio::MapBuilder (src/map_builder/MapBuilder.cc) -----------------------------------------------------------------------
@@ -566,6 +625,26 @@ static int mb_surround(lio_pm *m, const std::vector<size_t> &surround) {
   return m->vg_sur.run(m->d_sur, m->d_cnt + 5, total, m->map_leaf, m->d_sur_ds, m->sur_cap, m->d_cnt + 6, nullptr, st, nullptr);
 }
 
+// Buffers of the published clouds (full cloud in / registered, surround segments); the surround map itself grows on demand.
+// On failure nothing stays allocated and the handle does not publish.
+static bool pm_alloc_publish(lio_pm *m, int max_full_points) {
+  m->max_full = max_full_points;
+  bool ok = cudaMalloc(&m->d_full_in, sizeof(float4) * max_full_points) == cudaSuccess;
+  ok = ok && cudaMalloc(&m->d_full_out, sizeof(float4) * max_full_points) == cudaSuccess;
+  ok = ok && cudaMalloc(&m->d_sur_seg, sizeof(Segment) * 2 * 125) == cudaSuccess;
+  ok = ok && cudaMallocHost(&m->h_sur_seg, sizeof(Segment) * 2 * 125) == cudaSuccess;
+  ok = ok && cudaMallocHost(&m->h_sur_n, sizeof(int)) == cudaSuccess;
+  if (!ok) {
+    void *fr[] = {m->d_full_in, m->d_full_out, m->d_sur_seg};
+    for (void *q : fr) if (q) cudaFree(q);
+    if (m->h_sur_seg) cudaFreeHost(m->h_sur_seg);
+    if (m->h_sur_n) cudaFreeHost(m->h_sur_n);
+    m->d_full_in = m->d_full_out = nullptr; m->d_sur_seg = m->h_sur_seg = nullptr; m->h_sur_n = nullptr;
+    m->max_full = 0;
+  }
+  return ok;
+}
+
 extern "C" void lio_mb_default_config(lio_mb_config *cfg) {
   if (!cfg) return;
   cfg->corner_filter_size = 0.2f; cfg->surf_filter_size = 0.4f; cfg->map_filter_size = 0.2f;
@@ -580,14 +659,21 @@ extern "C" int lio_mb_create(const lio_mb_config *cfg, int max_points, int max_f
                          cfg->max_iterations, device, cuda_stream, &m);
   if (rc != LIO_OK) return rc;
   m->mb = true; m->enable_4d = cfg->enable_4d != 0; m->skip_count = cfg->skip_count; m->map_leaf = cfg->map_filter_size;
-  m->max_full = max_full_points;
-  bool ok = cudaMalloc(&m->d_full_in, sizeof(float4) * max_full_points) == cudaSuccess;
-  ok = ok && cudaMalloc(&m->d_full_out, sizeof(float4) * max_full_points) == cudaSuccess;
-  ok = ok && cudaMalloc(&m->d_sur_seg, sizeof(Segment) * 2 * 125) == cudaSuccess;
-  ok = ok && cudaMallocHost(&m->h_sur_seg, sizeof(Segment) * 2 * 125) == cudaSuccess;
-  ok = ok && cudaMallocHost(&m->h_sur_n, sizeof(int)) == cudaSuccess;
-  if (!ok) { lio_set_last_error(__FILE__, __LINE__, "lio_mb_create: allocation failed"); lio_pm_destroy(m); return LIO_ERR_CUDA; }
+  if (!pm_alloc_publish(m, max_full_points)) { lio_set_last_error(__FILE__, __LINE__, "lio_mb_create: allocation failed"); lio_pm_destroy(m); return LIO_ERR_CUDA; }
   *out = m;
+  return LIO_OK;
+}
+
+extern "C" int lio_pm_enable_publish(lio_pm *m, float map_filter_size, int max_full_points) {
+  if (!m || m->mb || m->publish || m->started || !(map_filter_size > 0) || max_full_points < 1) {
+    if (m && (m->mb || m->publish || m->started))
+      lio_set_last_error(__FILE__, __LINE__, "lio_pm_enable_publish: only once, on a plain PointMapping handle, before its first process call");
+    return LIO_ERR_INVALID;
+  }
+  LIO_CUDA_OK(cudaSetDevice(m->device));
+  if (!pm_alloc_publish(m, max_full_points)) { lio_set_last_error(__FILE__, __LINE__, "lio_pm_enable_publish: allocation failed"); return LIO_ERR_CUDA; }
+  m->map_leaf = map_filter_size;
+  m->publish = true;
   return LIO_OK;
 }
 
@@ -595,7 +681,6 @@ extern "C" int lio_mb_create(const lio_mb_config *cfg, int max_points, int max_f
 // Device sources, device counts {corner, surf, full}, host bounds n_max (already capped by the capacities).
 static int mb_process_map(lio_pm *m, const float4 *const src[2], const float4 *full, const int *n3_dev, const int n_max[3],
                           const float transform_sum7[7], float transform_tobe_mapped7[7], float transform_aft_mapped7[7], int info6[6]) {
-  cudaStream_t st = m->stream;
   const int nin[2] = {n_max[0], n_max[1]};
   m->sum = tf7_to_twist(transform_sum7);
   if (!m->system_init) { m->system_init = true; m->bef = m->sum; m->tobe = m->sum; m->aft = m->tobe; }   // :227-232
@@ -622,19 +707,8 @@ static int mb_process_map(lio_pm *m, const float4 *const src[2], const float4 *f
   ++m->odom_count;
   if ((rc = pm_update(m, valid, n_ds)) != LIO_OK) return rc;
   // PublishMapBuilderResults: surround map every num_map_frames_ (5) frames, registered full cloud every frame
-  const bool publish = ++m->map_frame_count >= 5;
-  if (publish) {
-    m->map_frame_count = 0;
-    if ((rc = mb_surround(m, surround)) != LIO_OK) return rc;
-  }
-  if (nf > 0) k_associate<<<(nf + 255) / 256, 256, 0, st>>>(m->d_full_in, m->d_full_out, m->d_cnt + 4, m->tobe, 0);
-  m->n_full = nf;
-  if (publish) {
-    LIO_CUDA_OK(cudaMemcpyAsync(m->h_sur_n, m->d_cnt + 6, sizeof(int), cudaMemcpyDeviceToHost, st));
-    LIO_CUDA_OK(cudaStreamSynchronize(st));
-    m->n_surround = *m->h_sur_n;
-  }
-  LIO_CUDA_OK(cudaGetLastError());
+  bool publish = false;
+  if ((rc = pm_publish(m, surround, nf, publish)) != LIO_OK) return rc;
   if (transform_tobe_mapped7) twist_to_tf7(m->tobe, transform_tobe_mapped7);
   if (transform_aft_mapped7) twist_to_tf7(m->aft, transform_aft_mapped7);
   if (info6) { info6[0] = m->last_iters; info6[1] = gate; info6[2] = K[0]; info6[3] = K[1]; info6[4] = publish; info6[5] = m->n_surround; }
@@ -671,13 +745,13 @@ extern "C" int lio_mb_process_map_dev(lio_pm *m, const float *corner_dev, const 
 }
 
 extern "C" int lio_mb_surround_dev(lio_pm *m, const float **ptr, int *n) {
-  if (!m || !m->mb || !ptr || !n) return LIO_ERR_INVALID;
+  if (!m || !(m->mb || m->publish) || !ptr || !n) return LIO_ERR_INVALID;
   *ptr = (const float *)m->d_sur_ds; *n = m->n_surround;
   return LIO_OK;
 }
 
 extern "C" int lio_mb_full_dev(lio_pm *m, const float **ptr, int *n) {
-  if (!m || !m->mb || !ptr || !n) return LIO_ERR_INVALID;
+  if (!m || !(m->mb || m->publish) || !ptr || !n) return LIO_ERR_INVALID;
   *ptr = (const float *)m->d_full_out; *n = m->n_full;
   return LIO_OK;
 }
@@ -692,12 +766,12 @@ static int mb_download(lio_pm *m, const float4 *src, int count, float *out, int 
 }
 
 extern "C" int lio_mb_surround_download(lio_pm *m, float *out_xyzi, int cap, int *n) {
-  if (!m || !m->mb || !n || (!out_xyzi && cap > 0)) return LIO_ERR_INVALID;
+  if (!m || !(m->mb || m->publish) || !n || (!out_xyzi && cap > 0)) return LIO_ERR_INVALID;
   return mb_download(m, m->d_sur_ds, m->n_surround, out_xyzi, cap, n);
 }
 
 extern "C" int lio_mb_full_download(lio_pm *m, float *out_xyzi, int cap, int *n) {
-  if (!m || !m->mb || !n || (!out_xyzi && cap > 0)) return LIO_ERR_INVALID;
+  if (!m || !(m->mb || m->publish) || !n || (!out_xyzi && cap > 0)) return LIO_ERR_INVALID;
   return mb_download(m, m->d_full_out, m->n_full, out_xyzi, cap, n);
 }
 

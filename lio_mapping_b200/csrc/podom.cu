@@ -15,7 +15,9 @@
 // coefficients from the stored indices, the 6 x 6 normal equations (float products accumulated in double, fixed tree),
 // colPivHouseholderQr solve, the first-iteration degeneracy projection and the convergence test; the iteration chain is
 // enqueued once and later rounds return at once when the state says converged.  Pose compositions happen once per sweep on the
-// host in the reference's float order (twistf.h).  Compiled with -fmad=false.
+// host in the reference's float order (twistf.h).  lio_po_process_host uploads the five clouds and runs po_run;
+// lio_po_process_dev (clouds in HBM, e.g. stage A's) copies the kept ones with po_stage and runs the same po_run.  Compiled with
+// -fmad=false.
 #include <algorithm>
 #include <cfloat>
 #include <cmath>
@@ -294,6 +296,40 @@ po_round(const float4 *__restrict__ sharp, int ns, const float4 *__restrict__ fl
   }
 }
 
+struct PoStage {                     // lio_po_process_dev, by value: the five count pointers and the clouds a call keeps, copied into
+  const int *n[5];                   // the context's own buffers (less_sharp, less_flat, full)
+  const float4 *src[3];
+  float4 *dst[3];
+};
+
+// Input counts {sharp, less_sharp, flat, less_flat, full} read on the device and clamped to n_max into cnt[0..4]; cnt[5] = 1 when
+// a count exceeded its bound.  Without an overflow the kept clouds are copied (count-guarded, grid-stride, blockIdx.y = cloud)
+// and pub_n = {less_sharp, less_flat, full}, the counts the clouds will have once they are the published ones; with an overflow
+// nothing of the context is written but cnt.
+__global__ void __launch_bounds__(256)
+po_stage(PoStage s, int n0, int n1, int n2, int n3, int n4, int *__restrict__ cnt, int *__restrict__ pub_n) {
+  const int mx[5] = {n0, n1, n2, n3, n4};
+  int v[5], over = 0;
+#pragma unroll
+  for (int k = 0; k < 5; ++k) {
+    v[k] = *s.n[k];
+    if (v[k] > mx[k]) { over = 1; v[k] = mx[k]; }
+    if (v[k] < 0) v[k] = 0;
+  }
+  if (blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) {
+#pragma unroll
+    for (int k = 0; k < 5; ++k) cnt[k] = v[k];
+    cnt[5] = over;
+    if (!over) { pub_n[0] = v[1]; pub_n[1] = v[3]; pub_n[2] = v[4]; }
+  }
+  if (over) return;
+  const int w = blockIdx.y;
+  const int n = w == 0 ? v[1] : w == 1 ? v[3] : v[4];
+  const float4 *__restrict__ in = w == 0 ? s.src[0] : w == 1 ? s.src[1] : s.src[2];   // constant indices: no local-memory copy of s
+  float4 *__restrict__ out = w == 0 ? s.dst[0] : w == 1 ? s.dst[1] : s.dst[2];
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) out[i] = __ldg(in + i);
+}
+
 }  // namespace lio
 
 using namespace lio;
@@ -301,6 +337,7 @@ using namespace lio;
 struct lio_po {
   int device = 0;
   cudaStream_t stream = nullptr;
+  int sm = 132;
   float time_factor = 10.f;
   int io_ratio = 2, max_iter = 25;
   int cap_feat = 0, cap_full = 0;
@@ -310,6 +347,9 @@ struct lio_po {
          *d_full = nullptr;
   int n_sharp = 0, n_flat = 0, n_less_sharp = 0, n_less_flat = 0, n_last_corner = 0, n_last_surf = 0, n_full = 0;
   int *d_idx_c = nullptr, *d_idx_s = nullptr, *d_nsel = nullptr;
+  int *d_cnt = nullptr;                // lio_po_process_dev: [0..4] clamped input counts, [5] a count over its bound
+  int h_cnt[6] = {};                   // their read-back
+  int *d_pub_n = nullptr;              // counts of the published clouds {last_corner, last_surf, full} (lio_po_clouds_dev)
   TransformF *d_tf = nullptr;
   OdomState *d_odom = nullptr;
   TwistF es, sum;
@@ -321,7 +361,7 @@ extern "C" int lio_po_destroy(lio_po *p) {
   if (!p) return LIO_OK;
   cudaSetDevice(p->device);
   void *fr[] = {p->d_sharp, p->d_flat, p->d_less_sharp, p->d_less_flat, p->d_last_corner, p->d_last_surf, p->d_full, p->d_idx_c, p->d_idx_s,
-                p->d_nsel, p->d_tf, p->d_odom};
+                p->d_nsel, p->d_cnt, p->d_pub_n, p->d_tf, p->d_odom};
   for (void *q : fr) if (q) cudaFree(q);
   delete p;
   return LIO_OK;
@@ -335,6 +375,7 @@ extern "C" int lio_po_create(float scan_period, int io_ratio, int num_max_iterat
   lio_po *p = new (std::nothrow) lio_po();
   if (!p) return LIO_ERR_INVALID;
   p->device = device; p->stream = (cudaStream_t)cuda_stream;
+  cudaDeviceGetAttribute(&p->sm, cudaDevAttrMultiProcessorCount, device);
   p->time_factor = 1 / scan_period; p->io_ratio = io_ratio; p->max_iter = num_max_iterations;
   p->cap_feat = max_feature_points; p->cap_full = max_full_points;
   bool ok = true;
@@ -346,6 +387,9 @@ extern "C" int lio_po_create(float scan_period, int io_ratio, int num_max_iterat
   ok = ok && cudaMalloc(&p->d_nsel, sizeof(int)) == cudaSuccess;
   ok = ok && cudaMalloc(&p->d_tf, sizeof(TransformF)) == cudaSuccess;
   ok = ok && cudaMalloc(&p->d_odom, sizeof(OdomState)) == cudaSuccess;
+  ok = ok && cudaMalloc(&p->d_cnt, sizeof(int) * 6) == cudaSuccess;
+  ok = ok && cudaMalloc(&p->d_pub_n, sizeof(int) * 3) == cudaSuccess;
+  ok = ok && cudaMemset(p->d_pub_n, 0, sizeof(int) * 3) == cudaSuccess;
   if (!ok) { lio_set_last_error(__FILE__, __LINE__, "lio_po_create: device allocation failed"); lio_po_destroy(p); return LIO_ERR_CUDA; }
   *out = p;
   return LIO_OK;
@@ -359,27 +403,18 @@ extern "C" int lio_po_set_enable_odom(lio_po *p, int enable) {   // the /enable_
 
 static void po_store(const TwistF &t, float *o) { o[0] = t.qx; o[1] = t.qy; o[2] = t.qz; o[3] = t.qw; o[4] = t.px; o[5] = t.py; o[6] = t.pz; }
 
-extern "C" int lio_po_process_host(lio_po *p, const float *sharp, int n_sharp, const float *less_sharp, int n_less_sharp, const float *flat,
-                                   int n_flat, const float *less_flat, int n_less_flat, const float *full, int n_full, float transform_sum7[7],
-                                   float transform_es7[7], int info4[4]) {
-  if (!p || n_sharp < 0 || n_less_sharp < 0 || n_flat < 0 || n_less_flat < 0 || n_full < 0 || (n_sharp && !sharp) || (n_less_sharp && !less_sharp) ||
-      (n_flat && !flat) || (n_less_flat && !less_flat) || (n_full && !full))
-    return LIO_ERR_INVALID;
-  if (std::max(std::max(n_sharp, n_less_sharp), std::max(n_flat, n_less_flat)) > p->cap_feat || n_full > p->cap_full) {
-    lio_set_last_error(__FILE__, __LINE__, "lio_po_process_host: a cloud exceeds the capacity given to lio_po_create");
-    return LIO_ERR_CAPACITY;
-  }
-  LIO_CUDA_OK(cudaSetDevice(p->device));
+// Process() + PublishResults() (:294-766) of one sweep whose kept clouds (less_sharp, less_flat, full) are in the context's own
+// buffers and whose counts are known on the host; sharp / flat are only read, wherever they are.  Synchronises the stream after the
+// iterations when odometry runs, and at the end only when sync_end is set.
+static int po_run(lio_po *p, const float4 *sharp, int n_sharp, int n_less_sharp, const float4 *flat, int n_flat, int n_less_flat, int n_full,
+                  bool sync_end, float transform_sum7[7], float transform_es7[7], int info4[4]) {
   cudaStream_t st = p->stream;
-  const float *src[5] = {sharp, less_sharp, flat, less_flat, full};
-  float4 *dst[5] = {p->d_sharp, p->d_less_sharp, p->d_flat, p->d_less_flat, p->d_full};
-  const int cnt[5] = {n_sharp, n_less_sharp, n_flat, n_less_flat, n_full};
-  for (int k = 0; k < 5; ++k)
-    if (cnt[k]) LIO_CUDA_OK(cudaMemcpyAsync(dst[k], src[k], sizeof(float4) * cnt[k], cudaMemcpyHostToDevice, st));
   p->n_sharp = n_sharp; p->n_less_sharp = n_less_sharp; p->n_flat = n_flat; p->n_less_flat = n_less_flat; p->n_full = n_full;
   p->published = 0; p->launches = 0;
   int iters = 0, nsel = 0;
   auto finish = [&]() {
+    if (sync_end) LIO_CUDA_OK(cudaStreamSynchronize(st));
+    LIO_CUDA_OK(cudaGetLastError());
     if (transform_sum7) po_store(p->sum, transform_sum7);
     if (transform_es7) po_store(p->es, transform_es7);
     if (info4) { info4[0] = iters; info4[1] = p->published; info4[2] = (int)p->frame_count; info4[3] = nsel; }
@@ -392,7 +427,6 @@ extern "C" int lio_po_process_host(lio_po *p, const float *sharp, int n_sharp, c
   if (!p->system_inited) {   // :302-310
     swap_in();
     p->system_inited = true;
-    LIO_CUDA_OK(cudaStreamSynchronize(st));
     return finish();
   }
   ++p->frame_count;
@@ -408,10 +442,10 @@ extern "C" int lio_po_process_host(lio_po *p, const float *sharp, int n_sharp, c
       LIO_CUDA_OK(cudaMemsetAsync(p->d_nsel, 0, sizeof(int), st));
       for (int it = 0; it < p->max_iter; ++it) {
         if (it % 5 == 0) {
-          if (n_sharp) { po_search<0><<<(n_sharp + kPoQ - 1) / kPoQ, kPoSearchThreads, 0, st>>>(p->d_sharp, n_sharp, p->d_last_corner, p->n_last_corner, p->d_tf, p->d_odom, tfac, p->d_idx_c); ++p->launches; }
-          if (n_flat) { po_search<1><<<(n_flat + kPoQ - 1) / kPoQ, kPoSearchThreads, 0, st>>>(p->d_flat, n_flat, p->d_last_surf, p->n_last_surf, p->d_tf, p->d_odom, tfac, p->d_idx_s); ++p->launches; }
+          if (n_sharp) { po_search<0><<<(n_sharp + kPoQ - 1) / kPoQ, kPoSearchThreads, 0, st>>>(sharp, n_sharp, p->d_last_corner, p->n_last_corner, p->d_tf, p->d_odom, tfac, p->d_idx_c); ++p->launches; }
+          if (n_flat) { po_search<1><<<(n_flat + kPoQ - 1) / kPoQ, kPoSearchThreads, 0, st>>>(flat, n_flat, p->d_last_surf, p->n_last_surf, p->d_tf, p->d_odom, tfac, p->d_idx_s); ++p->launches; }
         }
-        po_round<<<1, kPoRoundThreads, 0, st>>>(p->d_sharp, n_sharp, p->d_flat, n_flat, p->d_last_corner, p->d_last_surf, p->d_idx_c, p->d_idx_s, p->d_tf,
+        po_round<<<1, kPoRoundThreads, 0, st>>>(sharp, n_sharp, flat, n_flat, p->d_last_corner, p->d_last_surf, p->d_idx_c, p->d_idx_s, p->d_tf,
                                                p->d_odom, tfac, it, p->d_nsel);
         ++p->launches;
       }
@@ -436,9 +470,67 @@ extern "C" int lio_po_process_host(lio_po *p, const float *sharp, int n_sharp, c
     if (p->enable_odom) to_end(p->d_full, p->n_full);
     p->published = 1;
   }
+  return finish();
+}
+
+extern "C" int lio_po_process_host(lio_po *p, const float *sharp, int n_sharp, const float *less_sharp, int n_less_sharp, const float *flat,
+                                   int n_flat, const float *less_flat, int n_less_flat, const float *full, int n_full, float transform_sum7[7],
+                                   float transform_es7[7], int info4[4]) {
+  if (!p || n_sharp < 0 || n_less_sharp < 0 || n_flat < 0 || n_less_flat < 0 || n_full < 0 || (n_sharp && !sharp) || (n_less_sharp && !less_sharp) ||
+      (n_flat && !flat) || (n_less_flat && !less_flat) || (n_full && !full))
+    return LIO_ERR_INVALID;
+  if (std::max(std::max(n_sharp, n_less_sharp), std::max(n_flat, n_less_flat)) > p->cap_feat || n_full > p->cap_full) {
+    lio_set_last_error(__FILE__, __LINE__, "lio_po_process_host: a cloud exceeds the capacity given to lio_po_create");
+    return LIO_ERR_CAPACITY;
+  }
+  LIO_CUDA_OK(cudaSetDevice(p->device));
+  cudaStream_t st = p->stream;
+  const float *src[5] = {sharp, less_sharp, flat, less_flat, full};
+  float4 *dst[5] = {p->d_sharp, p->d_less_sharp, p->d_flat, p->d_less_flat, p->d_full};
+  const int cnt[5] = {n_sharp, n_less_sharp, n_flat, n_less_flat, n_full};
+  for (int k = 0; k < 5; ++k)
+    if (cnt[k]) LIO_CUDA_OK(cudaMemcpyAsync(dst[k], src[k], sizeof(float4) * cnt[k], cudaMemcpyHostToDevice, st));
+  // the published counts {last_corner, last_surf, full} once the call is done (lio_po_clouds_dev); pub stays alive until the final sync
+  const int pub[3] = {n_less_sharp, n_less_flat, n_full};
+  LIO_CUDA_OK(cudaMemcpyAsync(p->d_pub_n, pub, sizeof(pub), cudaMemcpyHostToDevice, st));
+  return po_run(p, p->d_sharp, n_sharp, n_less_sharp, p->d_flat, n_flat, n_less_flat, n_full, true, transform_sum7, transform_es7, info4);
+}
+
+extern "C" int lio_po_process_dev(lio_po *p, const float *const clouds_dev[5], const int *const n_dev[5], const int n_max[5], float transform_sum7[7],
+                                  float transform_es7[7], int info4[4]) {
+  if (!p || !clouds_dev || !n_dev || !n_max) return LIO_ERR_INVALID;
+  for (int k = 0; k < 5; ++k)
+    if (n_max[k] < 0 || !n_dev[k] || (n_max[k] > 0 && !clouds_dev[k])) return LIO_ERR_INVALID;
+  if (std::max(std::max(n_max[0], n_max[1]), std::max(n_max[2], n_max[3])) > p->cap_feat || n_max[4] > p->cap_full) {
+    lio_set_last_error(__FILE__, __LINE__, "lio_po_process_dev: a bound n_max exceeds the capacity given to lio_po_create");
+    return LIO_ERR_CAPACITY;
+  }
+  LIO_CUDA_OK(cudaSetDevice(p->device));
+  cudaStream_t st = p->stream;
+  PoStage sg;
+  for (int k = 0; k < 5; ++k) sg.n[k] = n_dev[k];
+  sg.src[0] = reinterpret_cast<const float4 *>(clouds_dev[1]); sg.dst[0] = p->d_less_sharp;
+  sg.src[1] = reinterpret_cast<const float4 *>(clouds_dev[3]); sg.dst[1] = p->d_less_flat;
+  sg.src[2] = reinterpret_cast<const float4 *>(clouds_dev[4]); sg.dst[2] = p->d_full;
+  const int most = std::max(std::max(n_max[1], n_max[3]), n_max[4]);
+  po_stage<<<dim3(std::max(1, std::min(4 * p->sm, (most + 255) / 256)), 3), 256, 0, st>>>(sg, n_max[0], n_max[1], n_max[2], n_max[3], n_max[4],
+                                                                                        p->d_cnt, p->d_pub_n);
+  // one read-back of the clamped counts and the overflow flag; nothing of the context has changed when it reports an overflow
+  LIO_CUDA_OK(cudaMemcpyAsync(p->h_cnt, p->d_cnt, sizeof(p->h_cnt), cudaMemcpyDeviceToHost, st));
   LIO_CUDA_OK(cudaStreamSynchronize(st));
   LIO_CUDA_OK(cudaGetLastError());
-  return finish();
+  if (p->h_cnt[5]) { lio_set_last_error(__FILE__, __LINE__, "lio_po_process_dev: a device count exceeds its bound n_max"); return LIO_ERR_CAPACITY; }
+  const int *c = p->h_cnt;
+  return po_run(p, reinterpret_cast<const float4 *>(clouds_dev[0]), c[0], c[1], reinterpret_cast<const float4 *>(clouds_dev[2]), c[2], c[3], c[4],
+                false, transform_sum7, transform_es7, info4);
+}
+
+extern "C" int lio_po_clouds_dev(lio_po *p, const float *ptr[3], const int **n_dev, int n_host[3]) {
+  if (!p || !ptr || !n_dev || !n_host) return LIO_ERR_INVALID;
+  ptr[0] = (const float *)p->d_last_corner; ptr[1] = (const float *)p->d_last_surf; ptr[2] = (const float *)p->d_full;
+  *n_dev = p->d_pub_n;
+  n_host[0] = p->n_last_corner; n_host[1] = p->n_last_surf; n_host[2] = p->n_full;
+  return LIO_OK;
 }
 
 static int po_cloud(lio_po *p, int which, const float4 **d, int *n) {

@@ -28,8 +28,9 @@ def _cloud(a):
 
 
 class MapBuilder(PointMapping):
-    """lio::MapBuilder : PointMapping.  centre(), cube_sizes() and cube() of PointMapping apply unchanged; Process() does not
-    (the library rejects it on a map-builder context)."""
+    """lio::MapBuilder : PointMapping.  centre(), cube_sizes(), cube(), surround_map(_dev) and registered_full_cloud(_dev) of
+    PointMapping apply unchanged; Process(), ProcessDev() and EnablePublish() do not (the library rejects them on a map-builder
+    context)."""
 
     def __init__(self, max_points: int = 1 << 17, max_full_points: int = 1 << 18, device: int = 0, stream: int = 0, **cfg):
         _lib.require_device()
@@ -68,29 +69,3 @@ class MapBuilder(PointMapping):
         self.transform_aft_mapped = aft
         return tobe, dict(iterations=int(info[0]), optimised=bool(info[1]), corner_from_map=int(info[2]), surf_from_map=int(info[3]),
                           surround_published=bool(info[4]), surround_size=int(info[5]))
-
-    def _download(self, fn, count):
-        n = C.c_int()
-        out = np.zeros((max(count, 1), 4), np.float32)
-        _lib.check(fn(self.h, out, out.shape[0], C.byref(n)), fn.__name__)
-        return out[:n.value]
-
-    def surround_map(self):
-        """laser_cloud_surround_downsampled_ of the last publishing frame (frames 0, 5, 10, ...), (n, 4) float32."""
-        return self._download(_lib.lib().lio_mb_surround_download, self.surround_map_dev()[1])
-
-    def registered_full_cloud(self):
-        """The last full cloud in the map frame (/cloud_registered), (n, 4) float32."""
-        return self._download(_lib.lib().lio_mb_full_download, self.registered_full_cloud_dev()[1])
-
-    def surround_map_dev(self):
-        """(device pointer, count) of the surround map: float4 in HBM, valid until the next ProcessMap."""
-        n, p = C.c_int(), C.c_void_p()
-        _lib.check(_lib.lib().lio_mb_surround_dev(self.h, C.byref(p), C.byref(n)), "lio_mb_surround_dev")
-        return p.value, n.value
-
-    def registered_full_cloud_dev(self):
-        """(device pointer, count) of the registered full cloud, valid until the next ProcessMap."""
-        n, p = C.c_int(), C.c_void_p()
-        _lib.check(_lib.lib().lio_mb_full_dev(self.h, C.byref(p), C.byref(n)), "lio_mb_full_dev")
-        return p.value, n.value

@@ -42,6 +42,24 @@ class PointMapping:
                                                   np.ascontiguousarray(transform_sum7, np.float32), tobe, info), "lio_pm_process_host")
         return tobe, dict(iterations=int(info[0]), corner_from_map=int(info[1]), surf_from_map=int(info[2]))
 
+    def EnablePublish(self, map_filter_size: float = 0.6, max_full_points: int = 1 << 18):
+        """PointMapping::PublishResults (PointMapping.cc:1210-1270) on every ProcessDev: the surround map on calls 1, 6, 11, ...
+        through VoxelGrid(map_filter_size) (0.6, :123) and the registered full cloud.  Once, before the first Process / ProcessDev;
+        a publishing mapper takes ProcessDev only."""
+        _lib.check(_lib.lib().lio_pm_enable_publish(self.h, float(map_filter_size), int(max_full_points)), "lio_pm_enable_publish")
+
+    def ProcessDev(self, ptrs, n_dev_ptr: int, n_max, transform_sum7):
+        """Process with the clouds in HBM: ptrs = device pointers {corner, surf, full} of float4 arrays (full may be 0 without
+        EnablePublish), n_dev_ptr = device pointer of their int[3] counts, n_max = host bounds of the counts - exactly what
+        PointOdometry.clouds_dev() returns.  Returns (transform_tobe_mapped tf7, transform_aft_mapped tf7, info dict); info has
+        Process's keys plus surround_published and surround_size.  Stream rule: share the producer's stream or order the streams."""
+        tobe = np.zeros(7, np.float32); aft = np.zeros(7, np.float32); info = np.zeros(5, np.int32)
+        _lib.check(_lib.lib().lio_pm_process_dev(self.h, C.c_void_p(ptrs[0]), C.c_void_p(ptrs[1]), C.c_void_p(ptrs[2]), C.c_void_p(n_dev_ptr),
+                                                 np.ascontiguousarray(n_max, np.int32), np.ascontiguousarray(transform_sum7, np.float32),
+                                                 tobe, aft, info), "lio_pm_process_dev")
+        return tobe, aft, dict(iterations=int(info[0]), corner_from_map=int(info[1]), surf_from_map=int(info[2]),
+                               surround_published=bool(info[3]), surround_size=int(info[4]))
+
     def centre(self):
         out = np.zeros(3, np.int32)
         _lib.check(_lib.lib().lio_pm_map_centre(self.h, out), "lio_pm_map_centre")
@@ -64,3 +82,30 @@ class PointMapping:
         out = np.zeros((max(n.value, 1), 4), np.float32)
         _lib.check(_lib.lib().lio_pm_cube_download(self.h, int(index), w, out, out.shape[0]), "lio_pm_cube_download")
         return out[:n.value]
+
+    def _download(self, fn, count):
+        n = C.c_int()
+        out = np.zeros((max(count, 1), 4), np.float32)
+        _lib.check(fn(self.h, out, out.shape[0], C.byref(n)), fn.__name__)
+        return out[:n.value]
+
+    def surround_map(self):
+        """laser_cloud_surround_downsampled_ of the last publishing call (calls 1, 6, 11, ...), (n, 4) float32.  Needs a publishing
+        mapper (EnablePublish) or a MapBuilder."""
+        return self._download(_lib.lib().lio_mb_surround_download, self.surround_map_dev()[1])
+
+    def registered_full_cloud(self):
+        """The last full cloud in the map frame (/cloud_registered), (n, 4) float32."""
+        return self._download(_lib.lib().lio_mb_full_download, self.registered_full_cloud_dev()[1])
+
+    def surround_map_dev(self):
+        """(device pointer, count) of the surround map: float4 in HBM, valid until the next process call."""
+        n, p = C.c_int(), C.c_void_p()
+        _lib.check(_lib.lib().lio_mb_surround_dev(self.h, C.byref(p), C.byref(n)), "lio_mb_surround_dev")
+        return p.value, n.value
+
+    def registered_full_cloud_dev(self):
+        """(device pointer, count) of the registered full cloud, valid until the next process call."""
+        n, p = C.c_int(), C.c_void_p()
+        _lib.check(_lib.lib().lio_mb_full_dev(self.h, C.byref(p), C.byref(n)), "lio_mb_full_dev")
+        return p.value, n.value

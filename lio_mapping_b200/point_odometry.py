@@ -47,6 +47,25 @@ class PointOdometry:
         _lib.check(_lib.lib().lio_po_process_host(self.h, *args, ts, te, info), "lio_po_process_host")
         return ts, te, dict(iterations=int(info[0]), published=int(info[1]), frame_count=int(info[2]), matches=int(info[3]))
 
+    def ProcessDev(self, ptrs, n_dev_ptrs, n_max):
+        """Process with the five clouds in HBM: ptrs / n_dev_ptrs = device pointers of the float4 clouds {sharp, less_sharp, flat,
+        less_flat, full} and of one int count each (PointProcessor.cloud_dev / cloud_count_dev), n_max = host bounds of the counts.
+        Same return value as Process; less_sharp, less_flat and full are copied, sharp and flat are read during the call.  Stream
+        rule: share the producer's stream or order the two streams."""
+        clouds = (C.c_void_p * 5)(*[C.c_void_p(int(p)) for p in ptrs])
+        counts = (C.c_void_p * 5)(*[C.c_void_p(int(p)) for p in n_dev_ptrs])
+        ts = np.zeros(7, np.float32); te = np.zeros(7, np.float32); info = np.zeros(4, np.int32)
+        _lib.check(_lib.lib().lio_po_process_dev(self.h, clouds, counts, np.ascontiguousarray(n_max, np.int32), ts, te, info),
+                   "lio_po_process_dev")
+        return ts, te, dict(iterations=int(info[0]), published=int(info[1]), frame_count=int(info[2]), matches=int(info[3]))
+
+    def clouds_dev(self):
+        """(device pointers {last_corner, last_surf, full}, device pointer of their int[3] counts, host counts): the published clouds in
+        HBM, what PointMapping.ProcessDev takes.  The pointers are valid until the next process call; the count pointer is stable."""
+        ptr = (C.c_void_p * 3)(); n_dev = C.c_void_p(); n = np.zeros(3, np.int32)
+        _lib.check(_lib.lib().lio_po_clouds_dev(self.h, ptr, C.byref(n_dev), n), "lio_po_clouds_dev")
+        return [p or 0 for p in ptr], n_dev.value, n.tolist()
+
     def cloud(self, which: str):
         w = _WHICH[which]
         n = C.c_int()

@@ -88,6 +88,12 @@ class PointProcessor:
         _lib.check(_lib.lib().lio_pp_cloud_dev(self._h, CLOUDS[name], C.byref(p)), "lio_pp_cloud_dev")
         return p.value
 
+    def cloud_count_dev(self, name: str) -> int:
+        """Device pointer of the int point count of one output cloud (stable), to chain stage A into the next stage on the device."""
+        p = C.c_void_p()
+        _lib.check(_lib.lib().lio_pp_cloud_count_dev(self._h, CLOUDS[name], C.byref(p)), "lio_pp_cloud_count_dev")
+        return p.value
+
     def index(self, name: str) -> np.ndarray:
         cap = self.sizes()["laser_scans"] + 1
         out = np.zeros(cap, np.int32)

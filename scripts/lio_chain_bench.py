@@ -15,7 +15,6 @@ synchronise.  The script also checks that both chains produced identical map-bui
 from __future__ import annotations
 
 import argparse
-import ctypes as C
 import json
 import os
 import sys
@@ -38,7 +37,7 @@ def main():
     import torch
     if not torch.cuda.is_available():
         raise SystemExit("lio_chain_bench: no CUDA device")
-    from lio_mapping_b200 import _lib, estimator, ops, scenario
+    from lio_mapping_b200 import estimator, ops, scenario
     from lio_mapping_b200.map_builder import MapBuilder
     from lio_mapping_b200.point_processor import PointProcessor
     W = O = scenario.WINDOWS["hdl64"]
@@ -48,14 +47,9 @@ def main():
     max_raw = max(s.shape[0] for s in scn.raw)
     cfg = dict(scenario.EST_CFG["hdl64"])
     pp = PointProcessor(sensor.lower_deg, sensor.upper_deg, sensor.rings, max_points=max_raw)
-    L = _lib.lib()
     names = {1: "cloud_in_rings", 3: "corner_points_less_sharp", 5: "surface_points_less_flat"}
-    ptr, cnt = {}, {}
-    for w, name in names.items():
-        ptr[w] = pp.cloud_dev(name)
-        p = C.c_void_p()
-        _lib.check(L.lio_pp_cloud_count_dev(pp._h, w, C.byref(p)), "lio_pp_cloud_count_dev")
-        cnt[w] = p.value
+    ptr = {w: pp.cloud_dev(name) for w, name in names.items()}
+    cnt = {w: pp.cloud_count_dev(name) for w, name in names.items()}
     warm = []
     for k in range(W):   # warm-start clouds: frame k's down-sampled surf / corner and its full cloud
         pp.SetInputCloud(scn.raw[k]); pp.Process()
