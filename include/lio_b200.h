@@ -188,6 +188,24 @@ int lio_pm_process_dev(lio_pm *pm, const float *corner_dev, const float *surf_de
  * call, a second call or an lio_mb handle returns LIO_ERR_INVALID.  A publishing handle rejects lio_pm_process_host (it has no full
  * cloud) with LIO_ERR_INVALID.  Without it the handle behaves as before and the lio_mb_* accessors return LIO_ERR_INVALID. */
 int lio_pm_enable_publish(lio_pm *pm, float map_filter_size, int max_full_points);
+/* PointMapping::UpdateMapDatabase (:1112-1208) on its own, for a caller that keeps the estimator's loop and calls it where the
+ * reference's Estimator does (Estimator.cc:703-708): corner_ds / surf_ds (host, nc / ns float4 points <= max_points) are the
+ * down-sampled clouds in the sensor frame, tf7 the insert pose, valid (nv <= 125 distinct cube indices) the valid list as computed
+ * with the cube-array centre margin_centre3 (which may differ from the current one, lio_pm_map_centre).  Inserts every point into
+ * its cube in order, then VoxelGrids every valid cube that still lies in the array, corner cubes with corner_filter_size and surf
+ * cubes with surf_filter_size.  lio_pm_process_* and lio_mb_process_map_* run the same code.
+ * The insert waits for the device once, plus once for every cube segment it moves to a larger one; the re-filter is one segmented
+ * VoxelGrid with a launch count independent of the number of cubes, and its new cube sizes are read back without a wait in this
+ * call: the next call on the handle or lio_pm_cube_size / lio_pm_cube_download wait for them (one host wait, after the call).
+ * When a cube's voxel grid exceeded 2^24 voxels (a leaf below ~0.2 m for a full 50 m cube) that reader returns LIO_ERR_CAPACITY,
+ * and so does every later call that reads or updates the cubes: the map is invalid and the handle must be re-created.
+ * Bad arguments, an index outside [0, 4851) or a repeated index return LIO_ERR_INVALID, too many points or valid cubes
+ * LIO_ERR_CAPACITY, before anything changes.  The clouds are copied before the call returns. */
+int lio_pm_update_map_database_host(lio_pm *pm, const float *corner_ds, int nc, const float *surf_ds, int ns, const long long *valid, int nv,
+                                    const float tf7[7], const int margin_centre3[3]);
+/* The last UpdateMapDatabase on the handle (any entry): info4 = {cube jobs re-filtered, kernel launches, host waits, points inserted}.
+ * The waits include the one for the re-filtered sizes that the next reader of the cubes makes. */
+int lio_pm_update_stats(lio_pm *pm, int info4[4]);
 
 /* ---- lio::MapBuilder, the global 4-D mapper (src/map_builder/MapBuilder.cc, src/map_builder_node.cc) ---------------------
  * MapBuilder derives from PointMapping; here a map-builder context is an lio_pm handle created by lio_mb_create, so

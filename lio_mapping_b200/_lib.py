@@ -192,6 +192,9 @@ def lib():
     L.lio_po_clouds_dev.argtypes = [vp, C.POINTER(vp), C.POINTER(vp), i32p]
     L.lio_pm_process_dev.argtypes = [vp, vp, vp, vp, vp, i32p, f32p, f32p, f32p, i32p]
     L.lio_pm_enable_publish.argtypes = [vp, C.c_float, ip]
+    L.lio_pm_update_map_database_host.argtypes = [vp, f32p, ip, f32p, ip, np.ctypeslib.ndpointer(np.int64, flags="C_CONTIGUOUS"), ip,
+                                                  f32p, i32p]
+    L.lio_pm_update_stats.argtypes = [vp, i32p]
     _LIB = L
     return L
 

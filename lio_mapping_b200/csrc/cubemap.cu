@@ -6,7 +6,9 @@
 //   map extraction             :1005-1011    one gather kernel over the valid cubes' HBM segments
 //   Process                    :765-1052     PointAssociateToMap / TobeMapped kernels, VoxelGrid of the stacks,
 //                                            OptimizeTransformTobeMapped (scan_to_map_run: voxel-hash k-NN + 6 x 6 float GN)
-//   UpdateMapDatabase          :1112-1208    order-preserving insert into the cubes + VoxelGrid of every touched valid cube
+//   UpdateMapDatabase          :1112-1208    order-preserving insert (cube keys, stable sort and append positions on the device,
+//                                            one wait for the touched cubes) + one segmented VoxelGrid of every valid cube
+//                                            (voxel.cu SegVoxelGrid); also an entry of its own, lio_pm_update_map_database_host
 //   PublishResults             :1210-1270    after lio_pm_enable_publish: the map-builder mode's surround map (every 5th call) and
 //                                            registered full cloud, shared with PublishMapBuilderResults (pm_publish)
 // Host entries upload into the context's own buffers and run the same steps as the device entries (lio_pm_process_dev,
@@ -75,29 +77,61 @@ __device__ __forceinline__ int cube_of(float v, int cen) {
   return c;
 }
 
-// UpdateMapDatabase insert, phase 1: map-frame point and destination cube of every down-sampled stack point (-1: outside)
+// UpdateMapDatabase insert (:1123-1168).  The corner (n0 points) then surf cloud are one sequence; a point's key is its cloud's
+// cube array entry w * kCubes + cube, kInsOutside when it falls outside the array.  A stable sort by key then puts every cube's new
+// points together in push_back order.
+constexpr int kInsOutside = 2 * kCubes, kInsKeyBits = 14;   // 2 * 4851 < 2^14
+static_assert(kInsOutside < (1 << kInsKeyBits), "insert key bits");
+
+// phase 1: map-frame point and key of every point; n_ins[0] = n (the sort's count), n_ins[1] = 0 (phase 2's run counter)
 __global__ void __launch_bounds__(256)
-k_cube_ids(const float4 *__restrict__ in, const int *__restrict__ n_dev, TwistF t, int cen_l, int cen_w, int cen_h, float4 *__restrict__ mapped,
-           int *__restrict__ cube) {
-  const int n = *n_dev;
+k_ins_keys(const float4 *__restrict__ corner, const float4 *__restrict__ surf, int n0, int n, TwistF t, int cen_l, int cen_w, int cen_h,
+           float4 *__restrict__ mapped, unsigned *__restrict__ keys, unsigned *__restrict__ vals, int *__restrict__ n_ins) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i == 0) { n_ins[0] = n; n_ins[1] = 0; }
   if (i >= n) return;
-  const float4 p = __ldg(in + i);
+  const int w = i < n0 ? 0 : 1;
+  const float4 p = w == 0 ? __ldg(corner + i) : __ldg(surf + (i - n0));
   float x, y, z;
   rotate_dev(t.qx, t.qy, t.qz, t.qw, p.x, p.y, p.z, x, y, z);
   x += t.px; y += t.py; z += t.pz;
   mapped[i] = make_float4(x, y, z, p.w);
   const int ci = cube_of(x, cen_l), cj = cube_of(y, cen_w), ck = cube_of(z, cen_h);
-  cube[i] = (ci >= 0 && ci < kCubeL && cj >= 0 && cj < kCubeW && ck >= 0 && ck < kCubeH) ? ci + kCubeL * cj + kCubeL * kCubeW * ck : -1;
+  const bool in = ci >= 0 && ci < kCubeL && cj >= 0 && cj < kCubeW && ck >= 0 && ck < kCubeH;
+  keys[i] = in ? (unsigned)(w * kCubes + ci + kCubeL * cj + kCubeL * kCubeW * ck) : (unsigned)kInsOutside;
+  vals[i] = (unsigned)i;
 }
 
-// phase 2: dst[i] is the address the host directory assigned to point i (append position inside its cube, input order kept)
+struct InsRun { int key, n; };
+// phase 2: one run per touched cube, found at its last sorted point: the run goes to the host's pinned list (runs, mapped into
+// the device's address space) in slot order, its slot and first sorted position to slot_of / start_of
 __global__ void __launch_bounds__(256)
-k_scatter_to_cubes(const float4 *__restrict__ mapped, float4 *const *__restrict__ dst, int n) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  float4 *d = dst[i];
-  if (d) *d = __ldg(mapped + i);
+k_ins_runs(const unsigned *__restrict__ keys, const int *__restrict__ n_ins, int *__restrict__ nruns, InsRun *__restrict__ runs,
+           int *__restrict__ slot_of, int *__restrict__ start_of) {
+  const int n = n_ins[0];
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= n) return;
+  const unsigned k = keys[p];
+  if (k >= (unsigned)kInsOutside || (p + 1 < n && keys[p + 1] == k)) return;
+  int lo = 0, hi = p;   // first position of key k
+  while (lo < hi) { const int mid = (lo + hi) >> 1; if (keys[mid] < k) lo = mid + 1; else hi = mid; }
+  const int slot = atomicAdd(nruns, 1);
+  runs[slot] = InsRun{(int)k, p + 1 - lo};
+  slot_of[k] = slot;
+  start_of[k] = lo;
+}
+
+struct CubeEnd { float4 *p; int n; };   // a touched cube's segment and its count before the insert
+// phase 3: every point to its append position, its rank inside the run
+__global__ void __launch_bounds__(256)
+k_ins_scatter(const unsigned *__restrict__ keys, const unsigned *__restrict__ vals, const float4 *__restrict__ mapped, const int *__restrict__ n_ins,
+              const int *__restrict__ slot_of, const int *__restrict__ start_of, const CubeEnd *__restrict__ tab) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= n_ins[0]) return;
+  const unsigned k = keys[p];
+  if (k >= (unsigned)kInsOutside) return;
+  const CubeEnd c = tab[slot_of[k]];
+  c.p[c.n + p - start_of[k]] = __ldg(mapped + vals[p]);
 }
 
 // Input counts of one call {corner, surf, full}, read on the device and clamped to n_max: cnt[0], cnt[1], cnt[4]; cnt[7] = 1 when
@@ -149,24 +183,39 @@ struct lio_pm {
   double delta_r_abort = 0.05, delta_t_abort = 0.05;
   TwistF sum, bef, aft, tobe;          // transform_sum_, transform_bef_mapped_, transform_aft_mapped_, transform_tobe_mapped_
   // device scratch
-  float4 *d_in[2] = {nullptr, nullptr}, *d_stack[2] = {nullptr, nullptr}, *d_ds[2] = {nullptr, nullptr}, *d_mapped = nullptr, *d_tmp = nullptr;
+  float4 *d_in[2] = {nullptr, nullptr}, *d_stack[2] = {nullptr, nullptr}, *d_ds[2] = {nullptr, nullptr}, *d_mapped = nullptr;
   float4 *d_map[2] = {nullptr, nullptr};
   int map_cap[2] = {0, 0};
   int *d_cnt = nullptr;                // [0,1] input sizes, [2,3] down-sampled sizes, [4] full cloud, [5,6] surround map in / out,
                                        // [7] input count over its bound, [8..10] counts uploaded by the host entries
   int h_cnt[8] = {};                   // read-back of d_cnt[0..7] after the down-sampling
-  int *d_cube = nullptr;
-  float4 **d_dst = nullptr;
   Segment *d_seg = nullptr;
-  int *d_vgout = nullptr;              // per re-filtered cube: output count
   VoxelGrid vg;
-  int vg_cap = 0;
   ScanToMapWork stm;
   int stm_cap[3] = {0, 0, 0};
   int last_iters = 0, last_from_map[2] = {0, 0};
-  std::vector<int> h_cube;
-  std::vector<float4 *> h_dst;
-  bool started = false;                // a process call has run (lio_pm_enable_publish must come before it)
+  // UpdateMapDatabase (pm_update).  Insert: sort buffers for 2 * max_points keys, per-key slot / first position, the run list
+  // (pinned, written by the device), the touched cubes' table (pinned and its device copy).
+  unsigned *d_ins_k[2] = {nullptr, nullptr}, *d_ins_v[2] = {nullptr, nullptr};
+  RadixSortTemp ins_rs;
+  int *d_ins_n = nullptr;              // [0] points, [1] runs
+  int *d_slot_of = nullptr, *d_start_of = nullptr;
+  InsRun *h_runs = nullptr, *h_runs_dev = nullptr;
+  int *h_nruns = nullptr;
+  CubeEnd *h_tab = nullptr, *d_tab = nullptr;
+  cudaEvent_t ev_ins = nullptr;
+  // Re-filter: one segmented VoxelGrid over the jobs; their output counts arrive in h_jn (pinned) behind ev_counts and are applied
+  // to the directory by pm_counts before anything reads it.
+  SegVoxelGrid svg;
+  VgJob *h_jobs = nullptr;
+  int *h_jn = nullptr;
+  std::vector<std::pair<int, size_t>> pend_jobs;   // (cloud, cube) of every job whose count is in flight
+  bool counts_pending = false;
+  bool counts_broken = false;          // a job exceeded the 2^24-voxel bound: its cubes are wrong, every later reader fails
+  cudaEvent_t ev_counts = nullptr;
+  int upd_stats[4] = {0, 0, 0, 0};     // last UpdateMapDatabase: cube jobs, kernel launches, host waits (the later wait for the
+                                       // re-filtered counts included), points inserted
+  bool started = false;               // a process call has run (lio_pm_enable_publish must come before it)
   bool publish = false;                // lio_pm_enable_publish: PointMapping::PublishResults on every lio_pm_process_dev
   // map-builder mode (lio_mb_*: MapBuilder : PointMapping, src/map_builder/MapBuilder.cc)
   bool mb = false, enable_4d = true, system_init = false;
@@ -195,13 +244,17 @@ extern "C" int lio_pm_destroy(lio_pm *m) {
     void *fr[] = {m->d_in[w], m->d_stack[w], m->d_ds[w], m->d_map[w]};
     for (void *q : fr) if (q) cudaFree(q);
   }
-  void *fr[] = {m->d_mapped, m->d_tmp, m->d_cnt, m->d_cube, m->d_dst, m->d_seg, m->d_vgout, m->d_full_in, m->d_full_out, m->d_sur,
-                m->d_sur_ds, m->d_sur_seg};
+  void *fr[] = {m->d_mapped, m->d_cnt, m->d_seg, m->d_full_in, m->d_full_out, m->d_sur, m->d_sur_ds, m->d_sur_seg, m->d_ins_k[0],
+                m->d_ins_k[1], m->d_ins_v[0], m->d_ins_v[1], m->d_ins_n, m->d_slot_of, m->d_start_of, m->d_tab};
   for (void *q : fr) if (q) cudaFree(q);
-  if (m->h_sur_seg) cudaFreeHost(m->h_sur_seg);
-  if (m->h_sur_n) cudaFreeHost(m->h_sur_n);
+  void *frh[] = {m->h_sur_seg, m->h_sur_n, m->h_runs, m->h_nruns, m->h_tab, m->h_jobs, m->h_jn};
+  for (void *q : frh) if (q) cudaFreeHost(q);
+  if (m->ev_ins) cudaEventDestroy(m->ev_ins);
+  if (m->ev_counts) cudaEventDestroy(m->ev_counts);
   m->vg.destroy();
   m->vg_sur.destroy();
+  m->svg.destroy();
+  m->ins_rs.destroy();
   m->stm.destroy();
   delete m;
   return LIO_OK;
@@ -226,18 +279,29 @@ extern "C" int lio_pm_create(int max_points, float corner_filter_size, float sur
     ok = ok && cudaMalloc(&m->d_stack[w], sizeof(float4) * max_points) == cudaSuccess;
     ok = ok && cudaMalloc(&m->d_ds[w], sizeof(float4) * max_points) == cudaSuccess;
   }
-  ok = ok && cudaMalloc(&m->d_mapped, sizeof(float4) * max_points) == cudaSuccess;
+  ok = ok && cudaMalloc(&m->d_mapped, sizeof(float4) * 2 * max_points) == cudaSuccess;
   ok = ok && cudaMalloc(&m->d_cnt, sizeof(int) * 12) == cudaSuccess;
-  ok = ok && cudaMalloc(&m->d_cube, sizeof(int) * max_points) == cudaSuccess;
-  ok = ok && cudaMalloc(&m->d_dst, sizeof(float4 *) * max_points) == cudaSuccess;
   ok = ok && cudaMalloc(&m->d_seg, sizeof(Segment) * 256) == cudaSuccess;
-  ok = ok && cudaMalloc(&m->d_vgout, sizeof(int) * 256) == cudaSuccess;
-  m->vg_cap = max_points;
-  ok = ok && cudaMalloc(&m->d_tmp, sizeof(float4) * m->vg_cap) == cudaSuccess;
-  ok = ok && m->vg.init(m->vg_cap) == 0;
+  ok = ok && m->vg.init(max_points) == 0;
+  for (int b = 0; b < 2 && ok; ++b) {
+    ok = ok && cudaMalloc(&m->d_ins_k[b], sizeof(unsigned) * 2 * max_points) == cudaSuccess;
+    ok = ok && cudaMalloc(&m->d_ins_v[b], sizeof(unsigned) * 2 * max_points) == cudaSuccess;
+  }
+  ok = ok && m->ins_rs.init(2 * max_points) == 0;
+  ok = ok && cudaMalloc(&m->d_ins_n, sizeof(int) * 2) == cudaSuccess;
+  ok = ok && cudaMalloc(&m->d_slot_of, sizeof(int) * kInsOutside) == cudaSuccess;
+  ok = ok && cudaMalloc(&m->d_start_of, sizeof(int) * kInsOutside) == cudaSuccess;
+  ok = ok && cudaMalloc(&m->d_tab, sizeof(CubeEnd) * kInsOutside) == cudaSuccess;
+  ok = ok && cudaHostAlloc(&m->h_runs, sizeof(InsRun) * kInsOutside, cudaHostAllocMapped) == cudaSuccess;
+  ok = ok && cudaHostGetDevicePointer(&m->h_runs_dev, m->h_runs, 0) == cudaSuccess;
+  ok = ok && cudaMallocHost(&m->h_nruns, sizeof(int)) == cudaSuccess;
+  ok = ok && cudaMallocHost(&m->h_tab, sizeof(CubeEnd) * kInsOutside) == cudaSuccess;
+  ok = ok && m->svg.init() == 0;
+  ok = ok && cudaMallocHost(&m->h_jobs, sizeof(VgJob) * kVgMaxJobs) == cudaSuccess;
+  ok = ok && cudaMallocHost(&m->h_jn, sizeof(int) * (kVgMaxJobs + 1)) == cudaSuccess;
+  ok = ok && cudaEventCreateWithFlags(&m->ev_ins, cudaEventDisableTiming) == cudaSuccess;
+  ok = ok && cudaEventCreateWithFlags(&m->ev_counts, cudaEventDisableTiming) == cudaSuccess;
   if (!ok) { lio_set_last_error(__FILE__, __LINE__, "lio_pm_create: device allocation failed"); lio_pm_destroy(m); return LIO_ERR_CUDA; }
-  m->h_cube.resize(max_points);
-  m->h_dst.resize(max_points);
   *out = m;
   return LIO_OK;
 }
@@ -339,64 +403,98 @@ static int pm_from_map(lio_pm *m, const std::vector<size_t> &valid, int w, int &
   return LIO_OK;
 }
 
-// UpdateMapDatabase (:1112-1208) with margin centre == current centre (the valid list was computed in this call)
-static int pm_update(lio_pm *m, const std::vector<size_t> &valid, const int n_ds[2]) {
+// The re-filter's output counts of the last UpdateMapDatabase into the directory; every reader of the cube counts calls this first.
+// This is the update's one host wait after it returned (counted in its upd_stats).  Once a job has exceeded the 2^24-voxel bound
+// its cubes hold wrong centroids: the error is sticky, this and every later call return LIO_ERR_CAPACITY.
+static int pm_counts(lio_pm *m) {
+  if (m->counts_broken) {
+    lio_set_last_error(__FILE__, __LINE__, "UpdateMapDatabase: an earlier re-filter exceeded the 2^24-voxel bound; the cube map is invalid");
+    return LIO_ERR_CAPACITY;
+  }
+  if (!m->counts_pending) return LIO_OK;
+  m->counts_pending = false;
+  LIO_CUDA_OK(cudaEventSynchronize(m->ev_counts));
+  const int nj = (int)m->pend_jobs.size();
+  if (m->h_jn[nj]) {
+    m->counts_broken = true;
+    lio_set_last_error(__FILE__, __LINE__, "UpdateMapDatabase: a cube's voxel index range exceeds 2^24 (leaf too small for a 50 m cube)");
+    return LIO_ERR_CAPACITY;
+  }
+  for (int j = 0; j < nj; ++j) m->cube[m->pend_jobs[j].first][m->pend_jobs[j].second].n = m->h_jn[j];
+  return LIO_OK;
+}
+
+// UpdateMapDatabase (:1112-1208) of the n_ds[0] corner and n_ds[1] surf points in d_ds with the pose t; valid holds cube indices
+// of the margin centre mc (:1173-1183 move them to the current centre).  Insert: the keys, a stable sort by key and the run list
+// on the device; the host waits once for the runs to size the touched segments (and once per segment it moves to a larger one),
+// then uploads their {segment, count} table.  Re-filter: one segmented VoxelGrid over every non-empty valid cube, corner and surf,
+// whose output counts reach the directory through pm_counts without a wait here (the next reader waits; upd_stats counts that wait).
+static int pm_update(lio_pm *m, const std::vector<size_t> &valid, const int n_ds[2], const TwistF &t, const int mc[3]) {
   cudaStream_t st = m->stream;
-  for (int w = 0; w < 2; ++w) {
-    const int n = n_ds[w];
-    if (n == 0) continue;
-    k_cube_ids<<<(n + 255) / 256, 256, 0, st>>>(m->d_ds[w], m->d_cnt + 2 + w, m->tobe, m->cen_l, m->cen_w, m->cen_h, m->d_mapped, m->d_cube);
-    LIO_CUDA_OK(cudaMemcpyAsync(m->h_cube.data(), m->d_cube, sizeof(int) * n, cudaMemcpyDeviceToHost, st));
-    LIO_CUDA_OK(cudaStreamSynchronize(st));
-    // append positions in input order (push_back order): first the per-cube totals to size the segments, then the addresses
-    std::vector<int> add(kCubes, 0);
-    for (int i = 0; i < n; ++i) if (m->h_cube[i] >= 0) ++add[m->h_cube[i]];
-    for (int c = 0; c < kCubes; ++c)
-      if (add[c]) { int rc = pm_grow(m, m->cube[w][c], m->cube[w][c].n + add[c]); if (rc != LIO_OK) return rc; }
-    for (int i = 0; i < n; ++i) {
-      const int c = m->h_cube[i];
-      if (c < 0) { m->h_dst[i] = nullptr; continue; }
-      lio_pm::Cube &cb = m->cube[w][c];
-      m->h_dst[i] = cb.p + cb.n;
-      ++cb.n;
+  int rc = pm_counts(m);
+  if (rc != LIO_OK) return rc;
+  int launches = 0, waits = 0;
+  const int n = n_ds[0] + n_ds[1];
+  if (n > 0) {
+    const int blocks = (n + 255) / 256;
+    k_ins_keys<<<blocks, 256, 0, st>>>(m->d_ds[0], m->d_ds[1], n_ds[0], n, t, m->cen_l, m->cen_w, m->cen_h, m->d_mapped, m->d_ins_k[0],
+                                       m->d_ins_v[0], m->d_ins_n);
+    ++launches;
+    const int b = radix_sort_pairs(m->d_ins_k[0], m->d_ins_v[0], m->d_ins_k[1], m->d_ins_v[1], m->d_ins_n, n, kInsKeyBits, m->ins_rs, st, &launches);
+    if (b < 0) return LIO_ERR_CAPACITY;
+    k_ins_runs<<<blocks, 256, 0, st>>>(m->d_ins_k[b], m->d_ins_n, m->d_ins_n + 1, m->h_runs_dev, m->d_slot_of, m->d_start_of);
+    ++launches;
+    LIO_CUDA_OK(cudaMemcpyAsync(m->h_nruns, m->d_ins_n + 1, sizeof(int), cudaMemcpyDeviceToHost, st));
+    LIO_CUDA_OK(cudaEventRecord(m->ev_ins, st));
+    LIO_CUDA_OK(cudaEventSynchronize(m->ev_ins));
+    ++waits;
+    const int nr = *m->h_nruns;
+    for (int r = 0; r < nr; ++r) {
+      const InsRun run = m->h_runs[r];
+      lio_pm::Cube &c = m->cube[run.key / kCubes][run.key % kCubes];
+      if (c.n + run.n > c.cap && c.p) ++waits;
+      if ((rc = pm_grow(m, c, c.n + run.n)) != LIO_OK) return rc;
+      m->h_tab[r] = CubeEnd{c.p, c.n};
+      c.n += run.n;
     }
-    LIO_CUDA_OK(cudaMemcpyAsync(m->d_dst, m->h_dst.data(), sizeof(float4 *) * n, cudaMemcpyHostToDevice, st));
-    k_scatter_to_cubes<<<(n + 255) / 256, 256, 0, st>>>(m->d_mapped, m->d_dst, n);
-    LIO_CUDA_OK(cudaStreamSynchronize(st));   // h_dst is reused by the next cloud
+    if (nr > 0) {
+      LIO_CUDA_OK(cudaMemcpyAsync(m->d_tab, m->h_tab, sizeof(CubeEnd) * nr, cudaMemcpyHostToDevice, st));
+      k_ins_scatter<<<blocks, 256, 0, st>>>(m->d_ins_k[b], m->d_ins_v[b], m->d_mapped, m->d_ins_n, m->d_slot_of, m->d_start_of, m->d_tab);
+      ++launches;
+    }
   }
   // re-filter every valid cube (corner then surf), each with its own bounding box like pcl::VoxelGrid on that cube's cloud
-  struct Job { int w; size_t idx; };
-  std::vector<Job> jobs;
+  m->pend_jobs.clear();
+  int total = 0;
   for (size_t index : valid) {
     int li, lj, lk;
     { int residual = (int)(index % (kCubeL * kCubeW)); lk = (int)(index / (kCubeL * kCubeW)); lj = residual / kCubeL; li = residual % kCubeL; }
-    const float center_x = 50.0f * (li - m->cen_l), center_y = 50.0f * (lj - m->cen_w), center_z = 50.0f * (lk - m->cen_h);
+    const float center_x = 50.0f * (li - mc[0]), center_y = 50.0f * (lj - mc[1]), center_z = 50.0f * (lk - mc[2]);
     const int ci = cube_of_host(center_x, m->cen_l), cj = cube_of_host(center_y, m->cen_w), ck = cube_of_host(center_z, m->cen_h);
     if (!(ci >= 0 && ci < kCubeL && cj >= 0 && cj < kCubeW && ck >= 0 && ck < kCubeH)) continue;
     const size_t idx = to_index(ci, cj, ck);
-    for (int w = 0; w < 2; ++w) if (m->cube[w][idx].n > 0) jobs.push_back(Job{w, idx});
-  }
-  for (size_t b0 = 0; b0 < jobs.size(); b0 += 256) {
-    const size_t b1 = std::min(jobs.size(), b0 + 256);
-    std::vector<int> hn(b1 - b0);
-    for (size_t j = b0; j < b1; ++j) {
-      lio_pm::Cube &c = m->cube[jobs[j].w][jobs[j].idx];
-      if (c.n > m->vg_cap) return LIO_ERR_CAPACITY;
-      // input count through d_vgout[j] itself (read before the filter overwrites it with the output count)
-      hn[j - b0] = c.n;
+    for (int w = 0; w < 2; ++w) {
+      const lio_pm::Cube &c = m->cube[w][idx];
+      if (c.n == 0) continue;
+      if ((int)m->pend_jobs.size() == kVgMaxJobs || c.n > INT_MAX / 2 - total) {
+        m->pend_jobs.clear();
+        lio_set_last_error(__FILE__, __LINE__, "UpdateMapDatabase: more than 256 cube jobs");
+        return LIO_ERR_CAPACITY;
+      }
+      m->h_jobs[m->pend_jobs.size()] = VgJob{c.p, c.n, total, m->leaf[w]};
+      m->pend_jobs.emplace_back(w, idx);
+      total += c.n;
     }
-    LIO_CUDA_OK(cudaMemcpyAsync(m->d_vgout, hn.data(), sizeof(int) * hn.size(), cudaMemcpyHostToDevice, st));
-    LIO_CUDA_OK(cudaStreamSynchronize(st));
-    for (size_t j = b0; j < b1; ++j) {
-      lio_pm::Cube &c = m->cube[jobs[j].w][jobs[j].idx];
-      int rc = m->vg.run(c.p, m->d_vgout + (j - b0), c.n, m->leaf[jobs[j].w], m->d_tmp, m->vg_cap, m->d_vgout + (j - b0), nullptr, st, nullptr);
-      if (rc != LIO_OK) return rc;
-      LIO_CUDA_OK(cudaMemcpyAsync(c.p, m->d_tmp, sizeof(float4) * c.n, cudaMemcpyDeviceToDevice, st));   // output <= input count
-    }
-    LIO_CUDA_OK(cudaMemcpyAsync(hn.data(), m->d_vgout, sizeof(int) * hn.size(), cudaMemcpyDeviceToHost, st));
-    LIO_CUDA_OK(cudaStreamSynchronize(st));
-    for (size_t j = b0; j < b1; ++j) m->cube[jobs[j].w][jobs[j].idx].n = hn[j - b0];
   }
+  const int nj = (int)m->pend_jobs.size();
+  if (nj > 0) {
+    if (m->svg.reserve(total) != 0) { m->pend_jobs.clear(); lio_set_last_error(__FILE__, __LINE__, "UpdateMapDatabase: workspace allocation failed"); return LIO_ERR_CUDA; }
+    if ((rc = m->svg.run(m->h_jobs, nj, total, m->h_jn, st, &launches)) != LIO_OK) { m->pend_jobs.clear(); return rc; }
+    LIO_CUDA_OK(cudaEventRecord(m->ev_counts, st));
+    m->counts_pending = true;
+    ++waits;   // pm_counts, at the next call or cube accessor (or in this call's surround publication)
+  }
+  m->upd_stats[0] = nj; m->upd_stats[1] = launches; m->upd_stats[2] = waits; m->upd_stats[3] = n;
   return LIO_OK;
 }
 
@@ -512,10 +610,11 @@ static int pm_process(lio_pm *m, const float4 *const src[2], const float4 *full,
                       float transform_tobe_mapped7[7], float transform_aft_mapped7[7], int *info, int n_info) {
   const int nin[2] = {n_max[0], n_max[1]};
   m->started = true;
+  int rc = pm_counts(m);
+  if (rc != LIO_OK) return rc;
   m->sum = tf7_to_twist(transform_sum7);
   m->tobe = twist_mul(m->tobe, twist_mul(twist_inverse(m->bef), m->sum));   // TransformAssociateToMap :753-756
-  int rc = pm_stack(m, src, full, n3_dev, n_max);
-  if (rc != LIO_OK) return rc;
+  if ((rc = pm_stack(m, src, full, n3_dev, n_max)) != LIO_OK) return rc;
   std::vector<size_t> valid, surround;
   int K[2] = {0, 0}, n_ds[2] = {0, 0};
   if ((rc = pm_locate(m, valid, m->publish ? &surround : nullptr, K)) != LIO_OK) return rc;
@@ -524,7 +623,8 @@ static int pm_process(lio_pm *m, const float4 *const src[2], const float4 *full,
   m->last_iters = 0;
   if (optimised && (rc = pm_optimise(m, K, n_ds, 0)) != LIO_OK) return rc;
   if (optimised) { m->bef = m->sum; m->aft = m->tobe; }   // TransformUpdate sits behind the optimiser's early return (:327-329, :716)
-  if ((rc = pm_update(m, valid, n_ds)) != LIO_OK) return rc;
+  const int cen[3] = {m->cen_l, m->cen_w, m->cen_h};   // margin centre == current centre: the valid list is this call's
+  if ((rc = pm_update(m, valid, n_ds, m->tobe, cen)) != LIO_OK) return rc;
   bool published = false;
   if (m->publish && (rc = pm_publish(m, surround, n_max[2] > 0 ? m->h_cnt[4] : 0, published)) != LIO_OK) return rc;
   if (transform_tobe_mapped7) twist_to_tf7(m->tobe, transform_tobe_mapped7);
@@ -563,6 +663,30 @@ extern "C" int lio_pm_process_dev(lio_pm *m, const float *corner_dev, const floa
                     transform_aft_mapped7, info5, 5);
 }
 
+extern "C" int lio_pm_update_map_database_host(lio_pm *m, const float *corner_ds, int nc, const float *surf_ds, int ns, const long long *valid,
+                                               int nv, const float tf7[7], const int margin_centre3[3]) {
+  if (!m || !tf7 || !margin_centre3 || nc < 0 || ns < 0 || nv < 0 || (nc > 0 && !corner_ds) || (ns > 0 && !surf_ds) || (nv > 0 && !valid))
+    return LIO_ERR_INVALID;
+  if (nc > m->max_points || ns > m->max_points || nv > 125) return LIO_ERR_CAPACITY;
+  std::vector<size_t> v(valid, valid + nv);
+  for (int i = 0; i < nv; ++i) {
+    if (valid[i] < 0 || valid[i] >= kCubes) return LIO_ERR_INVALID;
+    for (int k = 0; k < i; ++k) if (valid[k] == valid[i]) return LIO_ERR_INVALID;
+  }
+  LIO_CUDA_OK(cudaSetDevice(m->device));
+  cudaStream_t st = m->stream;
+  if (nc > 0) LIO_CUDA_OK(cudaMemcpyAsync(m->d_ds[0], corner_ds, sizeof(float4) * nc, cudaMemcpyHostToDevice, st));
+  if (ns > 0) LIO_CUDA_OK(cudaMemcpyAsync(m->d_ds[1], surf_ds, sizeof(float4) * ns, cudaMemcpyHostToDevice, st));
+  const int n_ds[2] = {nc, ns};
+  return pm_update(m, v, n_ds, tf7_to_twist(tf7), margin_centre3);
+}
+
+extern "C" int lio_pm_update_stats(lio_pm *m, int info4[4]) {
+  if (!m || !info4) return LIO_ERR_INVALID;
+  for (int k = 0; k < 4; ++k) info4[k] = m->upd_stats[k];
+  return LIO_OK;
+}
+
 // ---- lio::MapBuilder (src/map_builder/MapBuilder.cc) -----------------------------------------------------------------------
 static void mat3_mul(const float A[9], const float B[9], float C[9]) {   // Eigen's 3 x 3 float product, sum in k order
   for (int i = 0; i < 3; ++i)
@@ -599,6 +723,8 @@ static TwistF transform_4d_associate(const TwistF &tobe, const TwistF &bef, cons
 // down_size_filter_map_ over the whole cloud (:166-168).  Buffers grow on demand; the count stays on the device in d_cnt[6].
 static int mb_surround(lio_pm *m, const std::vector<size_t> &surround) {
   cudaStream_t st = m->stream;
+  int rc = pm_counts(m);
+  if (rc != LIO_OK) return rc;
   int nseg = 0, total = 0;
   for (size_t v : surround)
     for (int w = 0; w < 2; ++w) {
@@ -682,12 +808,13 @@ extern "C" int lio_pm_enable_publish(lio_pm *m, float map_filter_size, int max_f
 static int mb_process_map(lio_pm *m, const float4 *const src[2], const float4 *full, const int *n3_dev, const int n_max[3],
                           const float transform_sum7[7], float transform_tobe_mapped7[7], float transform_aft_mapped7[7], int info6[6]) {
   const int nin[2] = {n_max[0], n_max[1]};
+  int rc = pm_counts(m);
+  if (rc != LIO_OK) return rc;
   m->sum = tf7_to_twist(transform_sum7);
   if (!m->system_init) { m->system_init = true; m->bef = m->sum; m->tobe = m->sum; m->aft = m->tobe; }   // :227-232
   if (m->enable_4d) m->tobe = transform_4d_associate(m->tobe, m->bef, m->sum);
   else m->tobe = twist_mul(m->tobe, twist_mul(twist_inverse(m->bef), m->sum));   // TransformAssociateToMap (PointMapping.cc:755-758)
-  int rc = pm_stack(m, src, full, n3_dev, n_max);
-  if (rc != LIO_OK) return rc;
+  if ((rc = pm_stack(m, src, full, n3_dev, n_max)) != LIO_OK) return rc;
   std::vector<size_t> valid, surround;
   int K[2] = {0, 0}, n_ds[2] = {0, 0};
   if ((rc = pm_locate(m, valid, &surround, K)) != LIO_OK) return rc;
@@ -705,7 +832,8 @@ static int mb_process_map(lio_pm *m, const float4 *const src[2], const float4 *f
     m->bef = m->sum; m->aft = m->tobe;
   }
   ++m->odom_count;
-  if ((rc = pm_update(m, valid, n_ds)) != LIO_OK) return rc;
+  const int cen[3] = {m->cen_l, m->cen_w, m->cen_h};   // margin centre == current centre: the valid list is this call's
+  if ((rc = pm_update(m, valid, n_ds, m->tobe, cen)) != LIO_OK) return rc;
   // PublishMapBuilderResults: surround map every num_map_frames_ (5) frames, registered full cloud every frame
   bool publish = false;
   if ((rc = pm_publish(m, surround, nf, publish)) != LIO_OK) return rc;
@@ -783,15 +911,20 @@ extern "C" int lio_pm_map_centre(lio_pm *m, int centre3[3]) {
 
 extern "C" int lio_pm_cube_size(lio_pm *m, int cube_index, int which, int *n) {
   if (!m || !n || cube_index < 0 || cube_index >= kCubes || which < 0 || which > 1) return LIO_ERR_INVALID;
+  LIO_CUDA_OK(cudaSetDevice(m->device));
+  int rc = pm_counts(m);
+  if (rc != LIO_OK) return rc;
   *n = m->cube[which][cube_index].n;
   return LIO_OK;
 }
 
 extern "C" int lio_pm_cube_download(lio_pm *m, int cube_index, int which, float *out_xyzi, int cap) {
   if (!m || !out_xyzi || cube_index < 0 || cube_index >= kCubes || which < 0 || which > 1) return LIO_ERR_INVALID;
+  LIO_CUDA_OK(cudaSetDevice(m->device));
+  int rc = pm_counts(m);
+  if (rc != LIO_OK) return rc;
   const lio_pm::Cube &c = m->cube[which][cube_index];
   if (c.n > cap) return LIO_ERR_CAPACITY;
-  LIO_CUDA_OK(cudaSetDevice(m->device));
   if (c.n > 0) LIO_CUDA_OK(cudaMemcpyAsync(out_xyzi, c.p, sizeof(float4) * c.n, cudaMemcpyDeviceToHost, m->stream));
   LIO_CUDA_OK(cudaStreamSynchronize(m->stream));
   return LIO_OK;

@@ -8,6 +8,9 @@
 //   radix sort: stable, 4 x 8-bit passes (sort.cu)
 //   vg_emit   : heads of equal-key runs -> ordered compaction by decoupled look-back, one centroid
 //               per occupied voxel
+//
+// SegVoxelGrid runs the same steps over many clouds at once (UpdateMapDatabase's re-filter of the valid cubes).
+#include <algorithm>
 #include "voxel.cuh"
 
 namespace lio {
@@ -178,6 +181,170 @@ int VoxelGrid::run(const float4 *in, const int *n_dev_in, int n_max, float leaf,
   if (launches) *launches += 1;
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) { lio_set_last_error(__FILE__, __LINE__, cudaGetErrorString(e)); return LIO_ERR_CUDA; }
+  return LIO_OK;
+}
+
+// ---- segmented VoxelGrid ------------------------------------------------------------------------------------------------
+// The kernels repeat vg_bbox / vg_keys / vg_emit per job, in the same float expressions.
+__global__ void vg_seg_reset(unsigned *__restrict__ jbbox, int njobs, int total, int *__restrict__ ticket) {
+  for (int t = threadIdx.x; t < 6 * njobs; t += blockDim.x) jbbox[t] = (t % 6 < 3) ? 0xffffffffu : 0u;
+  if (threadIdx.x == 0) { ticket[0] = 0; ticket[1] = 0; ticket[2] = total; }
+}
+
+// concatenation of the jobs (blockIdx.y = job), the job id of every point (into the key buffer) and every job's bounding box
+__global__ void __launch_bounds__(256)
+vg_seg_gather(const VgJob *__restrict__ jobs, float4 *__restrict__ cat, unsigned *__restrict__ job_of, unsigned *__restrict__ jbbox) {
+  const int j = blockIdx.y;
+  const VgJob jb = jobs[j];
+  float mn0 = INFINITY, mn1 = INFINITY, mn2 = INFINITY, mx0 = -INFINITY, mx1 = -INFINITY, mx2 = -INFINITY;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < jb.n; i += gridDim.x * blockDim.x) {
+    const float4 p = jb.p[i];
+    cat[jb.off + i] = p;
+    job_of[jb.off + i] = (unsigned)j;
+    mn0 = fminf(mn0, p.x); mn1 = fminf(mn1, p.y); mn2 = fminf(mn2, p.z);
+    mx0 = fmaxf(mx0, p.x); mx1 = fmaxf(mx1, p.y); mx2 = fmaxf(mx2, p.z);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    mn0 = fminf(mn0, __shfl_xor_sync(0xffffffffu, mn0, o)); mn1 = fminf(mn1, __shfl_xor_sync(0xffffffffu, mn1, o));
+    mn2 = fminf(mn2, __shfl_xor_sync(0xffffffffu, mn2, o)); mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, o));
+    mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, o)); mx2 = fmaxf(mx2, __shfl_xor_sync(0xffffffffu, mx2, o));
+  }
+  __shared__ float sm[256 / 32][6];
+  if (lane_id() == 0) { float *r = sm[warp_id()]; r[0] = mn0; r[1] = mn1; r[2] = mn2; r[3] = mx0; r[4] = mx1; r[5] = mx2; }
+  __syncthreads();
+  if (threadIdx.x < 6) {
+    const bool is_min = threadIdx.x < 3;
+    float v = sm[0][threadIdx.x];
+#pragma unroll
+    for (int w = 1; w < 256 / 32; ++w) v = is_min ? fminf(v, sm[w][threadIdx.x]) : fmaxf(v, sm[w][threadIdx.x]);
+    if (is_min) { if (v != INFINITY) atomicMin(jbbox + 6 * j + threadIdx.x, f2ord(v)); }
+    else { if (v != -INFINITY) atomicMax(jbbox + 6 * j + threadIdx.x, f2ord(v)); }
+  }
+}
+
+// key = (job << 24) | PCL voxel index inside the job's own grid, value = position in the concatenation.  keys holds the job ids on
+// entry.  A job whose grid has more than 2^24 voxels raises the error flag (below that bound PCL's INT_MAX check cannot fire).
+__global__ void __launch_bounds__(256)
+vg_seg_keys(const float4 *__restrict__ cat, const int *__restrict__ n_dev, const VgJob *__restrict__ jobs, const unsigned *__restrict__ jbbox,
+            unsigned *__restrict__ keys, unsigned *__restrict__ vals, int *__restrict__ err) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= *n_dev) return;
+  const unsigned j = keys[i];
+  const float inv = 1.0f / jobs[j].leaf;
+  float a[6];
+  for (int q = 0; q < 6; ++q) a[q] = ord2f(jbbox[6 * j + q]);
+  const int mb0 = (int)floorf(a[0] * inv), mb1 = (int)floorf(a[1] * inv), mb2 = (int)floorf(a[2] * inv);
+  const int xb0 = (int)floorf(a[3] * inv), xb1 = (int)floorf(a[4] * inv), xb2 = (int)floorf(a[5] * inv);
+  const long long d0 = (long long)xb0 - mb0 + 1, d1 = (long long)xb1 - mb1 + 1, d2 = (long long)xb2 - mb2 + 1;
+  if (d0 * d1 * d2 > (1LL << kVgJobBits)) *err = 1;
+  const int s3 = (int)d0, s4 = (int)(d0 * d1);
+  const float4 p = __ldg(cat + i);
+  const int ijk0 = (int)(floorf(p.x * inv) - (float)mb0);
+  const int ijk1 = (int)(floorf(p.y * inv) - (float)mb1);
+  const int ijk2 = (int)(floorf(p.z * inv) - (float)mb2);
+  keys[i] = (j << kVgJobBits) | ((unsigned)(ijk0 + ijk1 * s3 + ijk2 * s4) & ((1u << kVgJobBits) - 1u));
+  vals[i] = (unsigned)i;
+}
+
+// vg_emit over the sorted concatenation; the first centroid of every job records where the job's output starts
+__global__ void __launch_bounds__(kEmitThreads)
+vg_seg_emit(const float4 *__restrict__ in, const int *__restrict__ n_dev, const unsigned *__restrict__ keys, const unsigned *__restrict__ vals,
+            float4 *__restrict__ out, int njobs, int *__restrict__ jstart, unsigned long long *__restrict__ status, int *__restrict__ ticket) {
+  __shared__ int sscan[40];
+  __shared__ int stile, sbc;
+  const int n = *n_dev;
+  const int ntiles = (n + kEmitThreads - 1) / kEmitThreads;
+  if (threadIdx.x == 0) stile = atomicAdd(ticket, 1);
+  __syncthreads();
+  const int tile = stile;
+  if (tile >= ntiles) return;
+  const int c = tile * kEmitThreads + threadIdx.x;
+  int head = 0;
+  unsigned v = 0;
+  if (c < n) {
+    v = keys[c];
+    head = (c == 0) || (v != keys[c - 1]);
+  }
+  int tot;
+  const int lpos = block_scan_excl(head, sscan, &tot);
+  const int excl = lookback_exclusive(status, tile, tot, &sbc);
+  if (head) {
+    float ax = 0.f, ay = 0.f, az = 0.f, ai = 0.f;
+    int cnt = 0;
+    for (int c2 = c; c2 < n && keys[c2] == v; ++c2) {
+      float4 p = __ldg(in + vals[c2]);
+      ax += p.x; ay += p.y; az += p.z; ai += p.w;
+      ++cnt;
+    }
+    float fn = (float)cnt;
+    out[excl + lpos] = make_float4(ax / fn, ay / fn, az / fn, ai / fn);
+    if (c == 0 || (keys[c - 1] >> kVgJobBits) != (v >> kVgJobBits)) jstart[v >> kVgJobBits] = excl + lpos;
+  }
+  if (tile == ntiles - 1 && threadIdx.x == 0) jstart[njobs] = excl + tot;
+}
+
+// every job's centroids back over its own input (blockIdx.y = job), its output count, and the error flag after the last job
+__global__ void __launch_bounds__(256)
+vg_seg_scatter(const VgJob *__restrict__ jobs, int njobs, const float4 *__restrict__ out, const int *__restrict__ jstart,
+               const int *__restrict__ ticket, int *__restrict__ jn) {
+  const int j = blockIdx.y;
+  const int s = jstart[j], e = jstart[j + 1];
+  float4 *dst = jobs[j].p;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < e - s; i += gridDim.x * blockDim.x) dst[i] = out[s + i];
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    jn[j] = e - s;
+    if (j == 0) jn[njobs] = ticket[1];
+  }
+}
+
+int SegVoxelGrid::init() {
+  if (cudaMalloc(&d_jobs, sizeof(VgJob) * kVgMaxJobs) != cudaSuccess) return -1;
+  if (cudaMalloc(&jbbox, sizeof(unsigned) * 6 * kVgMaxJobs) != cudaSuccess) return -1;
+  if (cudaMalloc(&jstart, sizeof(int) * (kVgMaxJobs + 1)) != cudaSuccess) return -1;
+  if (cudaMalloc(&jn, sizeof(int) * (kVgMaxJobs + 1)) != cudaSuccess) return -1;
+  return 0;
+}
+
+int SegVoxelGrid::reserve(int total) {
+  if (total <= cap) return 0;
+  ws.destroy();
+  if (cat) cudaFree(cat);
+  if (out) cudaFree(out);
+  cat = out = nullptr;
+  cap = 0;
+  const int c = std::max(2 * total, 1 << 16);
+  if (ws.init(c) != 0 || cudaMalloc(&cat, sizeof(float4) * c) != cudaSuccess || cudaMalloc(&out, sizeof(float4) * c) != cudaSuccess) return -1;
+  cap = c;
+  return 0;
+}
+
+void SegVoxelGrid::destroy() {
+  ws.destroy();
+  void *p[] = {cat, out, d_jobs, jbbox, jstart, jn};
+  for (void *q : p) if (q) cudaFree(q);
+  cat = out = nullptr; d_jobs = nullptr; jbbox = nullptr; jstart = jn = nullptr;
+  cap = 0;
+}
+
+int SegVoxelGrid::run(const VgJob *h_jobs, int njobs, int total, int *h_jn, cudaStream_t st, int *launches) {
+  if (njobs < 1 || njobs > kVgMaxJobs || total < 1 || total > cap) return LIO_ERR_CAPACITY;
+  LIO_CUDA_OK(cudaMemcpyAsync(d_jobs, h_jobs, sizeof(VgJob) * njobs, cudaMemcpyHostToDevice, st));
+  int *n_dev = ws.ticket + 2;
+  vg_seg_reset<<<1, 256, 0, st>>>(jbbox, njobs, total, ws.ticket);
+  vg_seg_gather<<<dim3(16, (unsigned)njobs), 256, 0, st>>>(d_jobs, cat, ws.keys_a, jbbox);
+  vg_seg_keys<<<(total + 255) / 256, 256, 0, st>>>(cat, n_dev, d_jobs, jbbox, ws.keys_a, ws.vals_a, ws.ticket + 1);
+  if (launches) *launches += 3;
+  const int which = radix_sort_pairs(ws.keys_a, ws.vals_a, ws.keys_b, ws.vals_b, n_dev, total, 32, ws.rs, st, launches);
+  if (which < 0) return LIO_ERR_CAPACITY;
+  const unsigned *k = which ? ws.keys_b : ws.keys_a, *v = which ? ws.vals_b : ws.vals_a;
+  const int etiles = (total + kEmitThreads - 1) / kEmitThreads;
+  LIO_CUDA_OK(cudaMemsetAsync(ws.status, 0, sizeof(unsigned long long) * (size_t)(etiles + 1), st));
+  vg_seg_emit<<<etiles, kEmitThreads, 0, st>>>(cat, n_dev, k, v, out, njobs, jstart, ws.status, ws.ticket);
+  vg_seg_scatter<<<dim3(16, (unsigned)njobs), 256, 0, st>>>(d_jobs, njobs, out, jstart, ws.ticket, jn);
+  if (launches) *launches += 2;
+  LIO_CUDA_OK(cudaMemcpyAsync(h_jn, jn, sizeof(int) * (njobs + 1), cudaMemcpyDeviceToHost, st));
+  LIO_CUDA_OK(cudaGetLastError());
   return LIO_OK;
 }
 

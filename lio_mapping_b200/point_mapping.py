@@ -60,6 +60,25 @@ class PointMapping:
         return tobe, aft, dict(iterations=int(info[0]), corner_from_map=int(info[1]), surf_from_map=int(info[2]),
                                surround_published=bool(info[3]), surround_size=int(info[4]))
 
+    def UpdateMapDatabase(self, corner_ds, surf_ds, valid, tf7, margin_centre):
+        """PointMapping::UpdateMapDatabase (PointMapping.cc:1112-1208) on its own: insert the down-sampled sensor-frame clouds with the
+        pose tf7, then VoxelGrid the valid cubes (indices computed with the cube-array centre margin_centre).  Returns the update's
+        statistics: cube jobs re-filtered, kernel launches, host waits, points inserted."""
+        c = np.ascontiguousarray(corner_ds, np.float32).reshape(-1, 4); s = np.ascontiguousarray(surf_ds, np.float32).reshape(-1, 4)
+        v = np.ascontiguousarray(valid, np.int64).reshape(-1)
+        _lib.check(_lib.lib().lio_pm_update_map_database_host(self.h, c if c.shape[0] else np.zeros((1, 4), np.float32), c.shape[0],
+                                                              s if s.shape[0] else np.zeros((1, 4), np.float32), s.shape[0],
+                                                              v if v.shape[0] else np.zeros(1, np.int64), v.shape[0],
+                                                              np.ascontiguousarray(tf7, np.float32),
+                                                              np.ascontiguousarray(margin_centre, np.int32)), "lio_pm_update_map_database_host")
+        return self.update_stats()
+
+    def update_stats(self):
+        """The last UpdateMapDatabase of this mapper (from any entry): jobs, launches, waits, points."""
+        out = np.zeros(4, np.int32)
+        _lib.check(_lib.lib().lio_pm_update_stats(self.h, out), "lio_pm_update_stats")
+        return dict(jobs=int(out[0]), launches=int(out[1]), waits=int(out[2]), points=int(out[3]))
+
     def centre(self):
         out = np.zeros(3, np.int32)
         _lib.check(_lib.lib().lio_pm_map_centre(self.h, out), "lio_pm_map_centre")
