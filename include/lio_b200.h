@@ -157,6 +157,9 @@ int lio_pm_destroy(lio_pm *pm);
 int lio_pm_process_host(lio_pm *pm, const float *corner_last, int nc, const float *surf_last, int ns, const float transform_sum7[7],
                         float transform_tobe_mapped7[7], int info3[3]);
 int lio_pm_map_centre(lio_pm *pm, int centre3[3]);                 /* laser_cloud_cen_length_ / width_ / height_ */
+/* laser_cloud_valid_idx_ and laser_cloud_surround_idx_ (the latter on publishing and map-builder handles) of the last process call,
+ * n2 = their counts (<= 125 each); valid / surround may be NULL.  An attached map keeps them frozen (lio_est_attach_map). */
+int lio_pm_cube_lists(lio_pm *pm, long long valid[125], long long surround[125], int n2[2]);
 int lio_pm_cube_size(lio_pm *pm, int cube_index, int which, int *n);  /* which: 0 corner, 1 surf */
 int lio_pm_cube_download(lio_pm *pm, int cube_index, int which, float *out_xyzi, int cap);
 /* lio_pm_process_host with the clouds already in HBM, e.g. the odometry's published clouds (lio_po_clouds_dev): corner_dev / surf_dev
@@ -520,6 +523,39 @@ int lio_est_local_clouds_download(lio_est *est, int which, float *out, int cap, 
  * transform_lb = transform_lb_.cast<double>(), rounded to float as the map builder's LaserOdometryHandler keeps it
  * (PointMapping.cc:267-282): tf7 = {qx,qy,qz,qw,px,py,pz}.  Works with or without local clouds. */
 int lio_est_local_laser_odom(lio_est *est, float tf7[7]);
+/* The global cube map after initialisation.  The reference's Estimator is a PointMapping: on every INITED scan it predicts
+ * transform_tobe_mapped_ (ProcessCompactData, Estimator.cc:776-809), inserts the oldest optimised frame into the cube map
+ * (UpdateMapDatabase, :703-708) and publishes (PublishResults, :721; PointMapping.cc:1210-1270).  PointMapping::Process is not run
+ * (:810-812), so the cube centre, the valid and surround cube lists and transform_aft_mapped_ stay at their pre-initialisation values.
+ *   lio_est_attach_map   hands the pre-initialisation map to the estimator: pm is a publishing PointMapping (lio_pm_enable_publish,
+ *                        not lio_mb_create) on the estimator's device that has run at least one process call.  Call it after
+ *                        lio_est_finish_init and before the first scan.  The estimator needs local clouds (the corner and full
+ *                        clouds come from there), imu_factor = 1 and no sharding; the map's corner / surf leaf sizes must equal
+ *                        corner_filter_size / surf_filter_size (the same members in the reference).  Any violation, a second attach
+ *                        or an attach after the first scan returns LIO_ERR_INVALID before anything changes; a map whose
+ *                        max_full_points is below the estimator's max_full_points returns LIO_ERR_CAPACITY.  An accumulated surf slot
+ *                        holds up to max_frame_points * (W - O + 1) points: the map's insert buffers grow to that at attach.
+ *                        While attached, lio_pm_process_*, lio_pm_update_map_database_host and lio_pm_destroy on pm return
+ *                        LIO_ERR_INVALID; the cube accessors, lio_pm_map_centre, lio_pm_update_stats and lio_mb_surround_* /
+ *                        lio_mb_full_* keep working and show the estimator's map.  lio_est_destroy releases the attachment.
+ *   per scan             at the scan entry tobe = tobe * lb * (prev^-1 * curr) * lb^-1 in float Twist, prev / curr the float casts
+ *                        of the states W - 1 and W (lb = transform_lb_).  After the solve, from the (O+1)-th scan on (the warm-start
+ *                        frames count as mapped), UpdateMapDatabase of the clouds opt_corner_stack_ / opt_surf_stack_.first() alias:
+ *                        with enable_deskew or cutoff_deskew the previous frame's (window frame W - O - 1, or the frame that has just
+ *                        left the window when W == O), otherwise frame W - O's; the surf cloud as SlideWindow has accumulated it, the
+ *                        corner cloud as pushed.  Pose: opt_transforms_[0] (:2279-2286), Quaterniond(Rs_[W-O] *
+ *                        transform_lb.rot.conjugate().normalized()), Ps_[W-O] - rot * transform_lb.pos, cast to float.  Then the
+ *                        surround map (every 5th call, counting on from the pre-initialisation calls) and /cloud_registered (the
+ *                        scan's raw staged full cloud through PointAssociateToMap with the predicted tobe).  The work runs on pm's
+ *                        stream, after the solve, ordered by events; the next scan entry and the next lio_est_set_scan_clouds_* wait
+ *                        for it.  /cloud_registered reads the staged full cloud when the scan closes, so with a map attached
+ *                        lio_est_set_scan_clouds_* inside an open scan (stepwise API) returns LIO_ERR_INVALID (not poisoning).  A failed map step poisons the estimator like any failed scan.
+ *   lio_est_map_poses    after lio_est_process_scan_* / lio_est_close_scan: tobe7 = transform_tobe_mapped_, aft7 = the frozen
+ *                        transform_aft_mapped_ (/aft_mapped_to_init), insert7 = the pose of the last insert, info4 = {inserted this
+ *                        scan, points inserted, surround published this scan, size of the last surround map}; any pointer may be NULL.
+ *                        LIO_ERR_INVALID without an attached map. */
+int lio_est_attach_map(lio_est *est, lio_pm *pm);
+int lio_est_map_poses(lio_est *est, float tobe7[7], float aft7[7], float insert7[7], int info4[4]);
 /* window states: (W+1) x 16 doubles (layout of state16) */
 int lio_est_get_states(lio_est *est, double *out);
 /* summary[32]: see lio_mapping_b200/estimator.py SUMMARY_KEYS */

@@ -103,6 +103,8 @@ def lib():
     L.lio_pm_destroy.argtypes = [vp]
     L.lio_pm_process_host.argtypes = [vp, f32p, ip, f32p, ip, f32p, f32p, i32p]
     L.lio_pm_map_centre.argtypes = [vp, i32p]
+    L.lio_pm_cube_lists.argtypes = [vp, np.ctypeslib.ndpointer(np.int64, flags="C_CONTIGUOUS"),
+                                    np.ctypeslib.ndpointer(np.int64, flags="C_CONTIGUOUS"), i32p]
     L.lio_pm_cube_size.argtypes = [vp, ip, ip, C.POINTER(ip)]
     L.lio_pm_cube_download.argtypes = [vp, ip, ip, f32p, ip]
     L.lio_mb_default_config.argtypes = [C.POINTER(MBConfig)]
@@ -187,6 +189,8 @@ def lib():
     L.lio_est_local_clouds_dev.argtypes = [vp, C.POINTER(vp), C.POINTER(vp), i32p]
     L.lio_est_local_clouds_download.argtypes = [vp, ip, f32p, ip, C.POINTER(ip)]
     L.lio_est_local_laser_odom.argtypes = [vp, f32p]
+    L.lio_est_attach_map.argtypes = [vp, vp]
+    L.lio_est_map_poses.argtypes = [vp, f32p, f32p, f32p, i32p]
     L.lio_mb_process_map_dev.argtypes = [vp, vp, vp, vp, vp, i32p, f32p, f32p, f32p, i32p]
     L.lio_po_process_dev.argtypes = [vp, C.POINTER(vp), C.POINTER(vp), i32p, f32p, f32p, i32p]
     L.lio_po_clouds_dev.argtypes = [vp, C.POINTER(vp), C.POINTER(vp), i32p]

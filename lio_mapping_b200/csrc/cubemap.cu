@@ -29,7 +29,7 @@
 #include <vector>
 #include "odom.cuh"
 #include "voxel.cuh"
-#include "twistf.h"
+#include "cubemap.cuh"
 
 namespace lio {
 
@@ -83,10 +83,13 @@ __device__ __forceinline__ int cube_of(float v, int cen) {
 constexpr int kInsOutside = 2 * kCubes, kInsKeyBits = 14;   // 2 * 4851 < 2^14
 static_assert(kInsOutside < (1 << kInsKeyBits), "insert key bits");
 
-// phase 1: map-frame point and key of every point; n_ins[0] = n (the sort's count), n_ins[1] = 0 (phase 2's run counter)
+// phase 1: map-frame point and key of every point; the counts *nc_dev / *ns_dev are clamped to [0, bc] / [0, bs] here;
+// n_ins[0] = n (the sort's count), n_ins[1] = 0 (phase 2's run counter)
 __global__ void __launch_bounds__(256)
-k_ins_keys(const float4 *__restrict__ corner, const float4 *__restrict__ surf, int n0, int n, TwistF t, int cen_l, int cen_w, int cen_h,
-           float4 *__restrict__ mapped, unsigned *__restrict__ keys, unsigned *__restrict__ vals, int *__restrict__ n_ins) {
+k_ins_keys(const float4 *__restrict__ corner, const float4 *__restrict__ surf, const int *__restrict__ nc_dev, const int *__restrict__ ns_dev,
+           int bc, int bs, TwistF t, int cen_l, int cen_w, int cen_h, float4 *__restrict__ mapped, unsigned *__restrict__ keys,
+           unsigned *__restrict__ vals, int *__restrict__ n_ins) {
+  const int n0 = min(max(*nc_dev, 0), bc), n = n0 + min(max(*ns_dev, 0), bs);
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i == 0) { n_ins[0] = n; n_ins[1] = 0; }
   if (i >= n) return;
@@ -194,14 +197,16 @@ struct lio_pm {
   ScanToMapWork stm;
   int stm_cap[3] = {0, 0, 0};
   int last_iters = 0, last_from_map[2] = {0, 0};
-  // UpdateMapDatabase (pm_update).  Insert: sort buffers for 2 * max_points keys, per-key slot / first position, the run list
+  std::vector<size_t> last_valid, last_surround;   // laser_cloud_valid_idx_ / laser_cloud_surround_idx_ of the last process call
+  // UpdateMapDatabase (pm_update).  Insert: sort buffers for ins_cap (initially 2 * max_points) keys, per-key slot / first position, the run list
   // (pinned, written by the device), the touched cubes' table (pinned and its device copy).
   unsigned *d_ins_k[2] = {nullptr, nullptr}, *d_ins_v[2] = {nullptr, nullptr};
   RadixSortTemp ins_rs;
+  int ins_cap = 0;
   int *d_ins_n = nullptr;              // [0] points, [1] runs
   int *d_slot_of = nullptr, *d_start_of = nullptr;
   InsRun *h_runs = nullptr, *h_runs_dev = nullptr;
-  int *h_nruns = nullptr;
+  int *h_nruns = nullptr;              // read-back of d_ins_n: [0] points inserted, [1] runs
   CubeEnd *h_tab = nullptr, *d_tab = nullptr;
   cudaEvent_t ev_ins = nullptr;
   // Re-filter: one segmented VoxelGrid over the jobs; their output counts arrive in h_jn (pinned) behind ev_counts and are applied
@@ -217,6 +222,7 @@ struct lio_pm {
                                        // re-filtered counts included), points inserted
   bool started = false;               // a process call has run (lio_pm_enable_publish must come before it)
   bool publish = false;                // lio_pm_enable_publish: PointMapping::PublishResults on every lio_pm_process_dev
+  bool attached = false;               // lio_est_attach_map: the estimator owns the map (its process / update / destroy entries refuse)
   // map-builder mode (lio_mb_*: MapBuilder : PointMapping, src/map_builder/MapBuilder.cc)
   bool mb = false, enable_4d = true, system_init = false;
   int skip_count = 2, odom_count = 0;
@@ -238,6 +244,7 @@ static int cube_of_host(float v, int cen) {
 
 extern "C" int lio_pm_destroy(lio_pm *m) {
   if (!m) return LIO_OK;
+  if (m->attached) { lio_set_last_error(__FILE__, __LINE__, "lio_pm_destroy: the map is attached to an estimator (lio_est_destroy releases it)"); return LIO_ERR_INVALID; }
   cudaSetDevice(m->device);
   for (int w = 0; w < 2; ++w) {
     for (lio_pm::Cube &c : m->cube[w]) if (c.p) cudaFree(c.p);
@@ -279,6 +286,7 @@ extern "C" int lio_pm_create(int max_points, float corner_filter_size, float sur
     ok = ok && cudaMalloc(&m->d_stack[w], sizeof(float4) * max_points) == cudaSuccess;
     ok = ok && cudaMalloc(&m->d_ds[w], sizeof(float4) * max_points) == cudaSuccess;
   }
+  m->ins_cap = 2 * max_points;
   ok = ok && cudaMalloc(&m->d_mapped, sizeof(float4) * 2 * max_points) == cudaSuccess;
   ok = ok && cudaMalloc(&m->d_cnt, sizeof(int) * 12) == cudaSuccess;
   ok = ok && cudaMalloc(&m->d_seg, sizeof(Segment) * 256) == cudaSuccess;
@@ -294,7 +302,7 @@ extern "C" int lio_pm_create(int max_points, float corner_filter_size, float sur
   ok = ok && cudaMalloc(&m->d_tab, sizeof(CubeEnd) * kInsOutside) == cudaSuccess;
   ok = ok && cudaHostAlloc(&m->h_runs, sizeof(InsRun) * kInsOutside, cudaHostAllocMapped) == cudaSuccess;
   ok = ok && cudaHostGetDevicePointer(&m->h_runs_dev, m->h_runs, 0) == cudaSuccess;
-  ok = ok && cudaMallocHost(&m->h_nruns, sizeof(int)) == cudaSuccess;
+  ok = ok && cudaMallocHost(&m->h_nruns, sizeof(int) * 2) == cudaSuccess;
   ok = ok && cudaMallocHost(&m->h_tab, sizeof(CubeEnd) * kInsOutside) == cudaSuccess;
   ok = ok && m->svg.init() == 0;
   ok = ok && cudaMallocHost(&m->h_jobs, sizeof(VgJob) * kVgMaxJobs) == cudaSuccess;
@@ -424,31 +432,35 @@ static int pm_counts(lio_pm *m) {
   return LIO_OK;
 }
 
-// UpdateMapDatabase (:1112-1208) of the n_ds[0] corner and n_ds[1] surf points in d_ds with the pose t; valid holds cube indices
+// UpdateMapDatabase (:1112-1208) of the corner src[0] and surf src[1] clouds in HBM with the pose t.  Their counts are read on the
+// device (*n_dev[w], clamped to [0, bound[w]]); bound[0] + bound[1] <= ins_cap.  valid holds cube indices
 // of the margin centre mc (:1173-1183 move them to the current centre).  Insert: the keys, a stable sort by key and the run list
 // on the device; the host waits once for the runs to size the touched segments (and once per segment it moves to a larger one),
 // then uploads their {segment, count} table.  Re-filter: one segmented VoxelGrid over every non-empty valid cube, corner and surf,
 // whose output counts reach the directory through pm_counts without a wait here (the next reader waits; upd_stats counts that wait).
-static int pm_update(lio_pm *m, const std::vector<size_t> &valid, const int n_ds[2], const TwistF &t, const int mc[3]) {
+static int pm_update(lio_pm *m, const std::vector<size_t> &valid, const float4 *const src[2], const int *const n_dev[2], const int bound[2],
+                     const TwistF &t, const int mc[3]) {
   cudaStream_t st = m->stream;
   int rc = pm_counts(m);
   if (rc != LIO_OK) return rc;
-  int launches = 0, waits = 0;
-  const int n = n_ds[0] + n_ds[1];
-  if (n > 0) {
-    const int blocks = (n + 255) / 256;
-    k_ins_keys<<<blocks, 256, 0, st>>>(m->d_ds[0], m->d_ds[1], n_ds[0], n, t, m->cen_l, m->cen_w, m->cen_h, m->d_mapped, m->d_ins_k[0],
-                                       m->d_ins_v[0], m->d_ins_n);
+  if (bound[0] + bound[1] > m->ins_cap) { lio_set_last_error(__FILE__, __LINE__, "UpdateMapDatabase: clouds exceed the insert buffers"); return LIO_ERR_CAPACITY; }
+  int launches = 0, waits = 0, n = 0;
+  const int nb = bound[0] + bound[1];
+  if (nb > 0) {
+    const int blocks = (nb + 255) / 256;
+    k_ins_keys<<<blocks, 256, 0, st>>>(src[0], src[1], n_dev[0], n_dev[1], bound[0], bound[1], t, m->cen_l, m->cen_w, m->cen_h, m->d_mapped,
+                                       m->d_ins_k[0], m->d_ins_v[0], m->d_ins_n);
     ++launches;
-    const int b = radix_sort_pairs(m->d_ins_k[0], m->d_ins_v[0], m->d_ins_k[1], m->d_ins_v[1], m->d_ins_n, n, kInsKeyBits, m->ins_rs, st, &launches);
+    const int b = radix_sort_pairs(m->d_ins_k[0], m->d_ins_v[0], m->d_ins_k[1], m->d_ins_v[1], m->d_ins_n, nb, kInsKeyBits, m->ins_rs, st, &launches);
     if (b < 0) return LIO_ERR_CAPACITY;
     k_ins_runs<<<blocks, 256, 0, st>>>(m->d_ins_k[b], m->d_ins_n, m->d_ins_n + 1, m->h_runs_dev, m->d_slot_of, m->d_start_of);
     ++launches;
-    LIO_CUDA_OK(cudaMemcpyAsync(m->h_nruns, m->d_ins_n + 1, sizeof(int), cudaMemcpyDeviceToHost, st));
+    LIO_CUDA_OK(cudaMemcpyAsync(m->h_nruns, m->d_ins_n, sizeof(int) * 2, cudaMemcpyDeviceToHost, st));
     LIO_CUDA_OK(cudaEventRecord(m->ev_ins, st));
     LIO_CUDA_OK(cudaEventSynchronize(m->ev_ins));
     ++waits;
-    const int nr = *m->h_nruns;
+    n = m->h_nruns[0];
+    const int nr = m->h_nruns[1];
     for (int r = 0; r < nr; ++r) {
       const InsRun run = m->h_runs[r];
       lio_pm::Cube &c = m->cube[run.key / kCubes][run.key % kCubes];
@@ -583,9 +595,9 @@ static void twist_to_tf7(const TwistF &t, float o[7]) { o[0] = t.qx; o[1] = t.qy
 static int mb_surround(lio_pm *m, const std::vector<size_t> &surround);
 
 // PublishResults (PointMapping.cc:1210-1270) / PublishMapBuilderResults (MapBuilder.cc:144-218): the surround map every
-// num_map_frames_ (5) calls, the first call included, and the nf-point full cloud in d_full_in to the map frame with the final
-// tobe every call.  The only synchronisation is the read of the surround size on calls that publish it.
-static int pm_publish(lio_pm *m, const std::vector<size_t> &surround, int nf, bool &published) {
+// num_map_frames_ (5) calls, the first call included, and the full cloud `full` (count *nf_dev, host value nf <= max_full) to the
+// map frame with the final tobe every call.  The only synchronisation is the read of the surround size on calls that publish it.
+static int pm_publish(lio_pm *m, const std::vector<size_t> &surround, const float4 *full, const int *nf_dev, int nf, bool &published) {
   cudaStream_t st = m->stream;
   published = ++m->map_frame_count >= 5;
   if (published) {
@@ -593,7 +605,7 @@ static int pm_publish(lio_pm *m, const std::vector<size_t> &surround, int nf, bo
     int rc = mb_surround(m, surround);
     if (rc != LIO_OK) return rc;
   }
-  if (nf > 0) k_associate<<<(nf + 255) / 256, 256, 0, st>>>(m->d_full_in, m->d_full_out, m->d_cnt + 4, m->tobe, 0);
+  if (nf > 0) k_associate<<<(nf + 255) / 256, 256, 0, st>>>(full, m->d_full_out, nf_dev, m->tobe, 0);
   m->n_full = nf;
   if (published) {
     LIO_CUDA_OK(cudaMemcpyAsync(m->h_sur_n, m->d_cnt + 6, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -615,18 +627,19 @@ static int pm_process(lio_pm *m, const float4 *const src[2], const float4 *full,
   m->sum = tf7_to_twist(transform_sum7);
   m->tobe = twist_mul(m->tobe, twist_mul(twist_inverse(m->bef), m->sum));   // TransformAssociateToMap :753-756
   if ((rc = pm_stack(m, src, full, n3_dev, n_max)) != LIO_OK) return rc;
-  std::vector<size_t> valid, surround;
   int K[2] = {0, 0}, n_ds[2] = {0, 0};
-  if ((rc = pm_locate(m, valid, m->publish ? &surround : nullptr, K)) != LIO_OK) return rc;
+  if ((rc = pm_locate(m, m->last_valid, m->publish ? &m->last_surround : nullptr, K)) != LIO_OK) return rc;
   if ((rc = pm_downsample(m, nin, n_ds)) != LIO_OK) return rc;
   const bool optimised = !(K[0] <= 10 || K[1] <= 100);
   m->last_iters = 0;
   if (optimised && (rc = pm_optimise(m, K, n_ds, 0)) != LIO_OK) return rc;
   if (optimised) { m->bef = m->sum; m->aft = m->tobe; }   // TransformUpdate sits behind the optimiser's early return (:327-329, :716)
   const int cen[3] = {m->cen_l, m->cen_w, m->cen_h};   // margin centre == current centre: the valid list is this call's
-  if ((rc = pm_update(m, valid, n_ds, m->tobe, cen)) != LIO_OK) return rc;
+  const float4 *ds[2] = {m->d_ds[0], m->d_ds[1]};
+  const int *n_ds_dev[2] = {m->d_cnt + 2, m->d_cnt + 3};
+  if ((rc = pm_update(m, m->last_valid, ds, n_ds_dev, n_ds, m->tobe, cen)) != LIO_OK) return rc;
   bool published = false;
-  if (m->publish && (rc = pm_publish(m, surround, n_max[2] > 0 ? m->h_cnt[4] : 0, published)) != LIO_OK) return rc;
+  if (m->publish && (rc = pm_publish(m, m->last_surround, m->d_full_in, m->d_cnt + 4, n_max[2] > 0 ? m->h_cnt[4] : 0, published)) != LIO_OK) return rc;
   if (transform_tobe_mapped7) twist_to_tf7(m->tobe, transform_tobe_mapped7);
   if (transform_aft_mapped7) twist_to_tf7(m->aft, transform_aft_mapped7);
   const int out[5] = {m->last_iters, K[0], K[1], published ? 1 : 0, m->publish ? m->n_surround : 0};
@@ -637,7 +650,8 @@ static int pm_process(lio_pm *m, const float4 *const src[2], const float4 *full,
 // Clouds: HOST arrays of n x 4 floats.
 extern "C" int lio_pm_process_host(lio_pm *m, const float *corner_last, int nc, const float *surf_last, int ns, const float transform_sum7[7],
                                    float transform_tobe_mapped7[7], int info3[3]) {
-  if (!m || m->mb || m->publish || !transform_sum7 || nc < 0 || ns < 0 || (nc > 0 && !corner_last) || (ns > 0 && !surf_last)) return LIO_ERR_INVALID;
+  if (!m || m->mb || m->publish || m->attached || !transform_sum7 || nc < 0 || ns < 0 || (nc > 0 && !corner_last) || (ns > 0 && !surf_last))
+    return LIO_ERR_INVALID;
   if (nc > m->max_points || ns > m->max_points) return LIO_ERR_CAPACITY;
   LIO_CUDA_OK(cudaSetDevice(m->device));
   const float *src[2] = {corner_last, surf_last};
@@ -652,7 +666,7 @@ extern "C" int lio_pm_process_host(lio_pm *m, const float *corner_last, int nc, 
 extern "C" int lio_pm_process_dev(lio_pm *m, const float *corner_dev, const float *surf_dev, const float *full_dev, const int *n3_dev,
                                   const int n3_max[3], const float transform_sum7[7], float transform_tobe_mapped7[7], float transform_aft_mapped7[7],
                                   int info5[5]) {
-  if (!m || m->mb || !transform_sum7 || !n3_dev || !n3_max || n3_max[0] < 0 || n3_max[1] < 0 || n3_max[2] < 0 || (n3_max[0] > 0 && !corner_dev) ||
+  if (!m || m->mb || m->attached || !transform_sum7 || !n3_dev || !n3_max || n3_max[0] < 0 || n3_max[1] < 0 || n3_max[2] < 0 || (n3_max[0] > 0 && !corner_dev) ||
       (n3_max[1] > 0 && !surf_dev) || (m->publish && n3_max[2] > 0 && !full_dev))
     return LIO_ERR_INVALID;
   LIO_CUDA_OK(cudaSetDevice(m->device));
@@ -665,7 +679,7 @@ extern "C" int lio_pm_process_dev(lio_pm *m, const float *corner_dev, const floa
 
 extern "C" int lio_pm_update_map_database_host(lio_pm *m, const float *corner_ds, int nc, const float *surf_ds, int ns, const long long *valid,
                                                int nv, const float tf7[7], const int margin_centre3[3]) {
-  if (!m || !tf7 || !margin_centre3 || nc < 0 || ns < 0 || nv < 0 || (nc > 0 && !corner_ds) || (ns > 0 && !surf_ds) || (nv > 0 && !valid))
+  if (!m || m->attached || !tf7 || !margin_centre3 || nc < 0 || ns < 0 || nv < 0 || (nc > 0 && !corner_ds) || (ns > 0 && !surf_ds) || (nv > 0 && !valid))
     return LIO_ERR_INVALID;
   if (nc > m->max_points || ns > m->max_points || nv > 125) return LIO_ERR_CAPACITY;
   std::vector<size_t> v(valid, valid + nv);
@@ -675,10 +689,13 @@ extern "C" int lio_pm_update_map_database_host(lio_pm *m, const float *corner_ds
   }
   LIO_CUDA_OK(cudaSetDevice(m->device));
   cudaStream_t st = m->stream;
+  const int n_ds[2] = {nc, ns};
   if (nc > 0) LIO_CUDA_OK(cudaMemcpyAsync(m->d_ds[0], corner_ds, sizeof(float4) * nc, cudaMemcpyHostToDevice, st));
   if (ns > 0) LIO_CUDA_OK(cudaMemcpyAsync(m->d_ds[1], surf_ds, sizeof(float4) * ns, cudaMemcpyHostToDevice, st));
-  const int n_ds[2] = {nc, ns};
-  return pm_update(m, v, n_ds, tf7_to_twist(tf7), margin_centre3);
+  LIO_CUDA_OK(cudaMemcpyAsync(m->d_cnt + 8, n_ds, sizeof(n_ds), cudaMemcpyHostToDevice, st));   // pageable: staged before the call returns
+  const float4 *ds[2] = {m->d_ds[0], m->d_ds[1]};
+  const int *n_ds_dev[2] = {m->d_cnt + 8, m->d_cnt + 9};
+  return pm_update(m, v, ds, n_ds_dev, n_ds, tf7_to_twist(tf7), margin_centre3);
 }
 
 extern "C" int lio_pm_update_stats(lio_pm *m, int info4[4]) {
@@ -815,9 +832,8 @@ static int mb_process_map(lio_pm *m, const float4 *const src[2], const float4 *f
   if (m->enable_4d) m->tobe = transform_4d_associate(m->tobe, m->bef, m->sum);
   else m->tobe = twist_mul(m->tobe, twist_mul(twist_inverse(m->bef), m->sum));   // TransformAssociateToMap (PointMapping.cc:755-758)
   if ((rc = pm_stack(m, src, full, n3_dev, n_max)) != LIO_OK) return rc;
-  std::vector<size_t> valid, surround;
   int K[2] = {0, 0}, n_ds[2] = {0, 0};
-  if ((rc = pm_locate(m, valid, &surround, K)) != LIO_OK) return rc;
+  if ((rc = pm_locate(m, m->last_valid, &m->last_surround, K)) != LIO_OK) return rc;
   if ((rc = pm_downsample(m, nin, n_ds)) != LIO_OK) return rc;
   const int nf = n_max[2] > 0 ? m->h_cnt[4] : 0;
   // optimisation gate (:529-544): OptimizeMap / OptimizeTransformTobeMapped end with the update behind their early return
@@ -833,10 +849,12 @@ static int mb_process_map(lio_pm *m, const float4 *const src[2], const float4 *f
   }
   ++m->odom_count;
   const int cen[3] = {m->cen_l, m->cen_w, m->cen_h};   // margin centre == current centre: the valid list is this call's
-  if ((rc = pm_update(m, valid, n_ds, m->tobe, cen)) != LIO_OK) return rc;
+  const float4 *ds[2] = {m->d_ds[0], m->d_ds[1]};
+  const int *n_ds_dev[2] = {m->d_cnt + 2, m->d_cnt + 3};
+  if ((rc = pm_update(m, m->last_valid, ds, n_ds_dev, n_ds, m->tobe, cen)) != LIO_OK) return rc;
   // PublishMapBuilderResults: surround map every num_map_frames_ (5) frames, registered full cloud every frame
   bool publish = false;
-  if ((rc = pm_publish(m, surround, nf, publish)) != LIO_OK) return rc;
+  if ((rc = pm_publish(m, m->last_surround, m->d_full_in, m->d_cnt + 4, nf, publish)) != LIO_OK) return rc;
   if (transform_tobe_mapped7) twist_to_tf7(m->tobe, transform_tobe_mapped7);
   if (transform_aft_mapped7) twist_to_tf7(m->aft, transform_aft_mapped7);
   if (info6) { info6[0] = m->last_iters; info6[1] = gate; info6[2] = K[0]; info6[3] = K[1]; info6[4] = publish; info6[5] = m->n_surround; }
@@ -909,6 +927,14 @@ extern "C" int lio_pm_map_centre(lio_pm *m, int centre3[3]) {
   return LIO_OK;
 }
 
+extern "C" int lio_pm_cube_lists(lio_pm *m, long long valid[125], long long surround[125], int n2[2]) {
+  if (!m || !n2) return LIO_ERR_INVALID;
+  n2[0] = (int)m->last_valid.size(); n2[1] = (int)m->last_surround.size();
+  if (valid) for (int i = 0; i < n2[0]; ++i) valid[i] = (long long)m->last_valid[i];
+  if (surround) for (int i = 0; i < n2[1]; ++i) surround[i] = (long long)m->last_surround[i];
+  return LIO_OK;
+}
+
 extern "C" int lio_pm_cube_size(lio_pm *m, int cube_index, int which, int *n) {
   if (!m || !n || cube_index < 0 || cube_index >= kCubes || which < 0 || which > 1) return LIO_ERR_INVALID;
   LIO_CUDA_OK(cudaSetDevice(m->device));
@@ -927,5 +953,71 @@ extern "C" int lio_pm_cube_download(lio_pm *m, int cube_index, int which, float 
   if (c.n > cap) return LIO_ERR_CAPACITY;
   if (c.n > 0) LIO_CUDA_OK(cudaMemcpyAsync(out_xyzi, c.p, sizeof(float4) * c.n, cudaMemcpyDeviceToHost, m->stream));
   LIO_CUDA_OK(cudaStreamSynchronize(m->stream));
+  return LIO_OK;
+}
+
+// ---- the device estimator's map after initialisation (cubemap.cuh, lio_est_attach_map) ------------------------------------
+int pm_attach(lio_pm *m, int device, float corner_leaf, float surf_leaf, int ins_bound, int full_bound) {
+  if (!m || m->mb || !m->publish || !m->started || m->attached || m->device != device) {
+    lio_set_last_error(__FILE__, __LINE__, "lio_est_attach_map: needs a publishing PointMapping (lio_pm_enable_publish) on the estimator's device "
+                                           "that has run a process call and is not attached");
+    return LIO_ERR_INVALID;
+  }
+  if (m->leaf[0] != corner_leaf || m->leaf[1] != surf_leaf) {
+    lio_set_last_error(__FILE__, __LINE__, "lio_est_attach_map: the map's corner / surf leaf sizes differ from the estimator's");
+    return LIO_ERR_INVALID;
+  }
+  if (m->max_full < full_bound) {
+    lio_set_last_error(__FILE__, __LINE__, "lio_est_attach_map: the map's max_full_points is below the estimator's full-cloud capacity");
+    return LIO_ERR_CAPACITY;
+  }
+  LIO_CUDA_OK(cudaSetDevice(m->device));
+  int rc = pm_counts(m);
+  if (rc != LIO_OK) return rc;
+  if (ins_bound > m->ins_cap) {   // an accumulated surf slot exceeds 2 * max_points: new insert buffers, swapped in on success
+    LIO_CUDA_OK(cudaStreamSynchronize(m->stream));
+    float4 *mapped = nullptr;
+    unsigned *k[2] = {nullptr, nullptr}, *v[2] = {nullptr, nullptr};
+    RadixSortTemp rs;
+    bool ok = cudaMalloc(&mapped, sizeof(float4) * ins_bound) == cudaSuccess;
+    for (int b = 0; b < 2 && ok; ++b) {
+      ok = ok && cudaMalloc(&k[b], sizeof(unsigned) * ins_bound) == cudaSuccess;
+      ok = ok && cudaMalloc(&v[b], sizeof(unsigned) * ins_bound) == cudaSuccess;
+    }
+    ok = ok && rs.init(ins_bound) == 0;
+    if (!ok) {
+      void *fr[] = {mapped, k[0], k[1], v[0], v[1]};
+      for (void *q : fr) if (q) cudaFree(q);
+      rs.destroy();
+      lio_set_last_error(__FILE__, __LINE__, "lio_est_attach_map: insert buffer allocation failed");
+      return LIO_ERR_CUDA;
+    }
+    void *fr[] = {m->d_mapped, m->d_ins_k[0], m->d_ins_k[1], m->d_ins_v[0], m->d_ins_v[1]};
+    for (void *q : fr) cudaFree(q);
+    m->ins_rs.destroy();
+    m->d_mapped = mapped;
+    for (int b = 0; b < 2; ++b) { m->d_ins_k[b] = k[b]; m->d_ins_v[b] = v[b]; }
+    m->ins_rs = rs;
+    m->ins_cap = ins_bound;
+  }
+  m->attached = true;
+  return LIO_OK;
+}
+
+void pm_detach(lio_pm *m) { if (m) m->attached = false; }
+cudaStream_t pm_stream(const lio_pm *m) { return m->stream; }
+TwistF *pm_tobe(lio_pm *m) { return &m->tobe; }
+TwistF pm_aft(const lio_pm *m) { return m->aft; }
+
+int pm_est_step(lio_pm *m, bool insert, const float4 *const src[2], const int *const n_dev[2], const int bound[2], const TwistF &pose,
+                const float4 *full, const int *nf_dev, int nf, int info4[4]) {
+  int rc = LIO_OK;
+  if (insert) {
+    const int cen[3] = {m->cen_l, m->cen_w, m->cen_h};   // opt_cube_centers_: the centre is frozen with the valid list
+    if ((rc = pm_update(m, m->last_valid, src, n_dev, bound, pose, cen)) != LIO_OK) return rc;
+  }
+  bool published = false;
+  if ((rc = pm_publish(m, m->last_surround, full, nf_dev, nf, published)) != LIO_OK) return rc;
+  info4[0] = insert ? 1 : 0; info4[1] = insert ? m->upd_stats[3] : 0; info4[2] = published ? 1 : 0; info4[3] = m->n_surround;
   return LIO_OK;
 }

@@ -9,6 +9,7 @@
 //   SlideWindow :2570-2666                  -> slide_window
 // There is no CPU path for the per-point work: without a CUDA device create() fails.
 #include "assemble.cuh"
+#include "cubemap.cuh"
 #include <atomic>
 #include <condition_variable>
 #include <functional>
@@ -576,6 +577,17 @@ struct lio_est {
   cudaStream_t lc_stream = nullptr;
   cudaEvent_t lc_ev_fork = nullptr, lc_ev_join = nullptr;
   TransformF es{0, 0, 0, 1, 0, 0, 0};   // transform_es_ (Estimator.h), kept across scans like the member
+  // ---- the global cube map after initialisation (lio_est_attach_map): the PointMapping the reference's Estimator is.  Its work
+  // runs on the map's stream, forked after the solve (map_ev_in) and joined at the next scan's entry and staging (map_ev_done).
+  lio_pm *map = nullptr;
+  bool scanned = false;               // a process_scan / open_scan has run: too late to attach
+  int map_scans = 0;                  // INITED scans since the attach: opt_point_coeff_mask_.first() is false from scan O on
+  bool map_pending = false;
+  float4 *d_keep[2] = {nullptr, nullptr};   // W == O with de-skew: the previous frame's corner / surf cloud, kept until its insert
+  int *d_keep_n = nullptr;            // [2]
+  cudaEvent_t map_ev_in = nullptr, map_ev_done = nullptr;
+  lio::TwistF map_insert;             // opt_transforms_.first() of the last insert
+  int map_info[4] = {0, 0, 0, 0};     // inserted, points inserted, surround published, last surround size
 };
 
 static Tw tlb_double(const lio_est *e) {
@@ -692,6 +704,14 @@ extern "C" int lio_est_destroy(lio_est *e) {
   if (!e) return LIO_OK;
   if (e->mjob.running) { e->worker.wait(); e->mjob.running = false; }
   cudaSetDevice(e->device);
+  if (e->map) {   // the pending insert reads the estimator's slots: wait for it, then release the map
+    if (e->map_pending) cudaEventSynchronize(e->map_ev_done);
+    pm_detach(e->map);
+  }
+  for (int w = 0; w < 2; ++w) if (e->d_keep[w]) cudaFree(e->d_keep[w]);
+  if (e->d_keep_n) cudaFree(e->d_keep_n);
+  if (e->map_ev_in) cudaEventDestroy(e->map_ev_in);
+  if (e->map_ev_done) cudaEventDestroy(e->map_ev_done);
   for (float4 *p : e->slot_ptr) if (p) cudaFree(p);
   for (FeatureOut &f : e->feats) if (f.src) cudaFree(f.src);
   void *ptrs[] = {e->d_slot_n, e->d_own_n, e->d_scan, e->d_local, e->d_map, e->d_tmp, e->d_counts, e->fslab, e->d_tf, e->d_odom, e->d_odom_partial};
@@ -897,7 +917,12 @@ extern "C" int lio_est_enable_local_clouds(lio_est *e, float corner_filter_size,
 
 // The staging buffers may still be read by the previous push's forked work (stepwise API: staging inside an open scan)
 static int lc_stage_wait(lio_est *e) {
+  if (e->map && e->window_open) {   // the open scan's /cloud_registered is registered from the staged full cloud when it closes
+    lio_set_last_error(__FILE__, __LINE__, "a map is attached: stage the next scan's clouds after lio_est_close_scan");
+    return LIO_ERR_INVALID;
+  }
   if (e->lc_pending) EST_CUDA(cudaStreamWaitEvent(e->stream, e->lc_ev_join, 0));
+  if (e->map_pending) EST_CUDA(cudaStreamWaitEvent(e->stream, e->map_ev_done, 0));   // the registration reads the staged full cloud
   return LIO_OK;
 }
 
@@ -1286,6 +1311,7 @@ static int build_local_map(lio_est *e, const std::function<int()> &before_sync =
     EST_CUDA(cudaMemcpyAsync(e->h_counts + W + 7, e->vg.overflow_flag(), sizeof(int), cudaMemcpyDeviceToHost, st));
     EST_CUDA(cudaMemcpyAsync(e->h_counts + W + 8, &e->d_odom->done, sizeof(int), cudaMemcpyDeviceToHost, st));
     if (e->fpeers) EST_CUDA(cudaMemcpyAsync(e->h_counts + W + 9, e->fslab + e->foff_flags + 128, sizeof(int), cudaMemcpyDeviceToHost, st));
+    if (e->map) EST_CUDA(cudaMemcpyAsync(e->h_counts + W + 13, e->d_lc_stage_n + 1, sizeof(int), cudaMemcpyDeviceToHost, st));   // /cloud_registered size
     EST_CUDA(cudaStreamSynchronize(st));
     return LIO_OK;
   };
@@ -1937,6 +1963,7 @@ static int solve_host(lio_est *e, int max_it) {
   return LIO_OK;
 }
 
+static int map_step(lio_est *e);
 static int scan_close_window(lio_est *e) {
   double_to_vector(e);
   const double t1 = now_s();
@@ -1948,8 +1975,9 @@ static int scan_close_window(lio_est *e) {
   }
   e->t_marg = now_s() - t1;
   e->window_open = false;
-  const int rc = lc_join(e);   // the forked /local/* work reads the surf slot that SlideWindow replaces
+  int rc = lc_join(e);   // the forked /local/* work reads the surf slot that SlideWindow replaces
   if (rc != LIO_OK) return rc;
+  if (e->map && (rc = map_step(e)) != LIO_OK) return rc;   // UpdateMapDatabase + PublishResults come before SlideWindow (:703-723)
   return slide_window(e);
 }
 
@@ -2139,6 +2167,124 @@ static int slide_window(lio_est *e) {  // Estimator.cc:2570-2666
   return LIO_OK;
 }
 
+// ---- the global cube map after initialisation (lio_est_attach_map; Estimator.cc:703-723, :776-812) -------------------------
+static bool map_deskew(const lio_est *e) { return e->cfg.enable_deskew || e->cfg.cutoff_deskew; }
+
+// Scan entry: join the previous scan's map work (it reads frame slots the push below may reuse, and the staged full cloud), predict
+// transform_tobe_mapped_ (ProcessCompactData :776-809, imu_factor: tobe * lb * (prev^-1 * curr) * lb^-1 in float Twist, prev / curr
+// the float casts of the states W - 1 and W) and, when W == O with de-skew, keep the clouds of the frame that leaves the window:
+// they are the ones this scan inserts (see map_step).
+static int map_scan_entry(lio_est *e) {
+  const int W = e->W, O = e->O;
+  cudaStream_t st = e->stream;
+  if (e->map_pending) { EST_CUDA(cudaStreamWaitEvent(st, e->map_ev_done, 0)); e->map_pending = false; }
+  auto twist_of = [](const M3 &R, const V3 &P) {
+    const Q q = fromR(R);
+    return lio::TwistF{(float)q.x, (float)q.y, (float)q.z, (float)q.w, (float)P.x, (float)P.y, (float)P.z};
+  };
+  const lio::TwistF d = lio::twist_mul(lio::twist_inverse(twist_of(e->Rs[W - 1], e->Ps[W - 1])), twist_of(e->Rs[W], e->Ps[W]));
+  const lio::TwistF lb{e->tlb_q[0], e->tlb_q[1], e->tlb_q[2], e->tlb_q[3], e->tlb_p[0], e->tlb_p[1], e->tlb_p[2]};
+  lio::TwistF *tobe = pm_tobe(e->map);
+  *tobe = lio::twist_mul(lio::twist_mul(lio::twist_mul(*tobe, lb), d), lio::twist_inverse(lb));
+  if (W == O && map_deskew(e) && e->map_scans >= O) {
+    const int s0 = e->slot_of[0];
+    k_copy_cloud<<<std::max(1, std::min(e->sm_count * 2, (e->lc_cap[0] + 255) / 256)), 256, 0, st>>>(
+        e->lc_slot[0][s0], e->d_lc_slot_n + s0, e->lc_cap[0], e->d_keep[0], e->d_keep_n);
+    k_copy_cloud<<<std::max(1, std::min(e->sm_count * 2, (e->slot_cap + 255) / 256)), 256, 0, st>>>(
+        e->slot_ptr[s0], e->d_slot_n + s0, e->slot_cap, e->d_keep[1], e->d_keep_n + 1);
+    e->launches += 2;
+    EST_CUDA(cudaGetLastError());
+  }
+  return LIO_OK;
+}
+
+// After the solve, before SlideWindow: UpdateMapDatabase of opt_*_stack_.first() (:703-708) from scan O on (the warm-start frames
+// count as mapped: opt_point_coeff_mask_ is true for them, :616, and false for INITED frames, :467), then PublishResults (:721).
+// The clouds those entries alias (:474-485, :689-693): with either de-skew flag the INITED push of a frame's clouds comes after its
+// opt entry was recorded, so the entry is the previous frame's cloud objects - logical frame pivot - 1 now, or the copy kept at the
+// scan's entry when W == O.  Without de-skew it is the frame's own objects, logical frame pivot.  The surf object is the slot as
+// SlideWindow (:2615) has accumulated it in place; the corner object is never rewritten.  With W == O SlideWindow's prepend drops
+// all of surf_stack_[0] (its size is size_surf_stack_[0]), so the frame's own cloud is what the reference inserts there too.
+// The pose is opt_transforms_[0] as SolveOptimization overwrites it (:2279-2286).  The work runs on the map's stream.
+static int map_step(lio_est *e) {
+  const int W = e->W, O = e->O, pivot = W - O;
+  const bool insert = e->map_scans >= O;
+  ++e->map_scans;
+  const float4 *src[2] = {nullptr, nullptr};
+  const int *n_dev[2] = {nullptr, nullptr};
+  int bound[2] = {0, 0};
+  if (insert) {
+    if (map_deskew(e) && pivot == 0) {
+      src[0] = e->d_keep[0]; src[1] = e->d_keep[1];
+      n_dev[0] = e->d_keep_n; n_dev[1] = e->d_keep_n + 1;
+    } else {
+      const int s = e->slot_of[map_deskew(e) ? pivot - 1 : pivot];
+      src[0] = e->lc_slot[0][s]; src[1] = e->slot_ptr[s];
+      n_dev[0] = e->d_lc_slot_n + s; n_dev[1] = e->d_slot_n + s;
+    }
+    bound[0] = e->lc_cap[0]; bound[1] = e->slot_cap;
+    const Tw tlb = tlb_double(e);
+    const Q rot = fromR(e->Rs[pivot] * toR(normalized(conj(tlb.rot))));
+    const V3 pos = e->Ps[pivot] - rotate(rot, tlb.pos);
+    e->map_insert = lio::TwistF{(float)rot.x, (float)rot.y, (float)rot.z, (float)rot.w, (float)pos.x, (float)pos.y, (float)pos.z};
+  }
+  cudaStream_t ms = pm_stream(e->map);
+  EST_CUDA(cudaEventRecord(e->map_ev_in, e->stream));
+  EST_CUDA(cudaStreamWaitEvent(ms, e->map_ev_in, 0));
+  e->map_pending = true;
+  const int rc = pm_est_step(e->map, insert, src, n_dev, bound, e->map_insert, e->d_lc_stage[1], e->d_lc_stage_n + 1, e->h_counts[W + 13], e->map_info);
+  if (rc != LIO_OK) return rc;
+  EST_CUDA(cudaEventRecord(e->map_ev_done, ms));
+  return LIO_OK;
+}
+
+extern "C" int lio_est_attach_map(lio_est *e, lio_pm *pm) {
+  if (!e || !pm) return LIO_ERR_INVALID;
+  const char *why = nullptr;
+  if (e->map) why = "lio_est_attach_map: a map is attached already";
+  else if (!e->tmp_pre) why = "lio_est_attach_map: call it after lio_est_finish_init";
+  else if (e->scanned) why = "lio_est_attach_map: call it before the first scan";
+  else if (!e->lc_on) why = "lio_est_attach_map: local clouds are off (lio_est_enable_local_clouds)";
+  else if (!e->cfg.imu_factor) why = "lio_est_attach_map: needs imu_factor = 1";
+  else if (e->world > 1 || e->npeers || e->fpeers) why = "lio_est_attach_map: not supported on a sharded context";
+  if (why) { lio_set_last_error(__FILE__, __LINE__, why); return LIO_ERR_INVALID; }
+  LIO_CUDA_OK(cudaSetDevice(e->device));
+  const bool keep = e->W == e->O && map_deskew(e);
+  bool ok = cudaEventCreateWithFlags(&e->map_ev_in, cudaEventDisableTiming) == cudaSuccess;
+  ok = ok && cudaEventCreateWithFlags(&e->map_ev_done, cudaEventDisableTiming) == cudaSuccess;
+  if (keep) {
+    ok = ok && cudaMalloc(&e->d_keep[0], sizeof(float4) * e->lc_cap[0]) == cudaSuccess;
+    ok = ok && cudaMalloc(&e->d_keep[1], sizeof(float4) * e->slot_cap) == cudaSuccess;
+    ok = ok && cudaMalloc(&e->d_keep_n, sizeof(int) * 2) == cudaSuccess;
+  }
+  int rc = ok ? LIO_OK : LIO_ERR_CUDA;
+  if (!ok) lio_set_last_error(__FILE__, __LINE__, "lio_est_attach_map: device allocation failed");
+  // an accumulated surf slot holds up to max_frame_points * (W - O + 1) points: the map's insert buffers grow to it
+  if (ok) rc = pm_attach(pm, e->device, e->lc_corner_leaf, e->cfg.surf_filter_size, e->lc_cap[0] + e->slot_cap, e->lc_cap[1]);
+  if (rc != LIO_OK) {   // nothing changed: the buffers go, the handle stays usable without a map
+    for (int w = 0; w < 2; ++w) { if (e->d_keep[w]) cudaFree(e->d_keep[w]); e->d_keep[w] = nullptr; }
+    if (e->d_keep_n) cudaFree(e->d_keep_n);
+    if (e->map_ev_in) cudaEventDestroy(e->map_ev_in);
+    if (e->map_ev_done) cudaEventDestroy(e->map_ev_done);
+    e->d_keep_n = nullptr; e->map_ev_in = e->map_ev_done = nullptr;
+    return rc;
+  }
+  e->map = pm;
+  e->map_scans = 0;
+  return LIO_OK;
+}
+
+extern "C" int lio_est_map_poses(lio_est *e, float tobe7[7], float aft7[7], float insert7[7], int info4[4]) {
+  if (!e) return LIO_ERR_INVALID;
+  if (!e->map) { lio_set_last_error(__FILE__, __LINE__, "no map attached (lio_est_attach_map)"); return LIO_ERR_INVALID; }
+  auto out = [](const lio::TwistF &t, float *o) { if (o) { o[0] = t.qx; o[1] = t.qy; o[2] = t.qz; o[3] = t.qw; o[4] = t.px; o[5] = t.py; o[6] = t.pz; } };
+  out(*pm_tobe(e->map), tobe7);
+  out(pm_aft(e->map), aft7);
+  out(e->map_insert, insert7);
+  if (info4) for (int k = 0; k < 4; ++k) info4[k] = e->map_info[k];
+  return LIO_OK;
+}
+
 static int process_scan_body(lio_est *e, const float4 *scan_dev, const int *n_dev, int n_max, bool open_only);
 // The pre-integration buffer, the slot rotation and size_surf_stack advance before the fallible device work.  A failure
 // after that point leaves the window half-slid, so the context is poisoned: later calls return LIO_ERR_INVALID instead of
@@ -2156,11 +2302,13 @@ static int process_scan_common(lio_est *e, const float4 *scan_dev, const int *n_
     return LIO_ERR_INVALID;
   }
   e->frames_started = true;
+  e->scanned = true;
   const int rc = process_scan_body(e, scan_dev, n_dev, n_max, open_only);
   if (rc != LIO_OK) { e->poisoned = true; std::snprintf(e->err, sizeof(e->err), "%s", lio_last_error()); }
   return rc;
 }
 
+static int map_scan_entry(lio_est *e);
 static int process_scan_body(lio_est *e, const float4 *scan_dev, const int *n_dev, int n_max, bool open_only) {
   const int W = e->W;
   cudaStream_t st = e->stream;
@@ -2170,6 +2318,10 @@ static int process_scan_body(lio_est *e, const float4 *scan_dev, const int *n_de
   e->t_lin_wait = e->t_lin_host = e->t_lin_lidar = e->t_marg_wait = 0;
   e->have_H0 = false;
   if (!e->tmp_pre) { lio_set_last_error(__FILE__, __LINE__, "process_scan before finish_init"); return LIO_ERR_INVALID; }
+  if (e->map) {
+    const int rc0 = map_scan_entry(e);
+    if (rc0 != LIO_OK) return rc0;
+  }
   push_shift(e->pre, e->tmp_pre);
   e->tmp_pre = std::make_shared<Preintegration>(e->acc_last, e->gyr_last, e->Bas[W], e->Bgs[W], e->noise);
   // frame slot rotation (CircularBuffer push): the dropped logical frame 0 becomes the new frame W

@@ -120,6 +120,7 @@ class Estimator:
         if getattr(self, "h", None):
             _lib.lib().lio_est_destroy(self.h)
             self.h = None
+        self._map = None
 
     def __del__(self):
         try:
@@ -333,6 +334,23 @@ class Estimator:
             _lib.check(_lib.lib().lio_est_local_clouds_download(self.h, w, a, a.shape[0], C.byref(n)), "lio_est_local_clouds_download")
             out[name] = a[:n.value].copy()
         return out
+
+    # ---- the global cube map after initialisation (lio_est_attach_map)
+    def attach_map(self, pm):
+        """Hand a publishing PointMapping (EnablePublish, at least one ProcessDev, same device) that built the pre-initialisation map
+        to the estimator: after finish_init, before the first scan, with local clouds on.  From then on every scan predicts
+        transform_tobe_mapped_, inserts the oldest optimised frame from the (O+1)-th scan on and publishes the surround map and the
+        registered full cloud on pm (pm.surround_map(), pm.registered_full_cloud(), pm.cube(...)).  pm refuses its own process
+        calls and close() until this estimator is closed; the estimator keeps a reference to it."""
+        _lib.check(_lib.lib().lio_est_attach_map(self.h, pm.h), "lio_est_attach_map")
+        self._map = pm
+
+    def map_poses(self):
+        """After a scan with an attached map: (tobe tf7 = transform_tobe_mapped_, aft tf7 = the frozen transform_aft_mapped_,
+        insert tf7 = the pose of the last insert, info dict)."""
+        tobe = np.zeros(7, np.float32); aft = np.zeros(7, np.float32); ins = np.zeros(7, np.float32); info = np.zeros(4, np.int32)
+        _lib.check(_lib.lib().lio_est_map_poses(self.h, tobe, aft, ins, info), "lio_est_map_poses")
+        return tobe, aft, ins, dict(inserted=bool(info[0]), points=int(info[1]), surround_published=bool(info[2]), surround_size=int(info[3]))
 
     def summary(self):
         s = np.zeros(32)

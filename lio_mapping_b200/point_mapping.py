@@ -23,8 +23,8 @@ class PointMapping:
                                             int(max_iterations), device, C.c_void_p(stream), C.byref(self.h)), "lio_pm_create")
 
     def close(self):
-        if getattr(self, "h", None):
-            _lib.lib().lio_pm_destroy(self.h)
+        # an attached map (Estimator.attach_map) is refused until its estimator is closed; the handle is kept for then
+        if getattr(self, "h", None) and _lib.lib().lio_pm_destroy(self.h) == 0:
             self.h = None
 
     def __del__(self):
@@ -83,6 +83,12 @@ class PointMapping:
         out = np.zeros(3, np.int32)
         _lib.check(_lib.lib().lio_pm_map_centre(self.h, out), "lio_pm_map_centre")
         return tuple(out.tolist())
+
+    def cube_lists(self):
+        """(laser_cloud_valid_idx_, laser_cloud_surround_idx_) of the last process call as int64 arrays."""
+        v = np.zeros(125, np.int64); s = np.zeros(125, np.int64); n = np.zeros(2, np.int32)
+        _lib.check(_lib.lib().lio_pm_cube_lists(self.h, v, s, n), "lio_pm_cube_lists")
+        return v[:n[0]].copy(), s[:n[1]].copy()
 
     def cube_sizes(self, which):
         w = 0 if which == "corner" else 1
