@@ -362,6 +362,19 @@ int lio_asm_set_fold_chunks(int chunks);
  * factorisation, trailing update incl. barrier} as seen by the warp that runs the serial chain, then the back substitution. */
 int lio_dev_cholesky_solve_host(const double *A, const double *b, int n, double *x, int *ok, long long *prof, int device);
 
+/* Test seam of the sort under every device VoxelGrid and the cube-map insert: the stable LSD radix sort of (key, value) pairs
+ * by the low key_bits (1..32) bits, rounded up to whole 8-bit passes, on n host pairs; the result is read from whichever
+ * buffer pair the last pass wrote.  Synchronous. */
+int lio_radix_sort_pairs_host(const uint32_t *keys, const uint32_t *vals, int n, int key_bits, uint32_t *keys_out,
+                              uint32_t *vals_out, int device);
+/* Test seam of the segmented VoxelGrid of UpdateMapDatabase's re-filter: njobs (1..256) clouds of n_per_job[j] >= 1 points,
+ * concatenated in xyzi (float4), each filtered as its own pcl::VoxelGrid with leaf_per_job[j].  out (sum of n_per_job float4)
+ * receives job j's centroids at the job's own input offset, n_out_per_job[j] their count; what follows them in the job's
+ * span is unspecified.  A job whose floor-space grid exceeds 2^24 voxels sets *index_bound_error and returns LIO_ERR_CAPACITY
+ * without writing out.  Synchronous. */
+int lio_seg_voxel_grid_host(const float *xyzi, const int *n_per_job, const float *leaf_per_job, int njobs, float *out,
+                            int *n_out_per_job, int *index_bound_error, int device);
+
 /* IntegrationBase (include/imu_processor/IntegrationBase.h:72-388) */
 typedef struct lio_pim lio_pim;
 int lio_pim_create(const double acc0[3], const double gyr0[3], const double ba[3], const double bg[3],

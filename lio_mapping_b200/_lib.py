@@ -86,6 +86,9 @@ def lib():
     L.lio_pp_start_ori.argtypes = [vp, C.POINTER(C.c_float)]
     L.lio_pp_last_launches.argtypes = [vp]
     L.lio_voxel_grid_host.argtypes = [f32p, ip, C.c_float, f32p, ip, C.POINTER(ip), ip]
+    u32p = np.ctypeslib.ndpointer(np.uint32, flags="C_CONTIGUOUS")
+    L.lio_radix_sort_pairs_host.argtypes = [u32p, u32p, ip, ip, u32p, u32p, ip]
+    L.lio_seg_voxel_grid_host.argtypes = [f32p, i32p, f32p, ip, f32p, i32p, C.POINTER(ip), ip]
     L.lio_calculate_features_host.argtypes = [f32p, ip, f32p, ip, f32p, C.c_float, C.c_float, f32p, f32p, i32p,
                                               C.POINTER(ip), ip]
     L.lio_calculate_line_features_host.argtypes = [f32p, ip, f32p, ip, f32p, C.c_float, f32p, f32p, i32p, C.POINTER(ip), ip]

@@ -156,3 +156,42 @@ int radix_sort_pairs(unsigned *keys_a, unsigned *vals_a, unsigned *keys_b, unsig
 }
 
 }  // namespace lio
+
+// ---- C-ABI test aid: radix_sort_pairs on host buffers ------------------------------------------------------------------
+using namespace lio;
+
+extern "C" int lio_radix_sort_pairs_host(const uint32_t *keys, const uint32_t *vals, int n, int key_bits, uint32_t *keys_out,
+                                         uint32_t *vals_out, int device) {
+  if (n < 0 || key_bits < 1 || key_bits > 32 || (n > 0 && (!keys || !vals || !keys_out || !vals_out))) return LIO_ERR_INVALID;
+  if (lio_device_count() <= 0) return LIO_ERR_NO_DEVICE;
+  LIO_CUDA_OK(cudaSetDevice(device));
+  if (n == 0) return LIO_OK;
+  RadixSortTemp tmp;
+  unsigned *ka = nullptr, *va = nullptr, *kb = nullptr, *vb = nullptr;
+  int *d_n = nullptr;
+  int rc = LIO_OK;
+  const size_t bytes = sizeof(unsigned) * (size_t)n;
+  if (tmp.init(n) != 0 || cudaMalloc(&ka, bytes) != cudaSuccess || cudaMalloc(&va, bytes) != cudaSuccess ||
+      cudaMalloc(&kb, bytes) != cudaSuccess || cudaMalloc(&vb, bytes) != cudaSuccess || cudaMalloc(&d_n, sizeof(int)) != cudaSuccess) {
+    lio_set_last_error(__FILE__, __LINE__, "cudaMalloc failed");
+    rc = LIO_ERR_CUDA;
+  }
+  if (rc == LIO_OK && (cudaMemcpy(ka, keys, bytes, cudaMemcpyHostToDevice) != cudaSuccess ||
+                       cudaMemcpy(va, vals, bytes, cudaMemcpyHostToDevice) != cudaSuccess ||
+                       cudaMemcpy(d_n, &n, sizeof(int), cudaMemcpyHostToDevice) != cudaSuccess)) {
+    lio_set_last_error(__FILE__, __LINE__, "upload failed");
+    rc = LIO_ERR_CUDA;
+  }
+  if (rc == LIO_OK) {
+    const int which = radix_sort_pairs(ka, va, kb, vb, d_n, n, key_bits, tmp, 0, nullptr);
+    cudaError_t e = which < 0 ? cudaSuccess : cudaDeviceSynchronize();
+    if (which < 0) rc = LIO_ERR_CAPACITY;
+    else if (e == cudaSuccess) e = cudaMemcpy(keys_out, which ? kb : ka, bytes, cudaMemcpyDeviceToHost);
+    if (e == cudaSuccess && rc == LIO_OK) e = cudaMemcpy(vals_out, which ? vb : va, bytes, cudaMemcpyDeviceToHost);
+    if (e != cudaSuccess) { lio_set_last_error(__FILE__, __LINE__, cudaGetErrorString(e)); rc = LIO_ERR_CUDA; }
+  }
+  void *p[] = {ka, va, kb, vb, d_n};
+  for (void *q : p) if (q) cudaFree(q);
+  tmp.destroy();
+  return rc;
+}

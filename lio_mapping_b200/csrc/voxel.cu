@@ -11,6 +11,7 @@
 //
 // SegVoxelGrid runs the same steps over many clouds at once (UpdateMapDatabase's re-filter of the valid cubes).
 #include <algorithm>
+#include <vector>
 #include "voxel.cuh"
 
 namespace lio {
@@ -387,5 +388,53 @@ extern "C" int lio_voxel_grid_host(const float *cloud, int n, float leaf, float 
   if (d_out) cudaFree(d_out);
   if (d_n) cudaFree(d_n);
   vg.destroy();
+  return rc;
+}
+
+// ---- C-ABI test aid: SegVoxelGrid::run on concatenated host clouds ------------------------------------------------------
+extern "C" int lio_seg_voxel_grid_host(const float *xyzi, const int *n_per_job, const float *leaf_per_job, int njobs, float *out,
+                                       int *n_out_per_job, int *index_bound_error, int device) {
+  if (!xyzi || !n_per_job || !leaf_per_job || !out || !n_out_per_job || !index_bound_error || njobs < 1) return LIO_ERR_INVALID;
+  long long total = 0;
+  for (int j = 0; j < njobs; ++j) {
+    if (n_per_job[j] < 1 || !(leaf_per_job[j] > 0)) return LIO_ERR_INVALID;
+    total += n_per_job[j];
+  }
+  if (njobs > kVgMaxJobs || total >= (1LL << 30)) return LIO_ERR_CAPACITY;
+  if (lio_device_count() <= 0) return LIO_ERR_NO_DEVICE;
+  LIO_CUDA_OK(cudaSetDevice(device));
+  *index_bound_error = 0;
+  SegVoxelGrid sg;
+  float4 *d = nullptr;
+  std::vector<VgJob> jobs(njobs);
+  std::vector<int> jn(njobs + 1, 0);
+  int rc = LIO_OK;
+  if (sg.init() != 0 || sg.reserve((int)total) != 0 || cudaMalloc(&d, sizeof(float4) * total) != cudaSuccess) {
+    lio_set_last_error(__FILE__, __LINE__, "cudaMalloc failed");
+    rc = LIO_ERR_CUDA;
+  }
+  if (rc == LIO_OK && cudaMemcpy(d, xyzi, sizeof(float4) * total, cudaMemcpyHostToDevice) != cudaSuccess) {
+    lio_set_last_error(__FILE__, __LINE__, "upload failed");
+    rc = LIO_ERR_CUDA;
+  }
+  if (rc == LIO_OK) {
+    for (int j = 0, off = 0; j < njobs; off += n_per_job[j], ++j) jobs[j] = VgJob{d + off, n_per_job[j], off, leaf_per_job[j]};
+    rc = sg.run(jobs.data(), njobs, (int)total, jn.data(), 0, nullptr);
+    cudaError_t e = rc == LIO_OK ? cudaDeviceSynchronize() : cudaSuccess;
+    if (e != cudaSuccess) { lio_set_last_error(__FILE__, __LINE__, cudaGetErrorString(e)); rc = LIO_ERR_CUDA; }
+  }
+  if (rc == LIO_OK) {
+    for (int j = 0; j < njobs; ++j) n_out_per_job[j] = jn[j];
+    *index_bound_error = jn[njobs] != 0;
+    if (*index_bound_error) {
+      lio_set_last_error(__FILE__, __LINE__, "a job's voxel grid exceeds 2^24 voxels");
+      rc = LIO_ERR_CAPACITY;
+    } else {
+      cudaError_t e = cudaMemcpy(out, d, sizeof(float4) * total, cudaMemcpyDeviceToHost);
+      if (e != cudaSuccess) { lio_set_last_error(__FILE__, __LINE__, cudaGetErrorString(e)); rc = LIO_ERR_CUDA; }
+    }
+  }
+  if (d) cudaFree(d);
+  sg.destroy();
   return rc;
 }

@@ -19,6 +19,34 @@ def voxel_grid(cloud: np.ndarray, leaf: float, device: int = 0) -> np.ndarray:
     return out[:n.value].copy()
 
 
+def radix_sort_pairs(keys: np.ndarray, vals: np.ndarray, key_bits: int, device: int = 0):
+    """The device's stable radix sort of (key, value) pairs by the low key_bits bits in whole bytes (lio_radix_sort_pairs_host)."""
+    _lib.require_device()
+    keys = np.ascontiguousarray(keys, np.uint32)
+    vals = np.ascontiguousarray(vals, np.uint32)
+    ko, vo = np.zeros_like(keys), np.zeros_like(vals)
+    _lib.check(_lib.lib().lio_radix_sort_pairs_host(keys, vals, keys.shape[0], key_bits, ko, vo, device), "lio_radix_sort_pairs_host")
+    return ko, vo
+
+
+def seg_voxel_grid(clouds, leaves, device: int = 0):
+    """The segmented VoxelGrid (lio_seg_voxel_grid_host): one pcl::VoxelGrid per cloud with its own leaf, in one pass.
+    Returns (the filtered clouds, False), or (None, True) when a cloud's grid exceeds the 2^24-voxel index bound."""
+    _lib.require_device()
+    clouds = [np.ascontiguousarray(c, np.float32).reshape(-1, 4) for c in clouds]
+    n = np.array([c.shape[0] for c in clouds], np.int32)
+    cat = np.ascontiguousarray(np.concatenate(clouds), np.float32)
+    out = np.zeros_like(cat)
+    n_out = np.zeros_like(n)
+    err = C.c_int()
+    rc = _lib.lib().lio_seg_voxel_grid_host(cat, n, np.asarray(leaves, np.float32), n.shape[0], out, n_out, C.byref(err), device)
+    if rc == -3 and err.value:
+        return None, True
+    _lib.check(rc, "lio_seg_voxel_grid_host")
+    off = np.concatenate([[0], np.cumsum(n)])
+    return [out[off[j]:off[j] + n_out[j]].copy() for j in range(n.shape[0])], False
+
+
 def calculate_features(map_pts, surf, tf7, min_match_sq_dis=1.0, min_plane_dis=0.2, device: int = 0):
     """Estimator::CalculateFeatures on explicit arrays (lio_calculate_features_host)."""
     _lib.require_device()
