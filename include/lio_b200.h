@@ -136,7 +136,9 @@ int lio_transform_to_end_host(float *cloud, int n, const float *tf7_es, float ti
 /* Estimator::CalculateLaserOdom (Estimator.cc:1099-1360): up to max_iter rounds of CalculateFeatures +
  * 6-DoF point-to-plane Gauss-Newton (float features, double normal equations, degeneracy projection at
  * the first round) refining tf7 in place.  Outputs are sized M * (keep_features ? max_iter : 1); *iters =
- * rounds executed before the delta_r / delta_t < 0.05 exit. */
+ * rounds executed before the delta_r / delta_t < 0.05 exit.  Runs the estimator's own chain: without
+ * keep_features each round is the batched k-NN launch plus the fused single-CTA k_odom_round, with it the
+ * k-NN launch plus k_odom_reduce / k_odom_solve over all kept features. */
 int lio_laser_odom_host(const float *map, int K, const float *surf, int M, float *tf7, float min_match_sq_dis,
                         float min_plane_dis, int keep_features, int max_iter, float *pts4, float *coef4, int32_t *src,
                         int *n_out, int *iters, int device);

@@ -35,24 +35,7 @@ namespace lio {
 
 constexpr int kCubeL = 21, kCubeW = 21, kCubeH = 11, kCubes = kCubeL * kCubeW * kCubeH;
 
-// q * v (Eigen _transformVector) in float, host copy of the device expression
-static void rotate_host(const TwistF &t, float vx, float vy, float vz, float &ox, float &oy, float &oz) {
-  volatile float ux = t.qy * vz - t.qz * vy, uy = t.qz * vx - t.qx * vz, uz = t.qx * vy - t.qy * vx;
-  volatile float ux2 = ux + ux, uy2 = uy + uy, uz2 = uz + uz;
-  volatile float cx = t.qy * uz2 - t.qz * uy2, cy = t.qz * ux2 - t.qx * uz2, cz = t.qx * uy2 - t.qy * ux2;
-  volatile float ax = ux2 * t.qw, ay = uy2 * t.qw, az = uz2 * t.qw;
-  volatile float rx = vx + ax, ry = vy + ay, rz = vz + az;
-  ox = rx + cx; oy = ry + cy; oz = rz + cz;
-}
-
 // ---- kernels ----------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void rotate_dev(float qx, float qy, float qz, float qw, float vx, float vy, float vz, float &ox, float &oy, float &oz) {
-  float ux = qy * vz - qz * vy, uy = qz * vx - qx * vz, uz = qx * vy - qy * vx;
-  ux += ux; uy += uy; uz += uz;
-  const float cx = qy * uz - qz * uy, cy = qz * ux - qx * uz, cz = qx * uy - qy * ux;
-  ox = vx + ux * qw + cx; oy = vy + uy * qw + cy; oz = vz + uz * qw + cz;
-}
-
 // mode 0: PointAssociateToMap (po = q * pi + t, :303-314); mode 1: PointAssociateTobeMapped (po = q^* * (pi - t), :316-323)
 __global__ void __launch_bounds__(256)
 k_associate(const float4 *__restrict__ in, float4 *__restrict__ out, const int *__restrict__ n_dev, TwistF t, int mode) {
@@ -62,10 +45,10 @@ k_associate(const float4 *__restrict__ in, float4 *__restrict__ out, const int *
   const float4 p = __ldg(in + i);
   float x, y, z;
   if (mode == 0) {
-    rotate_dev(t.qx, t.qy, t.qz, t.qw, p.x, p.y, p.z, x, y, z);
+    odom_qmul_vec(t.qx, t.qy, t.qz, t.qw, p.x, p.y, p.z, x, y, z);
     x += t.px; y += t.py; z += t.pz;
   } else {
-    rotate_dev(-t.qx, -t.qy, -t.qz, t.qw, p.x - t.px, p.y - t.py, p.z - t.pz, x, y, z);
+    odom_qmul_vec(-t.qx, -t.qy, -t.qz, t.qw, p.x - t.px, p.y - t.py, p.z - t.pz, x, y, z);
   }
   out[i] = make_float4(x, y, z, p.w);
 }
@@ -96,7 +79,7 @@ k_ins_keys(const float4 *__restrict__ corner, const float4 *__restrict__ surf, c
   const int w = i < n0 ? 0 : 1;
   const float4 p = w == 0 ? __ldg(corner + i) : __ldg(surf + (i - n0));
   float x, y, z;
-  rotate_dev(t.qx, t.qy, t.qz, t.qw, p.x, p.y, p.z, x, y, z);
+  odom_qmul_vec(t.qx, t.qy, t.qz, t.qw, p.x, p.y, p.z, x, y, z);
   x += t.px; y += t.py; z += t.pz;
   mapped[i] = make_float4(x, y, z, p.w);
   const int ci = cube_of(x, cen_l), cj = cube_of(y, cen_w), ck = cube_of(z, cen_h);

@@ -87,13 +87,6 @@ k_concat(const ConcatParams P, float4 *__restrict__ dst, int *__restrict__ n_out
   }
 }
 
-__device__ __forceinline__ void qmul_vec(float qx, float qy, float qz, float qw, float vx, float vy, float vz, float &ox, float &oy, float &oz) {
-  float ux = qy * vz - qz * vy, uy = qz * vx - qx * vz, uz = qx * vy - qy * vx;
-  ux += ux; uy += uy; uz += uz;
-  float cx = qy * uz - qz * uy, cy = qz * ux - qx * uz, cz = qx * uy - qy * ux;
-  ox = vx + ux * qw + cx; oy = vy + uy * qw + cy; oz = vz + uz * qw + cz;
-}
-
 // TransformToEnd (Estimator.cc:62-103), in place; keep_intensity leaves the intensity as is (the full-cloud call, :2416)
 __global__ void __launch_bounds__(256)
 k_deskew(float4 *__restrict__ cloud, const int *__restrict__ n_dev, TransformF es, float time_factor, bool keep_intensity = false) {
@@ -122,9 +115,9 @@ k_deskew(float4 *__restrict__ cloud, const int *__restrict__ n_dev, TransformF e
   float nn = sqrtf(sx * sx + sy * sy + sz * sz + sw * sw);
   float cx = -sx / nn, cy = -sy / nn, cz = -sz / nn, cw = sw / nn;
   float ax, ay, az;
-  qmul_vec(cx, cy, cz, cw, p.x, p.y, p.z, ax, ay, az);
+  odom_qmul_vec(cx, cy, cz, cw, p.x, p.y, p.z, ax, ay, az);
   float bx, by, bz;
-  qmul_vec(es.qx, es.qy, es.qz, es.qw, ax, ay, az, bx, by, bz);
+  odom_qmul_vec(es.qx, es.qy, es.qz, es.qw, ax, ay, az, bx, by, bz);
   cloud[i] = make_float4(bx + es.px, by + es.py, bz + es.pz, p.w);
 }
 
@@ -162,56 +155,31 @@ k_odom_reduce(const float4 *__restrict__ pts, const float4 *__restrict__ coef, c
   if (st->done) return;
   const int n = *n_dev;
   const TransformF tf = *tf_dev;
-  // rot.toRotationMatrix() of the (possibly un-normalised) quaternion, float
-  float R[9];
-  {
-    const float tx = 2.f * tf.qx, ty = 2.f * tf.qy, tz = 2.f * tf.qz;
-    const float twx = tx * tf.qw, twy = ty * tf.qw, twz = tz * tf.qw, txx = tx * tf.qx, txy = ty * tf.qx, txz = tz * tf.qx;
-    const float tyy = ty * tf.qy, tyz = tz * tf.qy, tzz = tz * tf.qz;
-    R[0] = 1.f - (tyy + tzz); R[1] = txy - twz; R[2] = txz + twy;
-    R[3] = txy + twz; R[4] = 1.f - (txx + tzz); R[5] = tyz - twx;
-    R[6] = txz - twy; R[7] = tyz + twx; R[8] = 1.f - (txx + tyy);
-  }
+  float R[9], Ri[9];
+  odom_rotation(tf, R);
   // mode 2 (MapBuilder::OptimizeMap, MapBuilder.cc:905-911): J_r is post-multiplied by rot.inverse().toRotationMatrix()
   // (inverse = conjugate / squaredNorm) and the rotation information matrix diag(5e-3, 5e-3, 1)
-  float Ri[9];
   {
     const float n2 = tf.qx * tf.qx + tf.qy * tf.qy + tf.qz * tf.qz + tf.qw * tf.qw;
-    const float ix = -tf.qx / n2, iy = -tf.qy / n2, iz = -tf.qz / n2, iw = tf.qw / n2;
-    const float tx = 2.f * ix, ty = 2.f * iy, tz = 2.f * iz;
-    const float twx = tx * iw, twy = ty * iw, twz = tz * iw, txx = tx * ix, txy = ty * ix, txz = tz * ix;
-    const float tyy = ty * iy, tyz = tz * iy, tzz = tz * iz;
-    Ri[0] = 1.f - (tyy + tzz); Ri[1] = txy - twz; Ri[2] = txz + twy;
-    Ri[3] = txy + twz; Ri[4] = 1.f - (txx + tzz); Ri[5] = tyz - twx;
-    Ri[6] = txz - twy; Ri[7] = tyz + twx; Ri[8] = 1.f - (txx + tyy);
+    TransformF inv = tf;
+    inv.qx = -tf.qx / n2; inv.qy = -tf.qy / n2; inv.qz = -tf.qz / n2; inv.qw = tf.qw / n2;
+    odom_rotation(inv, Ri);
   }
   double acc[27];
 #pragma unroll
   for (int k = 0; k < 27; ++k) acc[k] = 0.0;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    float4 p = __ldg(pts + i), c = __ldg(coef + i);
-    // RS = R * skew(p);  J_r = -w^T RS,  J_t = w^T
-    float RS[9];
-#pragma unroll
-    for (int r = 0; r < 3; ++r) {
-      RS[r * 3 + 0] = R[r * 3 + 1] * p.z + R[r * 3 + 2] * (-p.y);
-      RS[r * 3 + 1] = R[r * 3 + 0] * (-p.z) + R[r * 3 + 2] * p.x;
-      RS[r * 3 + 2] = R[r * 3 + 0] * p.y + R[r * 3 + 1] * (-p.x);
-    }
-    float row[6];
-#pragma unroll
-    for (int q = 0; q < 3; ++q) row[q] = -(c.x * RS[q] + c.y * RS[3 + q] + c.z * RS[6 + q]);
+    const float4 p = __ldg(pts + i), c = __ldg(coef + i);
+    // CalculateLaserOdom: d2 = w . (R p + t) + b (Estimator.cc:1282-1284); scan-to-map: d2 = coeff.intensity (PointMapping.cc:634)
+    float row[6], d2;
+    odom_row(tf, R, p, c, row, d2);
+    if (mode != 0) d2 = c.w;
     if (mode == 2) {
       const float t0 = row[0] * Ri[0] + row[1] * Ri[3] + row[2] * Ri[6];
       const float t1 = row[0] * Ri[1] + row[1] * Ri[4] + row[2] * Ri[7];
       const float t2 = row[0] * Ri[2] + row[1] * Ri[5] + row[2] * Ri[8];
       row[0] = t0 * 5e-3f; row[1] = t1 * 5e-3f; row[2] = t2 * 1.0f;
     }
-    row[3] = c.x; row[4] = c.y; row[5] = c.z;
-    float rx, ry, rz;
-    qmul_vec(tf.qx, tf.qy, tf.qz, tf.qw, p.x, p.y, p.z, rx, ry, rz);
-    // CalculateLaserOdom: d2 = w . (R p + t) + b (Estimator.cc:1282-1284); scan-to-map: d2 = coeff.intensity (PointMapping.cc:634)
-    float d2 = mode != 0 ? c.w : c.x * (rx + tf.px) + c.y * (ry + tf.py) + c.z * (rz + tf.pz) + c.w;
     int k = 0;
 #pragma unroll
     for (int a = 0; a < 6; ++a) {
@@ -328,6 +296,43 @@ k_odom_round(const float4 *__restrict__ pts, const float4 *__restrict__ coef, co
   }
   __syncthreads();
   if (threadIdx.x == 0) odom_solve_step(st, tf_dev, delta_r_abort, delta_t_abort);
+}
+
+// Rounds [from, to) of CalculateLaserOdom (Estimator.cc:1242-1359) for the frame cloud surf (*n_dev points, at most n_bound)
+// against the map's hash, refining *tf_dev: the estimator's chain, which lio_laser_odom_host runs as well.  A round after
+// convergence is a no-op on the device (done flag).  `launches` (optional) counts the kernel launches.
+static int odom_rounds(const CellHash &h, const float4 *surf, const int *n_dev, int n_bound, TransformF *tf_dev, const FeatureOut &fo,
+                       bool keep_features, OdomState *odom, double *partial, KnnWork &work, float min_match_sq_dis, float min_plane_dis,
+                       int from, int to, int sm, cudaStream_t q, int *launches) {
+  if (!keep_features) {
+    // two launches per round and no memset: the k-NN + plane fit of the frame, then ONE CTA that reduces the round's features
+    // to A^T A / A^T b, takes the 6 x 6 Gauss-Newton step and re-arms the k-NN launch state
+    KnnBatch ob;
+    ob.nframes = 1;
+    KnnFrame &f = ob.f[0];
+    f.surf = surf; f.n_dev = n_dev; f.n_bound = n_bound; f.tf = tf_dev;
+    f.out_p = fo.pts; f.out_c = fo.coef; f.out_src = fo.src; f.out_count = fo.count;
+    f.append = 0; f.tile0 = 0;
+    for (int it = from; it < to; ++it) {
+      int rc = calculate_features_batch(h, ob, min_match_sq_dis, min_plane_dis, &odom->done, work, q, launches, 0, it > 0);
+      if (rc != LIO_OK) return rc;
+      k_odom_round<<<1, kOdomRoundThreads, 0, q>>>(fo.pts, fo.coef, fo.count, tf_dev, odom, 0.05, 0.05, work.status, ob.ntiles, work.ticket);
+      if (launches) ++*launches;
+    }
+  } else {
+    // keep_features: every round re-evaluates ALL kept features at the current transform (Estimator.cc:978-980), so the
+    // reduction is a pass of its own
+    const int nb = std::max(1, std::min(sm, (fo.cap + kOdomThreads - 1) / kOdomThreads));
+    for (int it = from; it < to; ++it) {
+      int rc = calculate_features_dev(h, nullptr, surf, n_dev, n_bound, tf_dev, min_match_sq_dis, min_plane_dis, fo, 1, &odom->done, work, q,
+                                      launches);
+      if (rc != LIO_OK) return rc;
+      k_odom_reduce<<<nb, kOdomThreads, 0, q>>>(fo.pts, fo.coef, fo.count, tf_dev, odom, partial);
+      k_odom_solve<<<1, 32, 0, q>>>(odom, tf_dev, 0.05, 0.05);
+      if (launches) *launches += 2;
+    }
+  }
+  return LIO_OK;
 }
 
 }  // namespace lio
@@ -604,37 +609,13 @@ static Tw lidar_pose(const V3 &P, const M3 &R, const Tw &tlb) {  // Estimator.cc
 struct AffineF { float R[9]; float t[3]; TransformF tf; };
 static AffineF to_affine_f(const Tw &t) {
   AffineF a;
-  float qx = (float)t.rot.x, qy = (float)t.rot.y, qz = (float)t.rot.z, qw = (float)t.rot.w;
-  float n = std::sqrt(qx * qx + qy * qy + qz * qz + qw * qw);
-  qx /= n; qy /= n; qz /= n; qw /= n;
-  const float tx = 2.f * qx, ty = 2.f * qy, tz = 2.f * qz;
-  const float twx = tx * qw, twy = ty * qw, twz = tz * qw, txx = tx * qx, txy = ty * qx, txz = tz * qx;
-  const float tyy = ty * qy, tyz = tz * qy, tzz = tz * qz;
-  a.R[0] = 1.f - (tyy + tzz); a.R[1] = txy - twz; a.R[2] = txz + twy;
-  a.R[3] = txy + twz; a.R[4] = 1.f - (txx + tzz); a.R[5] = tyz - twx;
-  a.R[6] = txz - twy; a.R[7] = tyz + twx; a.R[8] = 1.f - (txx + tyy);
+  lio::TwistF tw;
+  tw.qx = (float)t.rot.x; tw.qy = (float)t.rot.y; tw.qz = (float)t.rot.z; tw.qw = (float)t.rot.w;
+  quat_to_matrix_normalized(tw, a.R);
   a.t[0] = (float)t.pos.x; a.t[1] = (float)t.pos.y; a.t[2] = (float)t.pos.z;
   // Twist<float>(Affine3f): Quaternionf(linear).normalized()
-  float m[3][3] = {{a.R[0], a.R[1], a.R[2]}, {a.R[3], a.R[4], a.R[5]}, {a.R[6], a.R[7], a.R[8]}};
   float q[4];
-  float tr = m[0][0] + m[1][1] + m[2][2];
-  if (tr > 0.f) {
-    float s = std::sqrt(tr + 1.0f);
-    q[3] = 0.5f * s;
-    s = 0.5f / s;
-    q[0] = (m[2][1] - m[1][2]) * s; q[1] = (m[0][2] - m[2][0]) * s; q[2] = (m[1][0] - m[0][1]) * s;
-  } else {
-    int i = 0;
-    if (m[1][1] > m[0][0]) i = 1;
-    if (m[2][2] > m[i][i]) i = 2;
-    int j = (i + 1) % 3, k = (j + 1) % 3;
-    float s = std::sqrt(m[i][i] - m[j][j] - m[k][k] + 1.0f);
-    q[i] = 0.5f * s;
-    s = 0.5f / s;
-    q[3] = (m[k][j] - m[j][k]) * s;
-    q[j] = (m[j][i] + m[i][j]) * s;
-    q[k] = (m[k][i] + m[i][k]) * s;
-  }
+  matrix_to_quat(a.R, q);
   float qn = std::sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]);
   a.tf.qx = q[0] / qn; a.tf.qy = q[1] / qn; a.tf.qz = q[2] / qn; a.tf.qw = q[3] / qn;
   a.tf.px = a.t[0]; a.tf.py = a.t[1]; a.tf.pz = a.t[2];
@@ -1233,40 +1214,10 @@ static int build_local_map(lio_est *e, const std::function<int()> &before_sync =
   // synchronisation (it converges in 2-3 rounds); only if the flag is still clear are the remaining rounds enqueued.
   constexpr int kOdomFirstBatch = 3;
   const bool odom = e->cfg.imu_factor && owns_frame(e, W);
-  KnnBatch ob;
-  auto odom_rounds = [&](int from, int to, cudaStream_t q) -> int {
-    const int idx = W, slot = e->slot_of[W];
-    if (!e->cfg.keep_features) {
-      // two launches per round and no memset: the k-NN + plane fit of the newest frame, then ONE CTA that reduces the
-      // round's features to A^T A / A^T b, takes the 6 x 6 Gauss-Newton step and re-arms the k-NN launch state
-      ob.nframes = 1;
-      KnnFrame &f = ob.f[0];
-      f.surf = e->slot_ptr[slot]; f.n_dev = e->d_slot_n + slot; f.n_bound = e->cfg.max_frame_points; f.tf = e->d_tf + idx;
-      f.out_p = e->feats[idx].pts; f.out_c = e->feats[idx].coef; f.out_src = e->feats[idx].src; f.out_count = e->feats[idx].count;
-      f.append = 0; f.tile0 = 0;
-      for (int it = from; it < to; ++it) {
-        int r2 = calculate_features_batch(e->hash, ob, e->cfg.min_match_sq_dis, e->cfg.min_plane_dis, &e->d_odom->done, e->knn2, q, &e->launches,
-                                          0, it > 0);
-        if (r2 != LIO_OK) return r2;
-        k_odom_round<<<1, kOdomRoundThreads, 0, q>>>(e->feats[idx].pts, e->feats[idx].coef, e->feats[idx].count, e->d_tf + idx, e->d_odom, 0.05, 0.05,
-                                                      e->knn2.status, ob.ntiles, e->knn2.ticket);
-        ++e->launches;
-      }
-    } else {
-      // keep_features: every round re-evaluates ALL kept features at the current transform (Estimator.cc:978-980), so the
-      // reduction is a pass of its own
-      const int nb = std::max(1, std::min(e->sm_count, (e->feats[idx].cap + kOdomThreads - 1) / kOdomThreads));
-      for (int it = from; it < to; ++it) {
-        int r2 = calculate_features_dev(e->hash, e->d_map, e->slot_ptr[slot], e->d_slot_n + slot, e->cfg.max_frame_points, e->d_tf + idx,
-                                        e->cfg.min_match_sq_dis, e->cfg.min_plane_dis, e->feats[idx], 1,
-                                        &e->d_odom->done, e->knn2, q, &e->launches);
-        if (r2 != LIO_OK) return r2;
-        k_odom_reduce<<<nb, kOdomThreads, 0, q>>>(e->feats[idx].pts, e->feats[idx].coef, e->feats[idx].count, e->d_tf + idx, e->d_odom, e->d_odom_partial);
-        k_odom_solve<<<1, 32, 0, q>>>(e->d_odom, e->d_tf + idx, 0.05, 0.05);
-        e->launches += 2;
-      }
-    }
-    return LIO_OK;
+  auto rounds = [&](int from, int to, cudaStream_t q) {
+    const int slot = e->slot_of[W];
+    return odom_rounds(e->hash, e->slot_ptr[slot], e->d_slot_n + slot, e->cfg.max_frame_points, e->d_tf + W, e->feats[W], e->cfg.keep_features,
+                       e->d_odom, e->d_odom_partial, e->knn2, e->cfg.min_match_sq_dis, e->cfg.min_plane_dis, from, to, e->sm_count, q, &e->launches);
   };
   const int odom_total = odom ? e->cfg.odom_max_iterations : 0;
   const int odom_first = e->fpeers ? odom_total : std::min(odom_total, kOdomFirstBatch);   // exchanged features must be final
@@ -1276,7 +1227,7 @@ static int build_local_map(lio_est *e, const std::function<int()> &before_sync =
     EST_CUDA(cudaEventRecord(e->ev_map, st));
     EST_CUDA(cudaStreamWaitEvent(e->ostream, e->ev_map, 0));
     EST_CUDA(cudaMemsetAsync(e->d_odom, 0, sizeof(OdomState), e->ostream));
-    rc = odom_rounds(0, odom_first, e->ostream);
+    rc = rounds(0, odom_first, e->ostream);
     if (rc != LIO_OK) return rc;
     EST_CUDA(cudaEventRecord(e->ev_odom, e->ostream));
   }
@@ -1352,7 +1303,7 @@ static int build_local_map(lio_est *e, const std::function<int()> &before_sync =
   rc = readback();
   if (rc != LIO_OK) return rc;
   if (odom && odom_first < odom_total && !e->h_counts[W + 8]) {   // not converged yet (rare): the rest of the chain, one more synchronisation
-    rc = odom_rounds(odom_first, odom_total, st);
+    rc = rounds(odom_first, odom_total, st);
     if (rc != LIO_OK) return rc;
     rc = readback();
     if (rc != LIO_OK) return rc;
@@ -2786,30 +2737,15 @@ extern "C" int lio_ppp_evaluate_batch_host(const float *pts4, const float *coef4
   LIO_CUDA_OK(cudaSetDevice(device));
   double Rt[12], M[108];
   ppp_frame_terms(pose_pivot, pose_i, pose_ex, Rt, Rt + 9, M);
+  DevBufs d;
   float4 *dp = nullptr, *dc = nullptr;
   double *dRt = nullptr, *dM = nullptr, *dr = nullptr, *dJ = nullptr;
-  int rc = LIO_OK;
-  if (cudaMalloc(&dp, sizeof(float4) * n) != cudaSuccess || cudaMalloc(&dc, sizeof(float4) * n) != cudaSuccess ||
-      cudaMalloc(&dRt, sizeof(Rt)) != cudaSuccess || cudaMalloc(&dM, sizeof(M)) != cudaSuccess ||
-      cudaMalloc(&dr, sizeof(double) * n) != cudaSuccess || cudaMalloc(&dJ, sizeof(double) * 18 * (size_t)n) != cudaSuccess) {
-    lio_set_last_error(__FILE__, __LINE__, "cudaMalloc failed");
-    rc = LIO_ERR_CUDA;
-  }
-  if (rc == LIO_OK) {
-    cudaMemcpy(dp, pts4, sizeof(float4) * n, cudaMemcpyHostToDevice);
-    cudaMemcpy(dc, coef4, sizeof(float4) * n, cudaMemcpyHostToDevice);
-    cudaMemcpy(dRt, Rt, sizeof(Rt), cudaMemcpyHostToDevice);
-    cudaMemcpy(dM, M, sizeof(M), cudaMemcpyHostToDevice);
-    rc = ppp_rows_launch(dp, dc, n, dRt, dM, dr, dJ, 0);
-    if (rc == LIO_OK) {
-      cudaError_t er = cudaMemcpy(r_out, dr, sizeof(double) * n, cudaMemcpyDeviceToHost);
-      if (er == cudaSuccess) er = cudaMemcpy(J_out, dJ, sizeof(double) * 18 * (size_t)n, cudaMemcpyDeviceToHost);
-      if (er != cudaSuccess) { lio_set_last_error(__FILE__, __LINE__, cudaGetErrorString(er)); rc = LIO_ERR_CUDA; }
-    }
-  }
-  void *fr[] = {dp, dc, dRt, dM, dr, dJ};
-  for (void *q : fr) if (q) cudaFree(q);
-  return rc;
+  if (!d.alloc(&dp, n) || !d.alloc(&dc, n) || !d.alloc(&dRt, 12) || !d.alloc(&dM, 108) || !d.alloc(&dr, n) || !d.alloc(&dJ, 18 * (size_t)n) ||
+      !d.up(dp, (const float4 *)pts4, n) || !d.up(dc, (const float4 *)coef4, n) || !d.up(dRt, Rt, 12) || !d.up(dM, M, 108))
+    return LIO_ERR_CUDA;
+  const int rc = ppp_rows_launch(dp, dc, n, dRt, dM, dr, dJ, 0);
+  if (rc != LIO_OK) return rc;
+  return d.down(r_out, dr, n) && d.down(J_out, dJ, 18 * (size_t)n) ? LIO_OK : LIO_ERR_CUDA;
 }
 
 // Stage C reduction of ONE frame on explicit host arrays (parity entry for the fused kernel):
@@ -2819,39 +2755,29 @@ extern "C" int lio_asm_ppp_host(const float *pts4, const float *coef4, int n, co
   if (!pts4 || !coef4 || n < 0 || !R9 || !t3 || !out32) return LIO_ERR_INVALID;
   if (lio_device_count() <= 0) return LIO_ERR_NO_DEVICE;
   LIO_CUDA_OK(cudaSetDevice(device));
+  DevBufs d;
   AsmWork w;
   float4 *dp = nullptr, *dc = nullptr;
+  double *dRt = nullptr;
+  double Rt[kAsmRtStride] = {};
+  std::memcpy(Rt, R9, sizeof(double) * 9); std::memcpy(Rt + 9, t3, sizeof(double) * 3);
   int rc = LIO_OK;
   const int nn = n > 0 ? n : 1;
-  if (w.init(nn) != 0 || cudaMalloc(&dp, sizeof(float4) * nn) != cudaSuccess || cudaMalloc(&dc, sizeof(float4) * nn) != cudaSuccess) {
-    lio_set_last_error(__FILE__, __LINE__, "cudaMalloc failed");
+  if (w.init(nn) != 0) { lio_set_last_error(__FILE__, __LINE__, "cudaMalloc failed"); rc = LIO_ERR_CUDA; }
+  else if (!d.alloc(&dp, nn) || !d.alloc(&dc, nn) || !d.alloc(&dRt, kAsmRtStride) || !d.up(dp, (const float4 *)pts4, n) ||
+           !d.up(dc, (const float4 *)coef4, n) || !d.up(dRt, Rt, kAsmRtStride))
     rc = LIO_ERR_CUDA;
-  }
   if (rc == LIO_OK) {
-    cudaMemcpy(dp, pts4, sizeof(float4) * n, cudaMemcpyHostToDevice);
-    cudaMemcpy(dc, coef4, sizeof(float4) * n, cudaMemcpyHostToDevice);
     AsmParams ap;
     std::memset(&ap, 0, sizeof(ap));
     ap.nframes = 1;
     ap.f[0].pts = dp; ap.f[0].coef = dc; ap.f[0].n = n;
-    double Rt[kAsmRtStride];
-    std::memcpy(Rt, R9, sizeof(double) * 9); std::memcpy(Rt + 9, t3, sizeof(double) * 3);
-    double *dRt = nullptr;
-    cudaMalloc(&dRt, sizeof(Rt));
-    cudaMemcpy(dRt, Rt, sizeof(Rt), cudaMemcpyHostToDevice);
     int sms = 132;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
     asm_plan(ap, sms);
     rc = asm_launch(ap, dRt, w, 0, nullptr);
-    cudaDeviceSynchronize();
-    cudaFree(dRt);
-    if (rc == LIO_OK) {
-      cudaError_t er = cudaMemcpy(out32, w.out, sizeof(double) * kAsmStride, cudaMemcpyDeviceToHost);
-      if (er != cudaSuccess) { lio_set_last_error(__FILE__, __LINE__, cudaGetErrorString(er)); rc = LIO_ERR_CUDA; }
-    }
+    if (rc == LIO_OK && (!d.ok(cudaDeviceSynchronize()) || !d.down(out32, w.out, kAsmStride))) rc = LIO_ERR_CUDA;
   }
-  if (dp) cudaFree(dp);
-  if (dc) cudaFree(dc);
   w.destroy();
   return rc;
 }
@@ -2876,31 +2802,20 @@ __global__ void k_fill_features(float4 *pts, float4 *coef, long long n, long lon
   coef[i] = make_float4(wx, wy, wz, (float)(-r0) + 0.08f * (a - 0.5f));
 }
 
-// Streaming-rate measurement of the fused stage-C kernel on a synthetic feature stream of n features
-// (choose n*32 B larger than L2 to measure the HBM-resident rate).  CUDA events around each launch on the
-// launching stream.  out = {avg ms per launch, min ms, bytes per launch, launches}.
 // ---- C-ABI: TransformToEnd on an explicit host array (parity entry) ----------------------------------------------
 extern "C" int lio_transform_to_end_host(float *cloud, int n, const float *tf7_es, float time_factor, int device) {
   if (!cloud || !tf7_es || n < 0) return LIO_ERR_INVALID;
   if (lio_device_count() <= 0) return LIO_ERR_NO_DEVICE;
   LIO_CUDA_OK(cudaSetDevice(device));
   if (n == 0) return LIO_OK;
+  DevBufs db;
   float4 *d = nullptr;
   int *dn = nullptr;
-  LIO_CUDA_OK(cudaMalloc(&d, sizeof(float4) * n));
-  cudaError_t ce = cudaMalloc(&dn, sizeof(int));
-  if (ce == cudaSuccess) ce = cudaMemcpy(d, cloud, sizeof(float4) * n, cudaMemcpyHostToDevice);
-  if (ce == cudaSuccess) ce = cudaMemcpy(dn, &n, sizeof(int), cudaMemcpyHostToDevice);
-  if (ce == cudaSuccess) {
-    TransformF es;
-    std::memcpy(&es, tf7_es, sizeof(es));
-    k_deskew<<<(n + 255) / 256, 256>>>(d, dn, es, time_factor);
-    ce = cudaMemcpy(cloud, d, sizeof(float4) * n, cudaMemcpyDeviceToHost);
-  }
-  cudaFree(d);
-  if (dn) cudaFree(dn);
-  if (ce != cudaSuccess) { lio_set_last_error(__FILE__, __LINE__, cudaGetErrorString(ce)); return LIO_ERR_CUDA; }
-  return LIO_OK;
+  if (!db.alloc(&d, n) || !db.alloc(&dn, 1) || !db.up(d, (const float4 *)cloud, n) || !db.up(dn, &n, 1)) return LIO_ERR_CUDA;
+  TransformF es;
+  std::memcpy(&es, tf7_es, sizeof(es));
+  k_deskew<<<(n + 255) / 256, 256>>>(d, dn, es, time_factor);
+  return db.down((float4 *)cloud, d, n) ? LIO_OK : LIO_ERR_CUDA;
 }
 
 // ---- PointMapping::OptimizeTransformTobeMapped (PointMapping.cc:325-753) on device-resident clouds -----------------------
@@ -2941,13 +2856,10 @@ int scan_to_map_run(ScanToMapWork &W, const float4 *d_cmap, int Kc, const float4
   LIO_CUDA_OK(cudaMemcpyAsync(W.d_tf, tf7, sizeof(TransformF), cudaMemcpyHostToDevice, st));
   LIO_CUDA_OK(cudaMemsetAsync(W.d_odom, 0, sizeof(OdomState), st));
   {  // point_on_z_axis_ = T0 * (0, 0, 10), fixed for the whole optimisation (PointMapping.cc:803-806); float, no FMA
-    const float qx = tf7[0], qy = tf7[1], qz = tf7[2], qw = tf7[3], vx = 0.0f, vy = 0.0f, vz = 10.0f;
-    volatile float ux = qy * vz - qz * vy, uy = qz * vx - qx * vz, uz = qx * vy - qy * vx;
-    volatile float ux2 = ux + ux, uy2 = uy + uy, uz2 = uz + uz;
-    volatile float cx = qy * uz2 - qz * uy2, cy = qz * ux2 - qx * uz2, cz = qx * uy2 - qy * ux2;
-    volatile float ax = ux2 * qw, ay = uy2 * qw, az = uz2 * qw;
-    volatile float rx = vx + ax, ry = vy + ay, rz = vz + az;
-    volatile float sx = rx + cx, sy = ry + cy, sz = rz + cz;
+    TwistF t0;
+    t0.qx = tf7[0]; t0.qy = tf7[1]; t0.qz = tf7[2]; t0.qw = tf7[3];
+    float sx, sy, sz;
+    rotate_host(t0, 0.0f, 0.0f, 10.0f, sx, sy, sz);
     const float hz[4] = {sx + tf7[4], sy + tf7[5], sz + tf7[6], 0.f};
     LIO_CUDA_OK(cudaMemcpyAsync(W.d_z, hz, sizeof(hz), cudaMemcpyHostToDevice, st));
     LIO_CUDA_OK(cudaStreamSynchronize(st));   // hn / hz are stack variables
@@ -2995,44 +2907,33 @@ extern "C" int lio_scan_to_map_host(const float *corner_map, int Kc, const float
   if (n_out) *n_out = 0;
   if (iters) *iters = 0;
   if (Kc <= 10 || Ks <= 100 || max_iter == 0) return LIO_OK;  // PointMapping.cc:327-329: nothing to optimise against
+  DevBufs d;
   ScanToMapWork W;
   float4 *d_cmap = nullptr, *d_smap = nullptr, *d_corner = nullptr, *d_surf = nullptr;
   int *d_cnt = nullptr;
   int rc = LIO_OK, sm = 132;
   cudaDeviceGetAttribute(&sm, cudaDevAttrMultiProcessorCount, device);
-  auto alloc = [&](void **p, size_t bytes) { return cudaMalloc(p, bytes ? bytes : 16) == cudaSuccess; };
-  if (W.init(Kc, Ks, Mc + Ms) != 0 || !(alloc((void **)&d_cmap, sizeof(float4) * Kc) && alloc((void **)&d_smap, sizeof(float4) * Ks) &&
-                                         alloc((void **)&d_corner, sizeof(float4) * Mc) && alloc((void **)&d_surf, sizeof(float4) * Ms) &&
-                                         alloc((void **)&d_cnt, sizeof(int) * 2))) {
-    lio_set_last_error(__FILE__, __LINE__, "cudaMalloc failed");
+  const int hn[2] = {Mc, Ms};
+  if (W.init(Kc, Ks, Mc + Ms) != 0) { lio_set_last_error(__FILE__, __LINE__, "cudaMalloc failed"); rc = LIO_ERR_CUDA; }
+  else if (!d.alloc(&d_cmap, Kc) || !d.alloc(&d_smap, Ks) || !d.alloc(&d_corner, Mc) || !d.alloc(&d_surf, Ms) || !d.alloc(&d_cnt, 2) ||
+           !d.up(d_cmap, (const float4 *)corner_map, Kc) || !d.up(d_smap, (const float4 *)surf_map, Ks) ||
+           !d.up(d_corner, (const float4 *)corner, Mc) || !d.up(d_surf, (const float4 *)surf, Ms) || !d.up(d_cnt, hn, 2))
     rc = LIO_ERR_CUDA;
-  }
-  if (rc == LIO_OK) {
-    const int hn[2] = {Mc, Ms};
-    cudaMemcpy(d_cmap, corner_map, sizeof(float4) * Kc, cudaMemcpyHostToDevice);
-    cudaMemcpy(d_smap, surf_map, sizeof(float4) * Ks, cudaMemcpyHostToDevice);
-    if (Mc) cudaMemcpy(d_corner, corner, sizeof(float4) * Mc, cudaMemcpyHostToDevice);
-    if (Ms) cudaMemcpy(d_surf, surf, sizeof(float4) * Ms, cudaMemcpyHostToDevice);
-    cudaMemcpy(d_cnt, hn, sizeof(hn), cudaMemcpyHostToDevice);
-    int m = 0;
+  int m = 0;
+  if (rc == LIO_OK)
     rc = scan_to_map_run(W, d_cmap, Kc, d_smap, Ks, d_corner, d_cnt, Mc, d_surf, d_cnt + 1, Ms, tf7, min_match_sq_dis, min_plane_dis, max_iter,
                          delta_r_abort, delta_t_abort, variant, &m, iters, sm, 0);
-    if (rc == LIO_OK) {
-      if (n_out) *n_out = m;
-      if (m > 0) {
-        if (pts4) cudaMemcpy(pts4, W.fo.pts, sizeof(float4) * m, cudaMemcpyDeviceToHost);
-        if (coef4) cudaMemcpy(coef4, W.fo.coef, sizeof(float4) * m, cudaMemcpyDeviceToHost);
-        if (src) cudaMemcpy(src, W.fo.src, sizeof(int) * m, cudaMemcpyDeviceToHost);
-      }
-    }
+  if (rc == LIO_OK) {
+    if (n_out) *n_out = m;
+    if ((pts4 && !d.down((float4 *)pts4, W.fo.pts, m)) || (coef4 && !d.down((float4 *)coef4, W.fo.coef, m)) || (src && !d.down(src, W.fo.src, m)))
+      rc = LIO_ERR_CUDA;
   }
-  void *fr[] = {d_cmap, d_smap, d_corner, d_surf, d_cnt};
-  for (void *q : fr) if (q) cudaFree(q);
   W.destroy();
   return rc;
 }
 
 // ---- C-ABI: Estimator::CalculateLaserOdom on explicit host arrays (parity entry) ---------------------------------
+// Runs the estimator's own round driver (odom_rounds): without keep_features the batched k-NN launch and the fused k_odom_round.
 extern "C" int lio_laser_odom_host(const float *map, int K, const float *surf, int M, float *tf7, float min_match_sq_dis,
                                    float min_plane_dis, int keep_features, int max_iter, float *pts4, float *coef4, int32_t *src,
                                    int *n_out, int *iters, int device) {
@@ -3043,6 +2944,7 @@ extern "C" int lio_laser_odom_host(const float *map, int K, const float *surf, i
   if (iters) *iters = 0;
   if (M == 0 || max_iter == 0) return LIO_OK;
   const int cap = M * (keep_features ? max_iter : 1);
+  DevBufs d;
   CellHash h;
   KnnWork w;
   float4 *d_map = nullptr, *d_surf = nullptr;
@@ -3054,53 +2956,31 @@ extern "C" int lio_laser_odom_host(const float *map, int K, const float *surf, i
   int rc = LIO_OK, sm = 132;
   cudaDeviceGetAttribute(&sm, cudaDevAttrMultiProcessorCount, device);
   const int Kc = K > 0 ? K : 1;
-  if (h.init(Kc) != 0 || w.init(M) != 0) rc = LIO_ERR_CUDA;
-  if (rc == LIO_OK && (cudaMalloc(&d_map, sizeof(float4) * Kc) != cudaSuccess || cudaMalloc(&d_surf, sizeof(float4) * M) != cudaSuccess ||
-                       cudaMalloc(&fo.pts, sizeof(float4) * cap) != cudaSuccess || cudaMalloc(&fo.coef, sizeof(float4) * cap) != cudaSuccess ||
-                       cudaMalloc(&fo.src, sizeof(int) * cap) != cudaSuccess || cudaMalloc(&d_n, sizeof(int) * 4) != cudaSuccess ||
-                       cudaMalloc(&d_tf, sizeof(TransformF)) != cudaSuccess || cudaMalloc(&d_odom, sizeof(OdomState)) != cudaSuccess ||
-                       cudaMalloc(&d_partial, sizeof(double) * 32 * 1024) != cudaSuccess))
+  const int hn[3] = {K, M, 0};
+  if (h.init(Kc) != 0 || w.init(M) != 0) { lio_set_last_error(__FILE__, __LINE__, "cudaMalloc failed"); rc = LIO_ERR_CUDA; }
+  else if (!d.alloc(&d_map, Kc) || !d.alloc(&d_surf, M) || !d.alloc(&fo.pts, cap) || !d.alloc(&fo.coef, cap) || !d.alloc(&fo.src, cap) ||
+           !d.alloc(&d_n, 4) || !d.alloc(&d_tf, 1) || !d.alloc(&d_odom, 1) || !d.alloc(&d_partial, 32 * 1024) ||
+           !d.up(d_map, (const float4 *)map, K) || !d.up(d_surf, (const float4 *)surf, M) || !d.up(d_n, hn, 3) ||
+           !d.up(d_tf, (const TransformF *)tf7, 1) || !d.ok(cudaMemset(d_odom, 0, sizeof(OdomState))))
     rc = LIO_ERR_CUDA;
-  if (rc != LIO_OK) lio_set_last_error(__FILE__, __LINE__, "cudaMalloc failed");
   if (rc == LIO_OK) {
-    const int hn[3] = {K, M, 0};
-    cudaMemcpy(d_map, map, sizeof(float4) * K, cudaMemcpyHostToDevice);
-    cudaMemcpy(d_surf, surf, sizeof(float4) * M, cudaMemcpyHostToDevice);
-    cudaMemcpy(d_n, hn, sizeof(hn), cudaMemcpyHostToDevice);
-    cudaMemcpy(d_tf, tf7, sizeof(TransformF), cudaMemcpyHostToDevice);
-    cudaMemset(d_odom, 0, sizeof(OdomState));
     fo.count = d_n + 2; fo.cap = cap;
     const float cell = sqrtf(min_match_sq_dis) * (1.0f + 1.0f / 1024.0f);
     rc = h.build(d_map, d_n, Kc, cell, 0, nullptr);
-    const int nb = std::max(1, std::min(sm, (cap + kOdomThreads - 1) / kOdomThreads));
-    for (int it = 0; it < max_iter && rc == LIO_OK; ++it) {
-      rc = calculate_features_dev(h, d_map, d_surf, d_n + 1, M, d_tf, min_match_sq_dis, min_plane_dis, fo, keep_features ? 1 : 0,
-                                  &d_odom->done, w, 0, nullptr);
-      if (rc != LIO_OK) break;
-      k_odom_reduce<<<nb, kOdomThreads>>>(fo.pts, fo.coef, fo.count, d_tf, d_odom, d_partial);
-      k_odom_solve<<<1, 32>>>(d_odom, d_tf, 0.05, 0.05);
-    }
-    if (rc == LIO_OK) {
-      int m = 0;
-      OdomState hs;
-      cudaError_t ce = cudaMemcpy(&m, d_n + 2, sizeof(int), cudaMemcpyDeviceToHost);
-      if (ce == cudaSuccess) ce = cudaMemcpy(&hs, d_odom, sizeof(OdomState), cudaMemcpyDeviceToHost);
-      if (ce == cudaSuccess) ce = cudaMemcpy(tf7, d_tf, sizeof(TransformF), cudaMemcpyDeviceToHost);
-      if (ce != cudaSuccess) { lio_set_last_error(__FILE__, __LINE__, cudaGetErrorString(ce)); rc = LIO_ERR_CUDA; }
-      else if (m > cap) { lio_set_last_error(__FILE__, __LINE__, "feature buffer overflow"); rc = LIO_ERR_CAPACITY; }
-      else {
-        *n_out = m;
-        if (iters) *iters = hs.iter;
-        if (m > 0) {
-          if (pts4) cudaMemcpy(pts4, fo.pts, sizeof(float4) * m, cudaMemcpyDeviceToHost);
-          if (coef4) cudaMemcpy(coef4, fo.coef, sizeof(float4) * m, cudaMemcpyDeviceToHost);
-          if (src) cudaMemcpy(src, fo.src, sizeof(int) * m, cudaMemcpyDeviceToHost);
-        }
-      }
-    }
+    if (rc == LIO_OK)
+      rc = odom_rounds(h, d_surf, d_n + 1, M, d_tf, fo, keep_features != 0, d_odom, d_partial, w, min_match_sq_dis, min_plane_dis, 0, max_iter,
+                       sm, 0, nullptr);
   }
-  void *fr[] = {d_map, d_surf, fo.pts, fo.coef, fo.src, d_n, d_tf, d_odom, d_partial};
-  for (void *q : fr) if (q) cudaFree(q);
+  int m = 0;
+  OdomState hs;
+  if (rc == LIO_OK && (!d.down(&m, d_n + 2, 1) || !d.down(&hs, d_odom, 1) || !d.down((TransformF *)tf7, d_tf, 1))) rc = LIO_ERR_CUDA;
+  if (rc == LIO_OK && m > cap) { lio_set_last_error(__FILE__, __LINE__, "feature buffer overflow"); rc = LIO_ERR_CAPACITY; }
+  if (rc == LIO_OK) {
+    *n_out = m;
+    if (iters) *iters = hs.iter;
+    if ((pts4 && !d.down((float4 *)pts4, fo.pts, m)) || (coef4 && !d.down((float4 *)coef4, fo.coef, m)) || (src && !d.down(src, fo.src, m)))
+      rc = LIO_ERR_CUDA;
+  }
   h.destroy();
   w.destroy();
   return rc;
@@ -3111,6 +2991,9 @@ extern "C" int lio_asm_set_fold_chunks(int chunks) {
   return LIO_OK;
 }
 
+// Streaming-rate measurement of the fused stage-C kernel on a synthetic feature stream of n features
+// (choose n*32 B larger than L2 to measure the HBM-resident rate).  CUDA events around each launch on the
+// launching stream.  out = {avg ms per launch, min ms, bytes per launch, launches}.
 extern "C" int lio_asm_stream_bench(long long n_features, int iters, int device, double out[4]) {
   if (n_features <= 0 || iters <= 0 || !out) return LIO_ERR_INVALID;
   if (lio_device_count() <= 0) return LIO_ERR_NO_DEVICE;
@@ -3118,31 +3001,30 @@ extern "C" int lio_asm_stream_bench(long long n_features, int iters, int device,
   const int O = 8;  // spread over 8 equal frames like a window
   const long long per = n_features / O;
   if (per <= 0 || per > 0x7fffffffLL) return LIO_ERR_INVALID;
+  DevBufs d;
   float4 *dp = nullptr, *dc = nullptr;
-  AsmWork w;
-  int rc = LIO_OK;
-  if (cudaMalloc(&dp, sizeof(float4) * per * O) != cudaSuccess || cudaMalloc(&dc, sizeof(float4) * per * O) != cudaSuccess ||
-      w.init((int)std::min<long long>(per * O, 1ll << 30)) != 0) {
-    lio_set_last_error(__FILE__, __LINE__, "cudaMalloc failed");
-    rc = LIO_ERR_CUDA;
-  }
-  cudaEvent_t e0 = nullptr, e1 = nullptr;
   double *dRt = nullptr;
+  AsmWork w;
+  cudaEvent_t e0 = nullptr, e1 = nullptr;
+  AsmParams ap;
+  std::memset(&ap, 0, sizeof(ap));
+  ap.nframes = O;
+  double hRt[8 * kAsmRtStride];
+  int rc = LIO_OK;
+  if (!d.alloc(&dp, per * O) || !d.alloc(&dc, per * O)) rc = LIO_ERR_CUDA;
+  else if (w.init((int)std::min<long long>(per * O, 1ll << 30)) != 0) { lio_set_last_error(__FILE__, __LINE__, "cudaMalloc failed"); rc = LIO_ERR_CUDA; }
   if (rc == LIO_OK) {
     k_fill_features<<<(unsigned)((per * O + 255) / 256), 256>>>(dp, dc, per * O, per);
-    cudaEventCreate(&e0); cudaEventCreate(&e1);
-    AsmParams ap;
-    std::memset(&ap, 0, sizeof(ap));
-    ap.nframes = O;
-    double hRt[8 * kAsmRtStride];
     for (int k = 0; k < O; ++k) {
       ap.f[k].pts = dp + per * k; ap.f[k].coef = dc + per * k; ap.f[k].n = (int)per;
       const double c = std::cos(0.01 * k), s = std::sin(0.01 * k);
       const double Rt[kAsmRtStride] = {c, -s, 0, s, c, 0, 0, 0, 1, 0.1 * k, 0.02 * k, 0.0};
       std::memcpy(hRt + k * kAsmRtStride, Rt, sizeof(Rt));
     }
-    cudaMalloc(&dRt, sizeof(hRt));
-    cudaMemcpy(dRt, hRt, sizeof(hRt), cudaMemcpyHostToDevice);
+    if (!d.ok(cudaEventCreate(&e0)) || !d.ok(cudaEventCreate(&e1)) || !d.alloc(&dRt, 8 * kAsmRtStride) || !d.up(dRt, hRt, 8 * kAsmRtStride))
+      rc = LIO_ERR_CUDA;
+  }
+  if (rc == LIO_OK) {
     int sms = 132;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
     asm_plan(ap, sms);
@@ -3160,9 +3042,6 @@ extern "C" int lio_asm_stream_bench(long long n_features, int iters, int device,
   }
   if (e0) cudaEventDestroy(e0);
   if (e1) cudaEventDestroy(e1);
-  if (dRt) cudaFree(dRt);
-  if (dp) cudaFree(dp);
-  if (dc) cudaFree(dc);
   w.destroy();
   return rc;
 }

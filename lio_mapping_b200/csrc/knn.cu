@@ -20,6 +20,7 @@
 //               registers, 5x3 column-pivoted Householder QR plane fit, validity / score / FOV
 //               tests, ordered compaction of accepted features by decoupled look-back
 #include "knn.cuh"
+#include "odom.cuh"
 #include "qr.cuh"
 #include <vector>
 
@@ -142,15 +143,6 @@ int CellHash::build(const float4 *map, const int *n_dev, int n_max, float cell_s
   return LIO_OK;
 }
 
-// Eigen quaternion * vector, then + pos (PointAssociateToMap)
-__device__ __forceinline__ void assoc_to_map(const TransformF &t, float vx, float vy, float vz, float &ox, float &oy, float &oz) {
-  float ux = t.qy * vz - t.qz * vy, uy = t.qz * vx - t.qx * vz, uz = t.qx * vy - t.qy * vx;
-  ux += ux; uy += uy; uz += uz;
-  float cx = t.qy * uz - t.qz * uy, cy = t.qz * ux - t.qx * uz, cz = t.qx * uy - t.qy * ux;
-  float rx = vx + ux * t.qw + cx, ry = vy + uy * t.qw + cy, rz = vz + uz * t.qw + cz;
-  ox = rx + t.px; oy = ry + t.py; oz = rz + t.pz;
-}
-
 // (d^2, map index) packed so that unsigned order == the oracle's total order (d^2 >= 0)
 __device__ __forceinline__ unsigned long long pack_key(float d, int mi) {
   return ((unsigned long long)__float_as_uint(d) << 32) | (unsigned)mi;
@@ -263,7 +255,8 @@ knn_plane(const KnnBatch B, const unsigned long long *__restrict__ hkeys, const 
   const int ql = threadIdx.x / kGroup;
   if (active) {
     p = __ldg(F.surf + q);
-    assoc_to_map(tf, p.x, p.y, p.z, sx, sy, sz);
+    odom_qmul_vec(tf.qx, tf.qy, tf.qz, tf.qw, p.x, p.y, p.z, sx, sy, sz);   // PointAssociateToMap
+    sx += tf.px; sy += tf.py; sz += tf.pz;
     const int cx = (int)floorf(sx * inv_cell), cy = (int)floorf(sy * inv_cell), cz = (int)floorf(sz * inv_cell);
     unsigned long long key4[4], got4[4];
     unsigned s4[4];
@@ -403,7 +396,7 @@ knn_plane(const KnnBatch B, const unsigned long long *__restrict__ hkeys, const 
         const float s = 1.f - 0.9f * fabsf(pd2) / sqrtf(dist);
         float zx, zy, zz;
         if (F.zaxis) { zx = F.zaxis[0]; zy = F.zaxis[1]; zz = F.zaxis[2]; }
-        else assoc_to_map(tf, 0.0f, 0.0f, 10.0f, zx, zy, zz);
+        else { odom_qmul_vec(tf.qx, tf.qy, tf.qz, tf.qw, 0.0f, 0.0f, 10.0f, zx, zy, zz); zx += tf.px; zy += tf.py; zz += tf.pz; }
         const float e0 = tf.px - sx, e1 = tf.py - sy, e2 = tf.pz - sz;
         const float squared_side1 = e0 * e0 + e1 * e1 + e2 * e2;
         const float f0 = zx - sx, f1 = zy - sy, f2 = zz - sz;
@@ -464,7 +457,7 @@ knn_plane(const KnnBatch B, const unsigned long long *__restrict__ hkeys, const 
         const float s = 1.f - 0.9f * fabsf(ld2);
         float zx, zy, zz;
         if (F.zaxis) { zx = F.zaxis[0]; zy = F.zaxis[1]; zz = F.zaxis[2]; }
-        else assoc_to_map(tf, 0.0f, 0.0f, 10.0f, zx, zy, zz);
+        else { odom_qmul_vec(tf.qx, tf.qy, tf.qz, tf.qw, 0.0f, 0.0f, 10.0f, zx, zy, zz); zx += tf.px; zy += tf.py; zz += tf.pz; }
         const float e0 = tf.px - sx, e1 = tf.py - sy, e2 = tf.pz - sz;
         const float squared_side1 = e0 * e0 + e1 * e1 + e2 * e2;
         const float f0 = zx - sx, f1 = zy - sy, f2 = zz - sz;
@@ -562,96 +555,91 @@ int calculate_features_dev(const CellHash &h, const float4 *map, const float4 *s
 
 }  // namespace lio
 
-// ---- C-ABI: Estimator::CalculateFeatures on explicit host arrays (parity entry) -----------------
+// ---- C-ABI: Estimator::CalculateFeatures on explicit host arrays (parity entries) and the test seams of the production
+// CellHash::build and calculate_features_batch on host buffers ---------------------------------------------------------
 using namespace lio;
 
-static int calculate_features_host_impl(const float *map, int K, const float *surf, int M, const float *tf7,
-                                        float min_match_sq_dis, float min_plane_dis, float *pts4, float *coef4, int32_t *src,
-                                        int *n_out, int device, int fit);
-
-extern "C" int lio_calculate_features_host(const float *map, int K, const float *surf, int M, const float *tf7,
-                                           float min_match_sq_dis, float min_plane_dis, float *pts4, float *coef4, int32_t *src,
-                                           int *n_out, int device) {
-  return calculate_features_host_impl(map, K, surf, M, tf7, min_match_sq_dis, min_plane_dis, pts4, coef4, src, n_out, device, 0);
-}
-
-extern "C" int lio_calculate_line_features_host(const float *corner_map, int K, const float *corner, int M, const float *tf7,
-                                                float min_match_sq_dis, float *pts4, float *coef4, int32_t *src, int *n_out,
-                                                int device) {
-  return calculate_features_host_impl(corner_map, K, corner, M, tf7, min_match_sq_dis, 0.f, pts4, coef4, src, n_out, device, 1);
-}
-
-static int calculate_features_host_impl(const float *map, int K, const float *surf, int M, const float *tf7,
-                                        float min_match_sq_dis, float min_plane_dis, float *pts4, float *coef4, int32_t *src,
-                                        int *n_out, int device, int fit) {
-  const int per = fit == 1 ? 2 : 1;
-  if (!map || !surf || !tf7 || !n_out || K < 0 || M < 0) return LIO_ERR_INVALID;
-  if (lio_device_count() <= 0) return LIO_ERR_NO_DEVICE;
-  LIO_CUDA_OK(cudaSetDevice(device));
-  *n_out = 0;
-  if (M == 0) return LIO_OK;
+// lio_calculate_features_batch_host behind its argument checks: one cell hash over map, one batched launch, then every
+// frame's outputs and count back to the host.  src_cat may be null (the one-frame entries): the source indices stay on the device.
+static int features_batch_host(const float *map, int K, float cell_size, float min_match_sq_dis, float min_plane_dis, int nframes,
+                               const float *surf_cat, const int *n_per_frame, const int *n_bound_per_frame, const float *tf7_per_frame,
+                               const int *append_per_frame, const float *zaxis3, int fit, int done_flag_value, int work_queries,
+                               const int *out_cap_per_frame, float *pts4_cat, float *coef4_cat, int32_t *src_cat, int *count_per_frame) {
+  size_t n_tot = 0, cap_tot = 0;
+  for (int k = 0; k < nframes; ++k) { n_tot += n_per_frame[k]; cap_tot += out_cap_per_frame[k]; }
+  std::vector<int> hn(2 + 2 * nframes);   // on the device as d_n: K, done flag, then per frame {n, count}
+  hn[0] = K; hn[1] = done_flag_value > 0 ? 1 : 0;
+  for (int k = 0; k < nframes; ++k) { hn[2 + 2 * k] = n_per_frame[k]; hn[3 + 2 * k] = count_per_frame[k]; }
+  DevBufs d;
   CellHash h;
   KnnWork w;
-  float4 *d_map = nullptr, *d_surf = nullptr;
-  FeatureOut fo;
-  int *d_n = nullptr;
+  float4 *d_map = nullptr, *d_surf = nullptr, *d_pts = nullptr, *d_coef = nullptr;
+  int *d_src = nullptr, *d_n = nullptr;
   TransformF *d_tf = nullptr;
+  float *d_z = nullptr;
   int rc = LIO_OK;
-  int Kc = K > 0 ? K : 1;
-  if (h.init(Kc) != 0 || w.init(M) != 0) rc = LIO_ERR_CUDA;
-  if (rc == LIO_OK && (cudaMalloc(&d_map, sizeof(float4) * Kc) != cudaSuccess || cudaMalloc(&d_surf, sizeof(float4) * M) != cudaSuccess ||
-                       cudaMalloc(&fo.pts, sizeof(float4) * M * per) != cudaSuccess || cudaMalloc(&fo.coef, sizeof(float4) * M * per) != cudaSuccess ||
-                       cudaMalloc(&fo.src, sizeof(int) * M * per) != cudaSuccess || cudaMalloc(&d_n, sizeof(int) * 4) != cudaSuccess ||
-                       cudaMalloc(&d_tf, sizeof(TransformF)) != cudaSuccess))
+  const int Kc = K > 0 ? K : 1;
+  if (h.init(Kc) != 0 || w.init(work_queries) != 0) { lio_set_last_error(__FILE__, __LINE__, "cudaMalloc failed"); rc = LIO_ERR_CUDA; }
+  else if (!d.alloc(&d_map, Kc) || !d.alloc(&d_surf, n_tot) || !d.alloc(&d_pts, cap_tot) || !d.alloc(&d_coef, cap_tot) ||
+           !d.alloc(&d_src, cap_tot) || !d.alloc(&d_n, hn.size()) || !d.alloc(&d_tf, nframes) || !d.alloc(&d_z, 3) ||
+           !d.up(d_map, (const float4 *)map, K) || !d.up(d_surf, (const float4 *)surf_cat, n_tot) ||
+           !d.up(d_pts, (const float4 *)pts4_cat, cap_tot) || !d.up(d_coef, (const float4 *)coef4_cat, cap_tot) ||
+           (src_cat && !d.up(d_src, src_cat, cap_tot)) || !d.up(d_n, hn.data(), hn.size()) ||
+           !d.up(d_tf, (const TransformF *)tf7_per_frame, nframes) || (zaxis3 && !d.up(d_z, zaxis3, 3)))
     rc = LIO_ERR_CUDA;
   if (rc == LIO_OK) {
-    int hn[3] = {K, M, 0};
-    cudaMemcpy(d_map, map, sizeof(float4) * K, cudaMemcpyHostToDevice);
-    cudaMemcpy(d_surf, surf, sizeof(float4) * M, cudaMemcpyHostToDevice);
-    cudaMemcpy(d_n, hn, sizeof(hn), cudaMemcpyHostToDevice);
-    cudaMemcpy(d_tf, tf7, sizeof(TransformF), cudaMemcpyHostToDevice);
-    fo.count = d_n + 2; fo.cap = M * per;
-    // cell edge >= search radius (with margin, see header)
-    float cell = sqrtf(min_match_sq_dis) * (1.0f + 1.0f / 1024.0f);
-    rc = h.build(d_map, d_n, Kc, cell, 0, nullptr);
-    if (rc == LIO_OK) rc = calculate_features_dev(h, d_map, d_surf, d_n + 1, M, d_tf, min_match_sq_dis, min_plane_dis, fo, 0, nullptr, w, 0, nullptr, fit);
-    if (rc == LIO_OK) {
-      int m = 0;
-      cudaError_t e = cudaMemcpy(&m, d_n + 2, sizeof(int), cudaMemcpyDeviceToHost);
-      if (e != cudaSuccess) { lio_set_last_error(__FILE__, __LINE__, cudaGetErrorString(e)); rc = LIO_ERR_CUDA; }
-      else {
-        *n_out = m;
-        if (m > 0) {
-          cudaMemcpy(pts4, fo.pts, sizeof(float4) * m, cudaMemcpyDeviceToHost);
-          cudaMemcpy(coef4, fo.coef, sizeof(float4) * m, cudaMemcpyDeviceToHost);
-          if (src) cudaMemcpy(src, fo.src, sizeof(int) * m, cudaMemcpyDeviceToHost);
-        }
-      }
+    KnnBatch b;
+    b.nframes = nframes;
+    size_t so = 0, oo = 0;
+    for (int k = 0; k < nframes; ++k) {
+      KnnFrame &f = b.f[k];
+      f.surf = d_surf + so; f.n_dev = d_n + 2 + 2 * k; f.n_bound = n_bound_per_frame[k]; f.tf = d_tf + k;
+      f.out_p = d_pts + oo; f.out_c = d_coef + oo; f.out_src = d_src + oo; f.out_count = d_n + 3 + 2 * k;
+      f.append = append_per_frame[k]; f.tile0 = 0; f.zaxis = zaxis3 ? d_z : nullptr;
+      so += n_per_frame[k]; oo += out_cap_per_frame[k];
     }
-  } else {
-    lio_set_last_error(__FILE__, __LINE__, "cudaMalloc failed");
+    rc = h.build(d_map, d_n, Kc, cell_size, 0, nullptr);
+    if (rc == LIO_OK)
+      rc = calculate_features_batch(h, b, min_match_sq_dis, min_plane_dis, done_flag_value >= 0 ? d_n + 1 : nullptr, w, 0, nullptr, fit);
   }
-  void *fr[] = {d_map, d_surf, fo.pts, fo.coef, fo.src, d_n, d_tf};
-  for (void *q : fr) if (q) cudaFree(q);
+  if (rc == LIO_OK && (!d.down((float4 *)pts4_cat, d_pts, cap_tot) || !d.down((float4 *)coef4_cat, d_coef, cap_tot) ||
+                       (src_cat && !d.down(src_cat, d_src, cap_tot)) || !d.down(hn.data(), d_n, hn.size())))
+    rc = LIO_ERR_CUDA;
+  if (rc == LIO_OK)
+    for (int k = 0; k < nframes; ++k) count_per_frame[k] = hn[3 + 2 * k];
   h.destroy();
   w.destroy();
   return rc;
 }
 
-// ---- C-ABI test seams: the production CellHash::build and calculate_features_batch on host buffers ----------------
+// One frame of the batched launch (fit 0: plane, 1: line), outputs sized M (line: 2 M), src optional
+static int features_one_frame(const float *map, int K, const float *surf, int M, const float *tf7, float min_match_sq_dis,
+                              float min_plane_dis, float *pts4, float *coef4, int32_t *src, int *n_out, int device, int fit) {
+  if (!map || !surf || !tf7 || !n_out || K < 0 || M < 0) return LIO_ERR_INVALID;
+  if (lio_device_count() <= 0) return LIO_ERR_NO_DEVICE;
+  LIO_CUDA_OK(cudaSetDevice(device));
+  *n_out = 0;
+  if (M == 0) return LIO_OK;
+  const float cell = sqrtf(min_match_sq_dis) * (1.0f + 1.0f / 1024.0f);   // cell edge >= search radius (with margin, see header)
+  const int append = 0, cap = M * (fit == 1 ? 2 : 1);
+  int count = 0;
+  const int rc = features_batch_host(map, K, cell, min_match_sq_dis, min_plane_dis, 1, surf, &M, &M, tf7, &append, nullptr, fit, -1, M,
+                                     &cap, pts4, coef4, src, &count);
+  if (rc == LIO_OK) *n_out = count;
+  return rc;
+}
 
-namespace {
-struct DevBufs {   // frees whatever was allocated when the seam returns
-  std::vector<void *> p;
-  template <class T> bool alloc(T **out, size_t n) {
-    void *q = nullptr;
-    if (cudaMalloc(&q, sizeof(T) * (n ? n : 1)) != cudaSuccess) return false;
-    p.push_back(q); *out = (T *)q;
-    return true;
-  }
-  ~DevBufs() { for (void *q : p) cudaFree(q); }
-};
-}  // namespace
+extern "C" int lio_calculate_features_host(const float *map, int K, const float *surf, int M, const float *tf7,
+                                           float min_match_sq_dis, float min_plane_dis, float *pts4, float *coef4, int32_t *src,
+                                           int *n_out, int device) {
+  return features_one_frame(map, K, surf, M, tf7, min_match_sq_dis, min_plane_dis, pts4, coef4, src, n_out, device, 0);
+}
+
+extern "C" int lio_calculate_line_features_host(const float *corner_map, int K, const float *corner, int M, const float *tf7,
+                                                float min_match_sq_dis, float *pts4, float *coef4, int32_t *src, int *n_out,
+                                                int device) {
+  return features_one_frame(corner_map, K, corner, M, tf7, min_match_sq_dis, 0.f, pts4, coef4, src, n_out, device, 1);
+}
 
 extern "C" int lio_cell_hash_build_host(const float *map, int n, int n_max, int cap_points, float cell_size, const float *prev_map,
                                         int prev_n, int *eff_size, unsigned long long *keys, int *count, int *start,
@@ -666,27 +654,21 @@ extern "C" int lio_cell_hash_build_host(const float *map, int n, int n_max, int 
   float4 *d_map = nullptr;
   int *d_n = nullptr;
   int rc = LIO_OK;
-  if (h.init(cap_points) != 0 || !d.alloc(&d_map, cap_points) || !d.alloc(&d_n, 1)) {
-    lio_set_last_error(__FILE__, __LINE__, "cudaMalloc failed");
-    rc = LIO_ERR_CUDA;
-  }
+  if (h.init(cap_points) != 0) { lio_set_last_error(__FILE__, __LINE__, "cudaMalloc failed"); rc = LIO_ERR_CUDA; }
+  else if (!d.alloc(&d_map, cap_points) || !d.alloc(&d_n, 1)) rc = LIO_ERR_CUDA;
   if (rc == LIO_OK && prev_n > 0) {   // an earlier, different build leaves its slots, ranges and scan state behind
-    cudaMemcpy(d_map, prev_map, sizeof(float4) * prev_n, cudaMemcpyHostToDevice);
-    cudaMemcpy(d_n, &prev_n, sizeof(int), cudaMemcpyHostToDevice);
-    rc = h.build(d_map, d_n, prev_n, cell_size, 0, nullptr);
+    if (!d.up(d_map, (const float4 *)prev_map, prev_n) || !d.up(d_n, &prev_n, 1)) rc = LIO_ERR_CUDA;
+    else rc = h.build(d_map, d_n, prev_n, cell_size, 0, nullptr);
   }
   if (rc == LIO_OK) {
-    cudaMemcpy(d_map, map, sizeof(float4) * n, cudaMemcpyHostToDevice);
-    cudaMemcpy(d_n, &n, sizeof(int), cudaMemcpyHostToDevice);
-    rc = h.build(d_map, d_n, n_max, cell_size, 0, nullptr);
+    if (!d.up(d_map, (const float4 *)map, n) || !d.up(d_n, &n, 1)) rc = LIO_ERR_CUDA;
+    else rc = h.build(d_map, d_n, n_max, cell_size, 0, nullptr);
   }
   if (rc == LIO_OK) {
     *eff_size = h.eff_size;
-    cudaMemcpy(keys, h.keys, sizeof(unsigned long long) * h.eff_size, cudaMemcpyDeviceToHost);
-    cudaMemcpy(count, h.count, sizeof(int) * h.eff_size, cudaMemcpyDeviceToHost);
-    cudaMemcpy(start, h.start, sizeof(int) * h.eff_size, cudaMemcpyDeviceToHost);
-    cudaError_t e = cudaMemcpy(cellpts, h.cellpts, sizeof(float4) * n, cudaMemcpyDeviceToHost);
-    if (e != cudaSuccess) { lio_set_last_error(__FILE__, __LINE__, cudaGetErrorString(e)); rc = LIO_ERR_CUDA; }
+    if (!d.down(keys, h.keys, h.eff_size) || !d.down(count, h.count, h.eff_size) || !d.down(start, h.start, h.eff_size) ||
+        !d.down((float4 *)cellpts, h.cellpts, n))
+      rc = LIO_ERR_CUDA;
   }
   h.destroy();
   return rc;
@@ -703,66 +685,15 @@ extern "C" int lio_calculate_features_batch_host(const float *map, int K, float 
       fit > 3 || work_queries < 0 || !(cell_size > 0.f))
     return LIO_ERR_INVALID;
   const int per = fit == 1 ? 2 : 1;
-  size_t n_tot = 0, cap_tot = 0;
   for (int k = 0; k < nframes; ++k) {   // the kernel's contracts: *n_dev <= n_bound, and room for every query of the frame
     const int base = append_per_frame[k] ? count_per_frame[k] : 0;
     if (n_per_frame[k] < 0 || n_per_frame[k] > n_bound_per_frame[k] || base < 0 ||
         (long long)base + (long long)per * n_per_frame[k] > out_cap_per_frame[k])
       return LIO_ERR_INVALID;
-    n_tot += n_per_frame[k]; cap_tot += out_cap_per_frame[k];
   }
   if (lio_device_count() <= 0) return LIO_ERR_NO_DEVICE;
   LIO_CUDA_OK(cudaSetDevice(device));
-  DevBufs d;
-  CellHash h;
-  KnnWork w;
-  float4 *d_map = nullptr, *d_surf = nullptr, *d_pts = nullptr, *d_coef = nullptr;
-  int *d_src = nullptr, *d_n = nullptr;   // d_n: K, done flag, then per frame {n, count}
-  TransformF *d_tf = nullptr;
-  float *d_z = nullptr;
-  int rc = LIO_OK;
-  const int Kc = K > 0 ? K : 1;
-  if (h.init(Kc) != 0 || w.init(work_queries) != 0 || !d.alloc(&d_map, Kc) || !d.alloc(&d_surf, n_tot) || !d.alloc(&d_pts, cap_tot) ||
-      !d.alloc(&d_coef, cap_tot) || !d.alloc(&d_src, cap_tot) || !d.alloc(&d_n, 2 + 2 * nframes) || !d.alloc(&d_tf, nframes) ||
-      !d.alloc(&d_z, 3)) {
-    lio_set_last_error(__FILE__, __LINE__, "cudaMalloc failed");
-    rc = LIO_ERR_CUDA;
-  }
-  if (rc == LIO_OK) {
-    std::vector<int> hn(2 + 2 * nframes);
-    hn[0] = K; hn[1] = done_flag_value > 0 ? 1 : 0;
-    for (int k = 0; k < nframes; ++k) { hn[2 + 2 * k] = n_per_frame[k]; hn[3 + 2 * k] = count_per_frame[k]; }
-    cudaMemcpy(d_map, map, sizeof(float4) * K, cudaMemcpyHostToDevice);
-    cudaMemcpy(d_surf, surf_cat, sizeof(float4) * n_tot, cudaMemcpyHostToDevice);
-    cudaMemcpy(d_pts, pts4_cat, sizeof(float4) * cap_tot, cudaMemcpyHostToDevice);
-    cudaMemcpy(d_coef, coef4_cat, sizeof(float4) * cap_tot, cudaMemcpyHostToDevice);
-    cudaMemcpy(d_src, src_cat, sizeof(int) * cap_tot, cudaMemcpyHostToDevice);
-    cudaMemcpy(d_n, hn.data(), sizeof(int) * hn.size(), cudaMemcpyHostToDevice);
-    cudaMemcpy(d_tf, tf7_per_frame, sizeof(TransformF) * nframes, cudaMemcpyHostToDevice);
-    if (zaxis3) cudaMemcpy(d_z, zaxis3, sizeof(float) * 3, cudaMemcpyHostToDevice);
-    KnnBatch b;
-    b.nframes = nframes;
-    size_t so = 0, oo = 0;
-    for (int k = 0; k < nframes; ++k) {
-      KnnFrame &f = b.f[k];
-      f.surf = d_surf + so; f.n_dev = d_n + 2 + 2 * k; f.n_bound = n_bound_per_frame[k]; f.tf = d_tf + k;
-      f.out_p = d_pts + oo; f.out_c = d_coef + oo; f.out_src = d_src + oo; f.out_count = d_n + 3 + 2 * k;
-      f.append = append_per_frame[k]; f.tile0 = 0; f.zaxis = zaxis3 ? d_z : nullptr;
-      so += n_per_frame[k]; oo += out_cap_per_frame[k];
-    }
-    rc = h.build(d_map, d_n, Kc, cell_size, 0, nullptr);
-    if (rc == LIO_OK)
-      rc = calculate_features_batch(h, b, min_match_sq_dis, min_plane_dis, done_flag_value >= 0 ? d_n + 1 : nullptr, w, 0, nullptr, fit);
-    if (rc == LIO_OK) {
-      cudaMemcpy(pts4_cat, d_pts, sizeof(float4) * cap_tot, cudaMemcpyDeviceToHost);
-      cudaMemcpy(coef4_cat, d_coef, sizeof(float4) * cap_tot, cudaMemcpyDeviceToHost);
-      cudaMemcpy(src_cat, d_src, sizeof(int) * cap_tot, cudaMemcpyDeviceToHost);
-      cudaError_t e = cudaMemcpy(hn.data(), d_n, sizeof(int) * hn.size(), cudaMemcpyDeviceToHost);
-      if (e != cudaSuccess) { lio_set_last_error(__FILE__, __LINE__, cudaGetErrorString(e)); rc = LIO_ERR_CUDA; }
-      else for (int k = 0; k < nframes; ++k) count_per_frame[k] = hn[3 + 2 * k];
-    }
-  }
-  h.destroy();
-  w.destroy();
-  return rc;
+  return features_batch_host(map, K, cell_size, min_match_sq_dis, min_plane_dis, nframes, surf_cat, n_per_frame, n_bound_per_frame,
+                             tf7_per_frame, append_per_frame, zaxis3, fit, done_flag_value, work_queries, out_cap_per_frame, pts4_cat,
+                             coef4_cat, src_cat, count_per_frame);
 }

@@ -1320,31 +1320,22 @@ extern "C" int lio_dev_cholesky_solve_host(const double *A, const double *b, int
   LIO_CUDA_OK(cudaSetDevice(device));
   const int NB = (n + 7) / 8;
   const size_t smem = sizeof(double) * ((size_t)(NB * (NB + 1) / 2) * 64 + (size_t)NB * 8);
+  DevBufs d;
   double *dA = nullptr, *db = nullptr, *dx = nullptr;
   int *dok = nullptr;
   long long *dprof = nullptr;
   const size_t nprof = 4 * (size_t)NB + 1, nprof_dev = nprof + 4;   // + 4 in-kernel phase stamps (not returned)
-  int rc = LIO_OK;
-  if (cudaMalloc(&dA, sizeof(double) * n * n) != cudaSuccess || cudaMalloc(&db, sizeof(double) * n) != cudaSuccess ||
-      cudaMalloc(&dx, sizeof(double) * n) != cudaSuccess || cudaMalloc(&dok, sizeof(int)) != cudaSuccess ||
-      cudaMalloc(&dprof, sizeof(long long) * nprof_dev) != cudaSuccess) rc = LIO_ERR_CUDA;
-  if (rc == LIO_OK) {
-    cudaMemcpy(dA, A, sizeof(double) * n * n, cudaMemcpyHostToDevice);
-    cudaMemcpy(db, b, sizeof(double) * n, cudaMemcpyHostToDevice);
-    cudaFuncSetAttribute(k_chol_test, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    cudaMemset(dprof, 0, sizeof(long long) * nprof_dev);
-    k_chol_test<<<1, kDsThreads, smem>>>(dA, db, n, dx, dok, prof ? dprof : nullptr);
-    cudaError_t e = cudaMemcpy(x, dx, sizeof(double) * n, cudaMemcpyDeviceToHost);
-    if (e == cudaSuccess && prof) e = cudaMemcpy(prof, dprof, sizeof(long long) * nprof, cudaMemcpyDeviceToHost);
-    if (e == cudaSuccess && prof) {   // the four %globaltimer stamps become durations (ns) appended behind the per-panel cycles when the caller left room
-      long long st[4];
-      e = cudaMemcpy(st, dprof + nprof, sizeof(st), cudaMemcpyDeviceToHost);
-      if (e == cudaSuccess) std::fprintf(stderr, "[k_chol_test] ns: entry->loop %lld, loop %lld, backsub %lld, total %lld\n", st[1] - st[0], st[2] - st[1], st[3] - st[2], st[3] - st[0]);
-    }
-    if (e == cudaSuccess) e = cudaMemcpy(ok, dok, sizeof(int), cudaMemcpyDeviceToHost);
-    if (e != cudaSuccess) { lio_set_last_error(__FILE__, __LINE__, cudaGetErrorString(e)); rc = LIO_ERR_CUDA; }
-  } else lio_set_last_error(__FILE__, __LINE__, "cudaMalloc failed");
-  void *fr[] = {dA, db, dx, dok, dprof};
-  for (void *q : fr) if (q) cudaFree(q);
-  return rc;
+  if (!d.alloc(&dA, (size_t)n * n) || !d.alloc(&db, n) || !d.alloc(&dx, n) || !d.alloc(&dok, 1) || !d.alloc(&dprof, nprof_dev) ||
+      !d.up(dA, A, (size_t)n * n) || !d.up(db, b, n) ||
+      !d.ok(cudaFuncSetAttribute(k_chol_test, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) ||
+      !d.ok(cudaMemset(dprof, 0, sizeof(long long) * nprof_dev)))
+    return LIO_ERR_CUDA;
+  k_chol_test<<<1, kDsThreads, smem>>>(dA, db, n, dx, dok, prof ? dprof : nullptr);
+  if (!d.down(x, dx, n) || (prof && !d.down(prof, dprof, nprof))) return LIO_ERR_CUDA;
+  if (prof) {   // the four %globaltimer stamps become durations (ns) appended behind the per-panel cycles when the caller left room
+    long long st[4];
+    if (!d.down(st, dprof + nprof, 4)) return LIO_ERR_CUDA;
+    std::fprintf(stderr, "[k_chol_test] ns: entry->loop %lld, loop %lld, backsub %lld, total %lld\n", st[1] - st[0], st[2] - st[1], st[3] - st[2], st[3] - st[0]);
+  }
+  return d.down(ok, dok, 1) ? LIO_OK : LIO_ERR_CUDA;
 }

@@ -19,6 +19,17 @@ inline void quat_to_matrix_normalized(const TwistF &t, float R[9]) {   // rot.no
   R[6] = txz - twy; R[7] = tyz + twx; R[8] = 1.f - (txx + tyy);
 }
 
+// q * v (Eigen _transformVector) in float: the host copy of the device odom_qmul_vec (odom.cuh), its steps volatile so that
+// the host compiler keeps them in the device expression's order.
+inline void rotate_host(const TwistF &t, float vx, float vy, float vz, float &ox, float &oy, float &oz) {
+  volatile float ux = t.qy * vz - t.qz * vy, uy = t.qz * vx - t.qx * vz, uz = t.qx * vy - t.qy * vx;
+  volatile float ux2 = ux + ux, uy2 = uy + uy, uz2 = uz + uz;
+  volatile float cx = t.qy * uz2 - t.qz * uy2, cy = t.qz * ux2 - t.qx * uz2, cz = t.qx * uy2 - t.qy * ux2;
+  volatile float ax = ux2 * t.qw, ay = uy2 * t.qw, az = uz2 * t.qw;
+  volatile float rx = vx + ax, ry = vy + ay, rz = vz + az;
+  ox = rx + cx; oy = ry + cy; oz = rz + cz;
+}
+
 inline void matrix_to_quat(const float m[9], float q[4]) {   // Eigen quaternionbase_assign_impl<Matrix3> (Shepperd); x y z w
   float t = m[0] + m[4] + m[8];
   if (t > 0.f) {

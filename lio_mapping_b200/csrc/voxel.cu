@@ -360,33 +360,22 @@ extern "C" int lio_voxel_grid_host(const float *cloud, int n, float leaf, float 
   LIO_CUDA_OK(cudaSetDevice(device));
   *n_out = 0;
   if (n == 0) return LIO_OK;
+  DevBufs d;
   VoxelGrid vg;
-  if (vg.init(n) != 0) { vg.destroy(); lio_set_last_error(__FILE__, __LINE__, "cudaMalloc failed"); return LIO_ERR_CUDA; }
   float4 *d_in = nullptr, *d_out = nullptr;
   int *d_n = nullptr;
   int rc = LIO_OK;
-  if (cudaMalloc(&d_in, sizeof(float4) * n) != cudaSuccess || cudaMalloc(&d_out, sizeof(float4) * n) != cudaSuccess ||
-      cudaMalloc(&d_n, 2 * sizeof(int)) != cudaSuccess) {
+  if (vg.init(n) != 0) { lio_set_last_error(__FILE__, __LINE__, "cudaMalloc failed"); rc = LIO_ERR_CUDA; }
+  else if (!d.alloc(&d_in, n) || !d.alloc(&d_out, n) || !d.alloc(&d_n, 2) || !d.up(d_in, (const float4 *)cloud, n) || !d.up(d_n, &n, 1))
     rc = LIO_ERR_CUDA;
-  }
+  if (rc == LIO_OK) rc = vg.run(d_in, d_n, n, leaf, d_out, n, d_n + 1, nullptr, 0, nullptr);
+  int m = 0;
+  if (rc == LIO_OK && !d.down(&m, d_n + 1, 1)) rc = LIO_ERR_CUDA;
   if (rc == LIO_OK) {
-    cudaMemcpy(d_in, cloud, sizeof(float4) * n, cudaMemcpyHostToDevice);
-    cudaMemcpy(d_n, &n, sizeof(int), cudaMemcpyHostToDevice);
-    rc = vg.run(d_in, d_n, n, leaf, d_out, n, d_n + 1, nullptr, 0, nullptr);
-    if (rc == LIO_OK) {
-      int m = 0;
-      cudaError_t e = cudaMemcpy(&m, d_n + 1, sizeof(int), cudaMemcpyDeviceToHost);
-      if (e != cudaSuccess) { lio_set_last_error(__FILE__, __LINE__, cudaGetErrorString(e)); rc = LIO_ERR_CUDA; }
-      else {
-        *n_out = m;
-        if (m > cap) rc = LIO_ERR_CAPACITY;
-        else if (m > 0) cudaMemcpy(out, d_out, sizeof(float4) * m, cudaMemcpyDeviceToHost);
-      }
-    }
+    *n_out = m;
+    if (m > cap) rc = LIO_ERR_CAPACITY;
+    else if (!d.down((float4 *)out, d_out, m)) rc = LIO_ERR_CUDA;
   }
-  if (d_in) cudaFree(d_in);
-  if (d_out) cudaFree(d_out);
-  if (d_n) cudaFree(d_n);
   vg.destroy();
   return rc;
 }
@@ -404,24 +393,18 @@ extern "C" int lio_seg_voxel_grid_host(const float *xyzi, const int *n_per_job, 
   if (lio_device_count() <= 0) return LIO_ERR_NO_DEVICE;
   LIO_CUDA_OK(cudaSetDevice(device));
   *index_bound_error = 0;
+  DevBufs db;
   SegVoxelGrid sg;
   float4 *d = nullptr;
   std::vector<VgJob> jobs(njobs);
   std::vector<int> jn(njobs + 1, 0);
   int rc = LIO_OK;
-  if (sg.init() != 0 || sg.reserve((int)total) != 0 || cudaMalloc(&d, sizeof(float4) * total) != cudaSuccess) {
-    lio_set_last_error(__FILE__, __LINE__, "cudaMalloc failed");
-    rc = LIO_ERR_CUDA;
-  }
-  if (rc == LIO_OK && cudaMemcpy(d, xyzi, sizeof(float4) * total, cudaMemcpyHostToDevice) != cudaSuccess) {
-    lio_set_last_error(__FILE__, __LINE__, "upload failed");
-    rc = LIO_ERR_CUDA;
-  }
+  if (sg.init() != 0 || sg.reserve((int)total) != 0) { lio_set_last_error(__FILE__, __LINE__, "cudaMalloc failed"); rc = LIO_ERR_CUDA; }
+  else if (!db.alloc(&d, total) || !db.up(d, (const float4 *)xyzi, total)) rc = LIO_ERR_CUDA;
   if (rc == LIO_OK) {
     for (int j = 0, off = 0; j < njobs; off += n_per_job[j], ++j) jobs[j] = VgJob{d + off, n_per_job[j], off, leaf_per_job[j]};
     rc = sg.run(jobs.data(), njobs, (int)total, jn.data(), 0, nullptr);
-    cudaError_t e = rc == LIO_OK ? cudaDeviceSynchronize() : cudaSuccess;
-    if (e != cudaSuccess) { lio_set_last_error(__FILE__, __LINE__, cudaGetErrorString(e)); rc = LIO_ERR_CUDA; }
+    if (rc == LIO_OK && !db.ok(cudaDeviceSynchronize())) rc = LIO_ERR_CUDA;
   }
   if (rc == LIO_OK) {
     for (int j = 0; j < njobs; ++j) n_out_per_job[j] = jn[j];
@@ -429,12 +412,10 @@ extern "C" int lio_seg_voxel_grid_host(const float *xyzi, const int *n_per_job, 
     if (*index_bound_error) {
       lio_set_last_error(__FILE__, __LINE__, "a job's voxel grid exceeds 2^24 voxels");
       rc = LIO_ERR_CAPACITY;
-    } else {
-      cudaError_t e = cudaMemcpy(out, d, sizeof(float4) * total, cudaMemcpyDeviceToHost);
-      if (e != cudaSuccess) { lio_set_last_error(__FILE__, __LINE__, cudaGetErrorString(e)); rc = LIO_ERR_CUDA; }
+    } else if (!db.down((float4 *)out, d, total)) {
+      rc = LIO_ERR_CUDA;
     }
   }
-  if (d) cudaFree(d);
   sg.destroy();
   return rc;
 }
