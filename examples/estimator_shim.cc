@@ -26,6 +26,7 @@ struct EstimatorConfig {   // include/imu_processor/Estimator.h:77-108 (the fiel
   float min_match_sq_dis = 1.0f, min_plane_dis = 0.2f, surf_filter_size = 0.4f;
   bool imu_factor = true, point_distance_factor = true, prior_factor = true, marginalization_factor = true;
   int estimate_extrinsic = 1, opt_extrinsic = 1;
+  int init_window_factor = 1;
 };
 
 class Estimator {
@@ -44,6 +45,7 @@ class Estimator {
     c.prior_factor = estimator_config_.prior_factor; c.marginalization_factor = estimator_config_.marginalization_factor;
     c.estimate_extrinsic = estimator_config_.estimate_extrinsic; c.opt_extrinsic = estimator_config_.opt_extrinsic;
     c.max_frame_points = 1 << 15; c.max_scan_points = 1 << 17;
+    c.init_window_factor = estimator_config_.init_window_factor;
     const int rc = lio_est_create(&c, 0, nullptr, &gpu_);
     if (rc != LIO_OK) { std::fprintf(stderr, "lio_est_create: %d %s\n", rc, lio_last_error()); return false; }
     return lio_est_set_extrinsic(gpu_, tf_lb) == LIO_OK;

@@ -444,6 +444,8 @@ typedef struct lio_est_config {   /* EstimatorConfig (Estimator.h:77-108), lidar
                                     before its solve); 0: inline at the end of scan k, the reference's order.  Same result. */
   int solver_graph;              /* 1 (default): the device solver's launches of one solve are captured once as a CUDA graph
                                     and replayed per scan (single-GPU contexts); 0: plain stream launches.  Same result. */
+  int init_window_factor;        /* 1 (default): with a mapping attached (imu_factor = 0), only every init_window_factor-th message
+                                    is pushed before initialisation (Estimator.cc:436-439); values < 1 are refused */
 } lio_est_config;
 
 typedef struct lio_est lio_est;
@@ -593,6 +595,42 @@ int lio_est_local_laser_odom(lio_est *est, float tf7[7]);
  *                        LIO_ERR_INVALID without an attached map. */
 int lio_est_attach_map(lio_est *est, lio_pm *pm);
 int lio_est_map_poses(lio_est *est, float tobe7[7], float aft7[7], float insert7[7], int info4[4]);
+/* ---- imu_factor = 0 from the odometry's clouds: the estimator starts itself from the mapped lidar poses, without ImuInitializer
+ * (Estimator::ProcessCompactData :776-856, ProcessLaserOdom :430-774 with update_laser_imu).
+ *   lio_est_attach_mapping       hands a FRESH publishing PointMapping (lio_pm_enable_publish done, no process call yet) on the estimator's
+ *                                device to an imu_factor = 0 estimator with local clouds on, no sharding, leaf sizes equal to the map's,
+ *                                before any lio_est_init_frame / lio_est_finish_init / scan.  Any violation returns LIO_ERR_INVALID and
+ *                                changes nothing; a map whose max_full_points is below the local full capacity LIO_ERR_CAPACITY.  While
+ *                                attached pm refuses the same calls as under lio_est_attach_map, and so do lio_est_process_scan_* /
+ *                                open_scan_* / init_frame / finish_init on the estimator; lio_est_destroy releases pm.
+ *   lio_est_process_compact_dev  one /compact_data message: corner_dev / surf_dev / full_dev / n3_dev / n3_max as lio_pm_process_dev takes
+ *                                them (lio_po_clouds_dev gives them), transform_sum7 the odometry's transform_sum_.
+ *                                NOT_INITED: PointMapping::Process in full (association, optimisation, UpdateMapDatabase, PublishResults);
+ *                                every init_window_factor-th message then pushes the frame: transform_aft_mapped_, PointMapping's
+ *                                down-sampled corner / surf stacks, the raw full cloud, the valid cube list and the cube centre.  The push
+ *                                that fills the window (the (W+1)-th) sets states 0..W to trans_li * transform_lb_ (float Twist, cast to
+ *                                double), switches pm to its IMU-inited mode, runs the first solve (no estimator insert or publication) and
+ *                                SlideWindow.
+ *                                INITED: Process without insert and publication (PointMapping.cc:784, :1033), then the INITED push rules
+ *                                of lio_est_process_scan_* (with either de-skew flag the scan's own VoxelGrid of surf_last and the staged
+ *                                corner, otherwise PointMapping's stacks), state W from the pushed transforms (:1670-1676), the solve with
+ *                                lidar, marginalisation and prior factors, from the (O+1)-th INITED message on UpdateMapDatabase of the
+ *                                oldest optimised frame with ITS saved valid list and cube centre (:703-708), PublishResults and
+ *                                SlideWindow.  The IMU (lio_est_process_imu) is optional: before initialisation it propagates state
+ *                                cir_buf_count_ (:379-401), afterwards state W as usual, and feeds transform_es_.
+ *                                Stream rule: the inputs are read on pm's stream (Process) and on the estimator's stream, which waits for
+ *                                Process.  A bound n3_max[2] above the local max_full_points, or with a de-skew flag n3_max[0] above
+ *                                max_corner_points, returns LIO_ERR_CAPACITY before anything changes.  Other errors poison the
+ *                                context as scans do.
+ *   lio_est_process_compact_host the same from host clouds: upload into pm's input buffers, then the same steps, bit for bit.
+ *   lio_est_compact_status       info4 = {inited, cir_buf_count_, frame pushed by the last call, window solved by the last call}.
+ * lio_est_map_poses works in this mode; its aft7 is the live transform_aft_mapped_. */
+int lio_est_attach_mapping(lio_est *est, lio_pm *pm);
+int lio_est_process_compact_dev(lio_est *est, const float *corner_dev, const float *surf_dev, const float *full_dev, const int *n3_dev,
+                                const int n3_max[3], const float transform_sum7[7]);
+int lio_est_process_compact_host(lio_est *est, const float *corner, int nc, const float *surf, int ns, const float *full, int nf,
+                                 const float transform_sum7[7]);
+int lio_est_compact_status(lio_est *est, int info4[4]);
 /* window states: (W+1) x 16 doubles (layout of state16) */
 int lio_est_get_states(lio_est *est, double *out);
 /* summary[32]: see lio_mapping_b200/estimator.py SUMMARY_KEYS */

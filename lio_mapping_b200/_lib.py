@@ -38,7 +38,8 @@ class EstConfig(C.Structure):
                 ("enable_deskew", C.c_int), ("cutoff_deskew", C.c_int), ("acc_n", C.c_double), ("gyr_n", C.c_double),
                 ("acc_w", C.c_double), ("gyr_w", C.c_double), ("g_norm", C.c_double), ("max_num_iterations", C.c_int),
                 ("odom_max_iterations", C.c_int), ("max_frame_points", C.c_int), ("max_scan_points", C.c_int),
-                ("device_solver", C.c_int), ("overlap_marginalization", C.c_int), ("solver_graph", C.c_int)]
+                ("device_solver", C.c_int), ("overlap_marginalization", C.c_int), ("solver_graph", C.c_int),
+                ("init_window_factor", C.c_int)]
 
 
 ALLREDUCE_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_int)
@@ -198,6 +199,10 @@ def lib():
     L.lio_est_local_laser_odom.argtypes = [vp, f32p]
     L.lio_est_attach_map.argtypes = [vp, vp]
     L.lio_est_map_poses.argtypes = [vp, f32p, f32p, f32p, i32p]
+    L.lio_est_attach_mapping.argtypes = [vp, vp]
+    L.lio_est_process_compact_dev.argtypes = [vp, vp, vp, vp, vp, i32p, f32p]
+    L.lio_est_process_compact_host.argtypes = [vp, f32p, ip, f32p, ip, f32p, ip, f32p]
+    L.lio_est_compact_status.argtypes = [vp, i32p]
     L.lio_mb_process_map_dev.argtypes = [vp, vp, vp, vp, vp, i32p, f32p, f32p, f32p, i32p]
     L.lio_po_process_dev.argtypes = [vp, C.POINTER(vp), C.POINTER(vp), i32p, f32p, f32p, i32p]
     L.lio_po_clouds_dev.argtypes = [vp, C.POINTER(vp), C.POINTER(vp), i32p]

@@ -24,6 +24,7 @@
 #include <algorithm>
 #include <climits>
 #include <cmath>
+#include <cstdio>
 #include <cstring>
 #include <new>
 #include <vector>
@@ -206,6 +207,7 @@ struct lio_pm {
   bool started = false;               // a process call has run (lio_pm_enable_publish must come before it)
   bool publish = false;                // lio_pm_enable_publish: PointMapping::PublishResults on every lio_pm_process_dev
   bool attached = false;               // lio_est_attach_map: the estimator owns the map (its process / update / destroy entries refuse)
+  bool imu_inited = false;             // imu_inited_ (SetInitFlag): Process skips UpdateMapDatabase and PublishResults (:1033)
   // map-builder mode (lio_mb_*: MapBuilder : PointMapping, src/map_builder/MapBuilder.cc)
   bool mb = false, enable_4d = true, system_init = false;
   int skip_count = 2, odom_count = 0;
@@ -617,12 +619,14 @@ static int pm_process(lio_pm *m, const float4 *const src[2], const float4 *full,
   m->last_iters = 0;
   if (optimised && (rc = pm_optimise(m, K, n_ds, 0)) != LIO_OK) return rc;
   if (optimised) { m->bef = m->sum; m->aft = m->tobe; }   // TransformUpdate sits behind the optimiser's early return (:327-329, :716)
-  const int cen[3] = {m->cen_l, m->cen_w, m->cen_h};   // margin centre == current centre: the valid list is this call's
-  const float4 *ds[2] = {m->d_ds[0], m->d_ds[1]};
-  const int *n_ds_dev[2] = {m->d_cnt + 2, m->d_cnt + 3};
-  if ((rc = pm_update(m, m->last_valid, ds, n_ds_dev, n_ds, m->tobe, cen)) != LIO_OK) return rc;
   bool published = false;
-  if (m->publish && (rc = pm_publish(m, m->last_surround, m->d_full_in, m->d_cnt + 4, n_max[2] > 0 ? m->h_cnt[4] : 0, published)) != LIO_OK) return rc;
+  if (!m->imu_inited) {
+    const int cen[3] = {m->cen_l, m->cen_w, m->cen_h};   // margin centre == current centre: the valid list is this call's
+    const float4 *ds[2] = {m->d_ds[0], m->d_ds[1]};
+    const int *n_ds_dev[2] = {m->d_cnt + 2, m->d_cnt + 3};
+    if ((rc = pm_update(m, m->last_valid, ds, n_ds_dev, n_ds, m->tobe, cen)) != LIO_OK) return rc;
+    if (m->publish && (rc = pm_publish(m, m->last_surround, m->d_full_in, m->d_cnt + 4, n_max[2] > 0 ? m->h_cnt[4] : 0, published)) != LIO_OK) return rc;
+  }
   if (transform_tobe_mapped7) twist_to_tf7(m->tobe, transform_tobe_mapped7);
   if (transform_aft_mapped7) twist_to_tf7(m->aft, transform_aft_mapped7);
   const int out[5] = {m->last_iters, K[0], K[1], published ? 1 : 0, m->publish ? m->n_surround : 0};
@@ -940,18 +944,23 @@ extern "C" int lio_pm_cube_download(lio_pm *m, int cube_index, int which, float 
 }
 
 // ---- the device estimator's map after initialisation (cubemap.cuh, lio_est_attach_map) ------------------------------------
-int pm_attach(lio_pm *m, int device, float corner_leaf, float surf_leaf, int ins_bound, int full_bound) {
-  if (!m || m->mb || !m->publish || !m->started || m->attached || m->device != device) {
-    lio_set_last_error(__FILE__, __LINE__, "lio_est_attach_map: needs a publishing PointMapping (lio_pm_enable_publish) on the estimator's device "
-                                           "that has run a process call and is not attached");
+int pm_attach(lio_pm *m, int device, float corner_leaf, float surf_leaf, int ins_bound, int full_bound, bool fresh) {
+  const char *who = fresh ? "lio_est_attach_mapping" : "lio_est_attach_map";
+  char msg[256];
+  if (!m || m->mb || !m->publish || m->started != !fresh || m->attached || m->device != device) {
+    std::snprintf(msg, sizeof(msg), "%s: needs a publishing PointMapping (lio_pm_enable_publish) on the estimator's device that %s and is not attached",
+                  who, fresh ? "has run no process call" : "has run a process call");
+    lio_set_last_error(__FILE__, __LINE__, msg);
     return LIO_ERR_INVALID;
   }
   if (m->leaf[0] != corner_leaf || m->leaf[1] != surf_leaf) {
-    lio_set_last_error(__FILE__, __LINE__, "lio_est_attach_map: the map's corner / surf leaf sizes differ from the estimator's");
+    std::snprintf(msg, sizeof(msg), "%s: the map's corner / surf leaf sizes differ from the estimator's", who);
+    lio_set_last_error(__FILE__, __LINE__, msg);
     return LIO_ERR_INVALID;
   }
   if (m->max_full < full_bound) {
-    lio_set_last_error(__FILE__, __LINE__, "lio_est_attach_map: the map's max_full_points is below the estimator's full-cloud capacity");
+    std::snprintf(msg, sizeof(msg), "%s: the map's max_full_points is below the estimator's full-cloud capacity", who);
+    lio_set_last_error(__FILE__, __LINE__, msg);
     return LIO_ERR_CAPACITY;
   }
   LIO_CUDA_OK(cudaSetDevice(m->device));
@@ -993,14 +1002,48 @@ TwistF *pm_tobe(lio_pm *m) { return &m->tobe; }
 TwistF pm_aft(const lio_pm *m) { return m->aft; }
 
 int pm_est_step(lio_pm *m, bool insert, const float4 *const src[2], const int *const n_dev[2], const int bound[2], const TwistF &pose,
-                const float4 *full, const int *nf_dev, int nf, int info4[4]) {
+                const std::vector<size_t> *valid, const int *margin_centre, const float4 *full, const int *nf_dev, int nf, int info4[4]) {
   int rc = LIO_OK;
   if (insert) {
     const int cen[3] = {m->cen_l, m->cen_w, m->cen_h};   // opt_cube_centers_: the centre is frozen with the valid list
-    if ((rc = pm_update(m, m->last_valid, src, n_dev, bound, pose, cen)) != LIO_OK) return rc;
+    if ((rc = pm_update(m, valid ? *valid : m->last_valid, src, n_dev, bound, pose, margin_centre ? margin_centre : cen)) != LIO_OK) return rc;
   }
   bool published = false;
   if ((rc = pm_publish(m, m->last_surround, full, nf_dev, nf, published)) != LIO_OK) return rc;
   info4[0] = insert ? 1 : 0; info4[1] = insert ? m->upd_stats[3] : 0; info4[2] = published ? 1 : 0; info4[3] = m->n_surround;
   return LIO_OK;
 }
+
+int pm_est_upload(lio_pm *m, const float *corner, int nc, const float *surf, int ns, const float *full, int nf, const float4 *src[3],
+                  const int **n3_dev) {
+  if (nc > m->max_points || ns > m->max_points || nf > m->max_full) {
+    lio_set_last_error(__FILE__, __LINE__, "lio_est_process_compact_host: a cloud exceeds the mapping's max_points / max_full_points");
+    return LIO_ERR_CAPACITY;
+  }
+  const float *in[2] = {corner, surf};
+  const int nin[2] = {nc, ns};
+  LIO_CUDA_OK(cudaSetDevice(m->device));
+  if (nf > 0) LIO_CUDA_OK(cudaMemcpyAsync(m->d_full_in, full, sizeof(float4) * nf, cudaMemcpyHostToDevice, m->stream));
+  int rc = pm_upload(m, in, nin, full, nf);   // full goes up above: pm_upload copies it for a map builder only
+  if (rc != LIO_OK) return rc;
+  src[0] = m->d_in[0]; src[1] = m->d_in[1]; src[2] = m->d_full_in;
+  *n3_dev = m->d_cnt + 8;
+  return LIO_OK;
+}
+
+int pm_est_process(lio_pm *m, const float4 *const src[2], const float4 *full, const int *n3_dev, const int n_max[3], const float sum7[7]) {
+  LIO_CUDA_OK(cudaSetDevice(m->device));
+  return pm_process(m, src, full, n3_dev, n_max, sum7, nullptr, nullptr, nullptr, 0);
+}
+
+void pm_est_caps(const lio_pm *m, const int n3_max[3], int out[3]) {
+  out[0] = std::min(n3_max[0], m->max_points); out[1] = std::min(n3_max[1], m->max_points); out[2] = std::min(n3_max[2], m->max_full);
+}
+
+void pm_set_imu_inited(lio_pm *m) { m->imu_inited = true; }
+const float4 *pm_ds(const lio_pm *m, int which) { return m->d_ds[which]; }
+const int *pm_counts_dev(const lio_pm *m) { return m->d_cnt; }
+int pm_ds_n(const lio_pm *m, int which) { return m->h_cnt[2 + which]; }
+const float4 *pm_full_in(const lio_pm *m) { return m->d_full_in; }
+const std::vector<size_t> &pm_valid(const lio_pm *m) { return m->last_valid; }
+void pm_centre(const lio_pm *m, int c[3]) { c[0] = m->cen_l; c[1] = m->cen_w; c[2] = m->cen_h; }

@@ -23,6 +23,7 @@
 #include "solver_dev.cuh"
 #include "solver_host.h"
 #include "voxel.cuh"
+#include <array>
 #include <chrono>
 #include <cstddef>
 #include <memory>
@@ -593,6 +594,16 @@ struct lio_est {
   cudaEvent_t map_ev_in = nullptr, map_ev_done = nullptr;
   lio::TwistF map_insert;             // opt_transforms_.first() of the last insert
   int map_info[4] = {0, 0, 0, 0};     // inserted, points inserted, surround published, last surround size
+  // ---- imu_factor = 0 from the odometry's clouds (lio_est_attach_mapping): the estimator's own PointMapping::Process on every message,
+  // the NOT_INITED window of the mapped poses and the start-up (ProcessCompactData / ProcessLaserOdom, Estimator.cc:430-856)
+  bool mapping = false;
+  bool inited = false;                // stage_flag_ == INITED
+  bool map_quiet = false;             // the start-up's solve: no estimator insert or publication on the NOT_INITED path
+  int cir_count = 0, recv_count = 0;  // cir_buf_count_, laser_odom_recv_count_
+  std::vector<lio::TwistF> laser_tf;  // all_laser_transforms_ (transform_aft_mapped_ of each push), logical frames
+  std::vector<std::vector<size_t>> opt_valid;   // opt_valid_idx_, logical frames
+  std::vector<std::array<int, 3>> opt_centre;   // opt_cube_centers_, logical frames
+  int compact_info[4] = {0, 0, 0, 0}; // inited, cir_buf_count_, pushed by the last call, solved by the last call
 };
 
 static Tw tlb_double(const lio_est *e) {
@@ -639,6 +650,7 @@ extern "C" void lio_est_default_config(lio_est_config *c) {
   c->device_solver = 1;   // GPU-resident dogleg loop (solver_dev.cu); 0 keeps the host controller (also used when O > 13)
   c->overlap_marginalization = 1;
   c->solver_graph = 1;
+  c->init_window_factor = 1;
 }
 
 // point the per-frame feature descriptors at one parity of the slab
@@ -739,7 +751,7 @@ extern "C" int lio_est_create(const lio_est_config *cfg, int device, void *cuda_
   if (!cfg || !out) return LIO_ERR_INVALID;
   const int W = cfg->window_size, O = cfg->opt_window_size;
   if (W < 1 || W >= kMaxWindow || O < 1 || O > W || O > kMaxOpt || cfg->max_frame_points < 16 || cfg->max_scan_points < 16 ||
-      !(cfg->surf_filter_size > 0) || !(cfg->min_match_sq_dis > 0) || cfg->odom_max_iterations < 1) {
+      !(cfg->surf_filter_size > 0) || !(cfg->min_match_sq_dis > 0) || cfg->odom_max_iterations < 1 || cfg->init_window_factor < 1) {
     lio_set_last_error(__FILE__, __LINE__, "lio_est_create: configuration outside supported limits");
     return LIO_ERR_INVALID;
   }
@@ -946,7 +958,7 @@ extern "C" int lio_est_set_scan_clouds_dev(lio_est *e, const float *corner_dev, 
 // corner TransformToEnd under the surf cloud's condition + VoxelGrid(corner_filter_size) into corner_stack_[W] (:662-693),
 // full_stack_[W] = the staged full cloud (:482), the /local/* gather of frame pivot + 1 (:2362-2375), then TransformToEnd of the
 // newest full cloud with keep_intensity (:2416) - after the gather, so that with O = 1 the frame is published before it, as there.
-static int lc_push(lio_est *e, bool deskew_corner) {
+static int lc_push(lio_est *e, bool deskew_corner, bool corner_filtered = false) {
   const int W = e->W, pivot = W - e->O, slot = e->slot_of[W], pub = e->slot_of[pivot + 1];
   cudaStream_t ls = e->lc_stream;
   const int grid_c = std::max(1, std::min(e->sm_count * 2, (e->lc_cap[0] + 255) / 256));
@@ -960,9 +972,14 @@ static int lc_push(lio_est *e, bool deskew_corner) {
     k_deskew<<<(e->lc_cap[0] + 255) / 256, 256, 0, ls>>>(e->d_lc_stage[0], e->d_lc_stage_n, e->es, 10.f);
     ++e->launches;
   }
-  int rc = e->lc_vg.run(e->d_lc_stage[0], e->d_lc_stage_n, e->lc_cap[0], e->lc_corner_leaf, e->lc_slot[0][slot], e->lc_cap[0], n_corner + slot,
-                        nullptr, ls, &e->launches);
-  if (rc != LIO_OK) return rc;
+  if (corner_filtered) {   // PointMapping's laser_cloud_corner_stack_downsampled_ (lio_est_attach_mapping, :478)
+    k_copy_cloud<<<grid_c, 256, 0, ls>>>(e->d_lc_stage[0], e->d_lc_stage_n, e->lc_cap[0], e->lc_slot[0][slot], n_corner + slot);
+    ++e->launches;
+  } else {
+    int rc = e->lc_vg.run(e->d_lc_stage[0], e->d_lc_stage_n, e->lc_cap[0], e->lc_corner_leaf, e->lc_slot[0][slot], e->lc_cap[0], n_corner + slot,
+                          nullptr, ls, &e->launches);
+    if (rc != LIO_OK) return rc;
+  }
   k_copy_cloud<<<grid_f, 256, 0, ls>>>(e->d_lc_stage[1], e->d_lc_stage_n + 1, e->lc_cap[1], e->lc_slot[1][slot], n_full + slot);
   LocalGather G;
   G.src[0] = e->lc_slot[0][pub]; G.n[0] = n_corner + pub;
@@ -993,6 +1010,7 @@ extern "C" int lio_est_init_frame(lio_est *e, int k, const double s[16], const f
   }
   LIO_CUDA_OK(cudaSetDevice(e->device));
   e->frames_started = true;
+  if (e->mapping) { lio_set_last_error(__FILE__, __LINE__, "a mapping is attached: the window starts from the mapped poses"); return LIO_ERR_INVALID; }
   if (e->lc_on) {   // the pre-initialisation corner_stack_ / full_stack_ entries (Estimator.cc:474-482), verbatim
     const int slot = e->slot_of[k + 1];
     for (int w = 0; w < 2; ++w) {
@@ -1015,7 +1033,7 @@ extern "C" int lio_est_init_frame(lio_est *e, int k, const double s[16], const f
 }
 
 extern "C" int lio_est_finish_init(lio_est *e, const double a[3], const double g[3]) {
-  if (!e || !a || !g) return LIO_ERR_INVALID;
+  if (!e || !a || !g || e->mapping) return LIO_ERR_INVALID;
   const int W = e->W;
   e->Ps[W] = e->Ps[W - 1]; e->Rs[W] = e->Rs[W - 1]; e->Vs[W] = e->Vs[W - 1]; e->Bas[W] = e->Bas[W - 1]; e->Bgs[W] = e->Bgs[W - 1];
   e->acc_last = V3(a); e->gyr_last = V3(g);
@@ -1030,7 +1048,8 @@ extern "C" int lio_est_process_imu(lio_est *e, double dt, const double a[3], con
   const V3 acc(a), gyr(g);
   if (!e->first_imu) { e->first_imu = true; e->acc_last = acc; e->gyr_last = gyr; }
   if (!e->tmp_pre) return LIO_ERR_INVALID;
-  const int j = e->W;
+  if (e->mapping && !e->inited && e->cir_count == 0) { e->acc_last = acc; e->gyr_last = gyr; return LIO_OK; }   // :379: no laser yet
+  const int j = (e->mapping && !e->inited) ? e->cir_count : e->W;
   e->tmp_pre->push_back(dt, acc, gyr);
   const V3 un_acc_0 = e->Rs[j] * (e->acc_last - e->Bas[j]) + e->g_vec;
   const V3 un_gyr = 0.5 * (e->gyr_last + gyr) - e->Bgs[j];
@@ -1928,7 +1947,7 @@ static int scan_close_window(lio_est *e) {
   e->window_open = false;
   int rc = lc_join(e);   // the forked /local/* work reads the surf slot that SlideWindow replaces
   if (rc != LIO_OK) return rc;
-  if (e->map && (rc = map_step(e)) != LIO_OK) return rc;   // UpdateMapDatabase + PublishResults come before SlideWindow (:703-723)
+  if (e->map && !e->map_quiet && (rc = map_step(e)) != LIO_OK) return rc;   // UpdateMapDatabase + PublishResults come before SlideWindow (:703-723)
   return slide_window(e);
 }
 
@@ -2133,10 +2152,12 @@ static int map_scan_entry(lio_est *e) {
     const Q q = fromR(R);
     return lio::TwistF{(float)q.x, (float)q.y, (float)q.z, (float)q.w, (float)P.x, (float)P.y, (float)P.z};
   };
-  const lio::TwistF d = lio::twist_mul(lio::twist_inverse(twist_of(e->Rs[W - 1], e->Ps[W - 1])), twist_of(e->Rs[W], e->Ps[W]));
-  const lio::TwistF lb{e->tlb_q[0], e->tlb_q[1], e->tlb_q[2], e->tlb_q[3], e->tlb_p[0], e->tlb_p[1], e->tlb_p[2]};
-  lio::TwistF *tobe = pm_tobe(e->map);
-  *tobe = lio::twist_mul(lio::twist_mul(lio::twist_mul(*tobe, lb), d), lio::twist_inverse(lb));
+  if (e->cfg.imu_factor) {   // imu_factor = 0: TransformAssociateToMap, run by the mapping's Process (:804)
+    const lio::TwistF d = lio::twist_mul(lio::twist_inverse(twist_of(e->Rs[W - 1], e->Ps[W - 1])), twist_of(e->Rs[W], e->Ps[W]));
+    const lio::TwistF lb{e->tlb_q[0], e->tlb_q[1], e->tlb_q[2], e->tlb_q[3], e->tlb_p[0], e->tlb_p[1], e->tlb_p[2]};
+    lio::TwistF *tobe = pm_tobe(e->map);
+    *tobe = lio::twist_mul(lio::twist_mul(lio::twist_mul(*tobe, lb), d), lio::twist_inverse(lb));
+  }
   if (W == O && map_deskew(e) && e->map_scans >= O) {
     const int s0 = e->slot_of[0];
     k_copy_cloud<<<std::max(1, std::min(e->sm_count * 2, (e->lc_cap[0] + 255) / 256)), 256, 0, st>>>(
@@ -2183,12 +2204,17 @@ static int map_step(lio_est *e) {
   EST_CUDA(cudaEventRecord(e->map_ev_in, e->stream));
   EST_CUDA(cudaStreamWaitEvent(ms, e->map_ev_in, 0));
   e->map_pending = true;
-  const int rc = pm_est_step(e->map, insert, src, n_dev, bound, e->map_insert, e->d_lc_stage[1], e->d_lc_stage_n + 1, e->h_counts[W + 13], e->map_info);
+  // imu_factor = 0: the frame's own valid list and the cube centre it was computed with (opt_valid_idx_ / opt_cube_centers_.first())
+  const std::vector<size_t> *valid = e->mapping ? &e->opt_valid[pivot] : nullptr;
+  const int *centre = e->mapping ? e->opt_centre[pivot].data() : nullptr;
+  const int rc = pm_est_step(e->map, insert, src, n_dev, bound, e->map_insert, valid, centre, e->d_lc_stage[1], e->d_lc_stage_n + 1, e->h_counts[W + 13],
+                             e->map_info);
   if (rc != LIO_OK) return rc;
   EST_CUDA(cudaEventRecord(e->map_ev_done, ms));
   return LIO_OK;
 }
 
+static int attach_common(lio_est *e, lio_pm *pm, bool fresh);
 extern "C" int lio_est_attach_map(lio_est *e, lio_pm *pm) {
   if (!e || !pm) return LIO_ERR_INVALID;
   const char *why = nullptr;
@@ -2199,6 +2225,11 @@ extern "C" int lio_est_attach_map(lio_est *e, lio_pm *pm) {
   else if (!e->cfg.imu_factor) why = "lio_est_attach_map: needs imu_factor = 1";
   else if (e->world > 1 || e->npeers || e->fpeers) why = "lio_est_attach_map: not supported on a sharded context";
   if (why) { lio_set_last_error(__FILE__, __LINE__, why); return LIO_ERR_INVALID; }
+  return attach_common(e, pm, false);
+}
+
+// The estimator's side of both attaches: the map-step events, the W == O de-skew copies, and the handle's own checks (pm_attach).
+static int attach_common(lio_est *e, lio_pm *pm, bool fresh) {
   LIO_CUDA_OK(cudaSetDevice(e->device));
   const bool keep = e->W == e->O && map_deskew(e);
   bool ok = cudaEventCreateWithFlags(&e->map_ev_in, cudaEventDisableTiming) == cudaSuccess;
@@ -2211,7 +2242,7 @@ extern "C" int lio_est_attach_map(lio_est *e, lio_pm *pm) {
   int rc = ok ? LIO_OK : LIO_ERR_CUDA;
   if (!ok) lio_set_last_error(__FILE__, __LINE__, "lio_est_attach_map: device allocation failed");
   // an accumulated surf slot holds up to max_frame_points * (W - O + 1) points: the map's insert buffers grow to it
-  if (ok) rc = pm_attach(pm, e->device, e->lc_corner_leaf, e->cfg.surf_filter_size, e->lc_cap[0] + e->slot_cap, e->lc_cap[1]);
+  if (ok) rc = pm_attach(pm, e->device, e->lc_corner_leaf, e->cfg.surf_filter_size, e->lc_cap[0] + e->slot_cap, e->lc_cap[1], fresh);
   if (rc != LIO_OK) {   // nothing changed: the buffers go, the handle stays usable without a map
     for (int w = 0; w < 2; ++w) { if (e->d_keep[w]) cudaFree(e->d_keep[w]); e->d_keep[w] = nullptr; }
     if (e->d_keep_n) cudaFree(e->d_keep_n);
@@ -2236,7 +2267,202 @@ extern "C" int lio_est_map_poses(lio_est *e, float tobe7[7], float aft7[7], floa
   return LIO_OK;
 }
 
-static int process_scan_body(lio_est *e, const float4 *scan_dev, const int *n_dev, int n_max, bool open_only);
+// A push of lio_est_process_compact_* (imu_factor = 0): surf_ds / surf_ds_n, when set, is PointMapping's down-sampled surf stack, copied
+// into the frame slot instead of the VoxelGrid of the scan (:474-480); corner_filtered: the staged corner cloud is that stack's corner
+// cloud, copied likewise; startup: the NOT_INITED push that reaches a full window (:505-517), no transform_es_.
+struct CompactPush { const float4 *surf_ds; const int *surf_ds_n; bool corner_filtered, startup; };
+static int process_scan_body(lio_est *e, const float4 *scan_dev, const int *n_dev, int n_max, bool open_only, const CompactPush *cp = nullptr);
+
+// ---- imu_factor = 0 from the odometry's clouds (lio_est_attach_mapping; Estimator.cc:430-856) ------------------------------
+static lio::TwistF lb_twist(const lio_est *e) {
+  return lio::TwistF{e->tlb_q[0], e->tlb_q[1], e->tlb_q[2], e->tlb_q[3], e->tlb_p[0], e->tlb_p[1], e->tlb_p[2]};
+}
+
+// SolveOptimization :1670-1676: state W from the increment of the last two pushed laser transforms, incre = (lb^-1 * T_{W-1}^-1 * T_W
+// * lb) in float Twist, cast to double; Ps_[W] = Rs_[W-1] * incre.pos + Ps_[W-1], Rs_[W] = Rs_[W-1] * incre.rot.  Every input is host
+// state (the mapping's optimiser reads its pose back before the call returns), so this is host arithmetic with no device round trip.
+static void predict_state_w(lio_est *e) {
+  const int W = e->W;
+  const lio::TwistF lb = lb_twist(e);
+  const lio::TwistF inc = lio::twist_mul(lio::twist_mul(lio::twist_mul(lio::twist_inverse(lb), lio::twist_inverse(e->laser_tf[W - 1])), e->laser_tf[W]), lb);
+  const V3 p((double)inc.px, (double)inc.py, (double)inc.pz);
+  e->Ps[W] = e->Rs[W - 1] * p + e->Ps[W - 1];
+  e->Rs[W] = e->Rs[W - 1] * toR(Q((double)inc.qw, (double)inc.qx, (double)inc.qy, (double)inc.qz));
+}
+
+extern "C" int lio_est_attach_mapping(lio_est *e, lio_pm *pm) {
+  if (!e || !pm) return LIO_ERR_INVALID;
+  const char *why = nullptr;
+  if (e->map) why = "lio_est_attach_mapping: a map is attached already";
+  else if (e->frames_started || e->tmp_pre) why = "lio_est_attach_mapping: call it before lio_est_init_frame / lio_est_finish_init and the first scan";
+  else if (!e->lc_on) why = "lio_est_attach_mapping: local clouds are off (lio_est_enable_local_clouds)";
+  else if (e->cfg.imu_factor) why = "lio_est_attach_mapping: needs imu_factor = 0";
+  else if (e->world > 1 || e->npeers || e->fpeers) why = "lio_est_attach_mapping: not supported on a sharded context";
+  if (why) { lio_set_last_error(__FILE__, __LINE__, why); return LIO_ERR_INVALID; }
+  const int rc = attach_common(e, pm, true);
+  if (rc != LIO_OK) return rc;
+  const int W = e->W;
+  e->mapping = true;
+  e->laser_tf.assign(W + 1, lio::TwistF{});
+  e->opt_valid.assign(W + 1, std::vector<size_t>());
+  e->opt_centre.assign(W + 1, std::array<int, 3>{0, 0, 0});
+  // ProcessImu needs a pre-integration to fill once the first laser frame is in (:379-381); ImuFactors are not part of the solve
+  e->tmp_pre = std::make_shared<Preintegration>(e->acc_last, e->gyr_last, e->Bas[0], e->Bgs[0], e->noise);
+  return LIO_OK;
+}
+
+// ProcessCompactData (:776-856) with update_laser_imu: PointMapping::Process on the mapping's stream, then ProcessLaserOdom.  corner /
+// surf / full and n3_dev are the message's clouds and counts, n_max their bounds (already capped by the mapping's capacities).
+static int compact_body(lio_est *e, const float4 *const src[3], const int *n3_dev, const int n_max[3], const float sum7[7]) {
+  const int W = e->W;
+  cudaStream_t st = e->stream, ms = pm_stream(e->map);
+  // Process overwrites the handle's stacks and full cloud, which the estimator's previous pushes read on its own stream
+  EST_CUDA(cudaEventRecord(e->map_ev_in, st));
+  EST_CUDA(cudaStreamWaitEvent(ms, e->map_ev_in, 0));
+  int rc = pm_est_process(e->map, src, src[2], n3_dev, n_max, sum7);
+  if (rc != LIO_OK) return rc;
+  EST_CUDA(cudaEventRecord(e->map_ev_done, ms));
+  EST_CUDA(cudaStreamWaitEvent(st, e->map_ev_done, 0));
+  e->map_pending = false;
+  ++e->recv_count;
+  e->compact_info[0] = e->inited ? 1 : 0; e->compact_info[1] = e->cir_count; e->compact_info[2] = e->compact_info[3] = 0;
+  if (!e->inited && e->recv_count % e->cfg.init_window_factor != 0) return LIO_OK;   // :436-439
+  // the push (:441-487): the laser transform is transform_aft_mapped_, the stacks PointMapping's down-sampled ones unless the INITED
+  // de-skew rules push their own (:474-480, :628-693)
+  const bool deskew_flags = e->cfg.enable_deskew || e->cfg.cutoff_deskew;
+  const bool pm_stacks = !e->inited || !deskew_flags;
+  const int nds[2] = {pm_ds_n(e->map, 0), pm_ds_n(e->map, 1)};
+  if (pm_stacks && (nds[1] > e->cfg.max_frame_points || nds[0] > e->lc_cap[0])) {
+    lio_set_last_error(__FILE__, __LINE__, "the mapping's down-sampled stacks exceed max_frame_points / the local corner capacity");
+    return LIO_ERR_CAPACITY;
+  }
+  const int *cnt = pm_counts_dev(e->map);   // {corner in, surf in, corner ds, surf ds, full}
+  rc = lc_stage_wait(e);
+  if (rc != LIO_OK) return rc;
+  {
+    const float4 *sc[2] = {pm_stacks ? pm_ds(e->map, 0) : src[0], pm_full_in(e->map)};
+    const int *nc[2] = {pm_stacks ? cnt + 2 : cnt, cnt + 4};
+    const int nb[2] = {e->lc_cap[0], n_max[2]};
+    for (int w = 0; w < 2; ++w)
+      k_copy_cloud<<<std::max(1, std::min(e->sm_count * 2, (nb[w] + 255) / 256)), 256, 0, st>>>(sc[w], nc[w], nb[w], e->d_lc_stage[w], e->d_lc_stage_n + w);
+    EST_CUDA(cudaGetLastError());
+    e->lc_staged = true;
+  }
+  push_shift(e->laser_tf, pm_aft(e->map));
+  push_shift(e->opt_valid, pm_valid(e->map));
+  {
+    std::array<int, 3> c;
+    pm_centre(e->map, c.data());
+    push_shift(e->opt_centre, c);
+  }
+  e->compact_info[2] = 1;
+  const int c = e->cir_count;
+  if (!e->inited && c < W) {   // NOT_INITED, window not full: push, SlideWindow's state copy, ++cir_buf_count_ (:603-614)
+    push_shift(e->pre, e->tmp_pre);
+    e->tmp_pre = std::make_shared<Preintegration>(e->acc_last, e->gyr_last, e->Bas[c], e->Bgs[c], e->noise);
+    const int freed = e->slot_of[0];
+    e->slot_of.erase(e->slot_of.begin());
+    e->slot_of.push_back(freed);
+    const int slot = e->slot_of[W];
+    const int grid = std::max(1, std::min(e->sm_count * 2, (e->cfg.max_frame_points + 255) / 256));
+    k_copy_cloud<<<grid, 256, 0, st>>>(pm_ds(e->map, 1), cnt + 3, e->cfg.max_frame_points, e->slot_ptr[slot], e->d_slot_n + slot);
+    for (int w = 0; w < 2; ++w)
+      k_copy_cloud<<<std::max(1, std::min(e->sm_count * 2, (e->lc_cap[w] + 255) / 256)), 256, 0, st>>>(
+          e->d_lc_stage[w], e->d_lc_stage_n + w, e->lc_cap[w], e->lc_slot[w][slot], e->d_lc_slot_n + w * (W + 1) + slot);
+    EST_CUDA(cudaGetLastError());
+    EST_CUDA(cudaMemcpyAsync(e->d_own_n + slot, e->d_slot_n + slot, sizeof(int), cudaMemcpyDeviceToDevice, st));
+    e->lc_staged = false;
+    push_shift(e->size_surf_stack, nds[1]);
+    e->Ps[c + 1] = e->Ps[c]; e->Vs[c + 1] = e->Vs[c]; e->Rs[c + 1] = e->Rs[c]; e->Bas[c + 1] = e->Bas[c]; e->Bgs[c + 1] = e->Bgs[c];
+    e->compact_info[1] = ++e->cir_count;
+    return LIO_OK;
+  }
+  CompactPush cp{nullptr, nullptr, pm_stacks, !e->inited};
+  if (pm_stacks) { cp.surf_ds = pm_ds(e->map, 1); cp.surf_ds_n = cnt + 3; }
+  if (!e->inited) {   // the start-up (:505-517): states 0..W from the W + 1 pushed laser transforms, then the first solve and slide
+    const lio::TwistF lb = lb_twist(e);
+    for (int i = 0; i <= W; ++i) {
+      const lio::TwistF tb = lio::twist_mul(e->laser_tf[i], lb);
+      float R[9];
+      lio::quat_to_matrix_normalized(tb, R);
+      e->Ps[i] = V3((double)tb.px, (double)tb.py, (double)tb.pz);
+      for (int a = 0; a < 3; ++a) for (int b = 0; b < 3; ++b) e->Rs[i](a, b) = (double)R[3 * a + b];
+    }
+    e->inited = true;
+    pm_set_imu_inited(e->map);   // SetInitFlag(true) (:544)
+    e->map_quiet = true;
+  }
+  rc = process_scan_body(e, src[1], cnt + 1, std::max(1, std::min(n_max[1], e->cfg.max_scan_points)), false, &cp);
+  e->map_quiet = false;
+  if (rc != LIO_OK) return rc;
+  e->compact_info[0] = 1; e->compact_info[3] = 1;
+  return LIO_OK;
+}
+
+static int compact_common(lio_est *e, const float4 *const src[3], const int *n3_dev, const int n_max[3], const float sum7[7]) {
+  if (e->poisoned) {
+    lio_set_last_error(__FILE__, __LINE__, "estimator context poisoned by an earlier failed scan: destroy and re-create it");
+    return LIO_ERR_INVALID;
+  }
+  // the full cloud is pushed into a local full slot, and with a de-skew flag the raw corner cloud is staged after initialisation:
+  // bounds above those capacities are refused before anything changes, as lio_est_set_scan_clouds_* refuses them
+  if (n_max[2] > e->lc_cap[1] || ((e->cfg.enable_deskew || e->cfg.cutoff_deskew) && n_max[0] > e->lc_cap[0])) {
+    lio_set_last_error(__FILE__, __LINE__, "a cloud bound exceeds the local-cloud capacity (lio_est_enable_local_clouds)");
+    return LIO_ERR_CAPACITY;
+  }
+  e->frames_started = true;
+  e->scanned = true;
+  const int rc = compact_body(e, src, n3_dev, n_max, sum7);
+  if (rc != LIO_OK) { e->poisoned = true; std::snprintf(e->err, sizeof(e->err), "%s", lio_last_error()); }
+  return rc;
+}
+
+static int compact_check(lio_est *e) {
+  if (!e->mapping) { lio_set_last_error(__FILE__, __LINE__, "no mapping attached (lio_est_attach_mapping)"); return LIO_ERR_INVALID; }
+  return LIO_OK;
+}
+
+extern "C" int lio_est_process_compact_dev(lio_est *e, const float *corner_dev, const float *surf_dev, const float *full_dev, const int *n3_dev,
+                                           const int n3_max[3], const float transform_sum7[7]) {
+  if (!e || !n3_dev || !n3_max || !transform_sum7 || n3_max[0] < 0 || n3_max[1] < 0 || n3_max[2] < 0 || (n3_max[0] > 0 && !corner_dev) ||
+      (n3_max[1] > 0 && !surf_dev) || (n3_max[2] > 0 && !full_dev))
+    return LIO_ERR_INVALID;
+  int rc = compact_check(e);
+  if (rc != LIO_OK) return rc;
+  LIO_CUDA_OK(cudaSetDevice(e->device));
+  int n_max[3];
+  pm_est_caps(e->map, n3_max, n_max);
+  const float4 *src[3] = {reinterpret_cast<const float4 *>(corner_dev), reinterpret_cast<const float4 *>(surf_dev), reinterpret_cast<const float4 *>(full_dev)};
+  return compact_common(e, src, n3_dev, n_max, transform_sum7);
+}
+
+extern "C" int lio_est_process_compact_host(lio_est *e, const float *corner, int nc, const float *surf, int ns, const float *full, int nf,
+                                            const float transform_sum7[7]) {
+  if (!e || !transform_sum7 || nc < 0 || ns < 0 || nf < 0 || (nc > 0 && !corner) || (ns > 0 && !surf) || (nf > 0 && !full)) return LIO_ERR_INVALID;
+  int rc = compact_check(e);
+  if (rc != LIO_OK) return rc;
+  LIO_CUDA_OK(cudaSetDevice(e->device));
+  if (e->poisoned || nf > e->lc_cap[1] || ((e->cfg.enable_deskew || e->cfg.cutoff_deskew) && nc > e->lc_cap[0])) {
+    const int n_max[3] = {nc, ns, nf};
+    return compact_common(e, nullptr, nullptr, n_max, transform_sum7);
+  }
+  // the handle's input buffers are rewritten: the previous message's pushes (on the estimator's stream) read them
+  LIO_CUDA_OK(cudaStreamSynchronize(e->stream));
+  const float4 *src[3];
+  const int *n3_dev = nullptr;
+  if ((rc = pm_est_upload(e->map, corner, nc, surf, ns, full, nf, src, &n3_dev)) != LIO_OK) return rc;
+  const int n_max[3] = {nc, ns, nf};
+  return compact_common(e, src, n3_dev, n_max, transform_sum7);
+}
+
+extern "C" int lio_est_compact_status(lio_est *e, int info4[4]) {
+  if (!e || !info4) return LIO_ERR_INVALID;
+  int rc = compact_check(e);
+  if (rc != LIO_OK) return rc;
+  for (int k = 0; k < 4; ++k) info4[k] = e->compact_info[k];
+  return LIO_OK;
+}
+
 // The pre-integration buffer, the slot rotation and size_surf_stack advance before the fallible device work.  A failure
 // after that point leaves the window half-slid, so the context is poisoned: later calls return LIO_ERR_INVALID instead of
 // running on inconsistent state (documented in lio_b200.h).
@@ -2247,6 +2473,10 @@ static int process_scan_common(lio_est *e, const float4 *scan_dev, const int *n_
     return LIO_ERR_INVALID;
   }
   if (!e->tmp_pre) { lio_set_last_error(__FILE__, __LINE__, "process_scan before finish_init"); return LIO_ERR_INVALID; }
+  if (e->mapping) {
+    lio_set_last_error(__FILE__, __LINE__, "a mapping is attached: feed the odometry's clouds with lio_est_process_compact_*");
+    return LIO_ERR_INVALID;
+  }
   if (e->lc_on && !e->lc_staged) {   // before the window advances: the context stays usable
     lio_set_last_error(__FILE__, __LINE__, "local clouds are on: stage the scan's corner / full cloud with lio_est_set_scan_clouds_* first");
     std::snprintf(e->err, sizeof(e->err), "%s", lio_last_error());
@@ -2260,7 +2490,8 @@ static int process_scan_common(lio_est *e, const float4 *scan_dev, const int *n_
 }
 
 static int map_scan_entry(lio_est *e);
-static int process_scan_body(lio_est *e, const float4 *scan_dev, const int *n_dev, int n_max, bool open_only) {
+static void predict_state_w(lio_est *e);
+static int process_scan_body(lio_est *e, const float4 *scan_dev, const int *n_dev, int n_max, bool open_only, const CompactPush *cp) {
   const int W = e->W;
   cudaStream_t st = e->stream;
   marg_start(e);
@@ -2285,7 +2516,7 @@ static int process_scan_body(lio_est *e, const float4 *scan_dev, const int *n_de
   const float4 *src = scan_dev;
   // transform_es_ is computed whenever either flag is set (:628-664); the surf (and corner) clouds are de-skewed with it only
   // without cutoff_deskew (:666-673), the full cloud always (:2416, local clouds on)
-  const bool es_on = (e->cfg.enable_deskew || e->cfg.cutoff_deskew) && !e->imu_stamped.empty();
+  const bool es_on = (e->cfg.enable_deskew || e->cfg.cutoff_deskew) && !e->imu_stamped.empty() && !(cp && cp->startup);
   const bool deskew_surf = es_on && !e->cfg.cutoff_deskew;
   if (es_on) {
     // transform_es_ from the IMU-propagated poses of the last 0.1 s (:632-664), float Twist algebra on the host
@@ -2320,11 +2551,20 @@ static int process_scan_body(lio_est *e, const float4 *scan_dev, const int *n_de
     ++e->launches;
     src = e->d_scan;
   }
-  int rc = e->vg.run(src, n_dev, n_max, e->cfg.surf_filter_size, e->slot_ptr[slot], e->cfg.max_frame_points, e->d_slot_n + slot, nullptr, st, &e->launches);
-  if (rc != LIO_OK) return rc;
+  int rc = LIO_OK;
+  if (cp && cp->surf_ds) {
+    k_copy_cloud<<<std::max(1, std::min(e->sm_count * 2, (e->cfg.max_frame_points + 255) / 256)), 256, 0, st>>>(
+        cp->surf_ds, cp->surf_ds_n, e->cfg.max_frame_points, e->slot_ptr[slot], e->d_slot_n + slot);
+    ++e->launches;
+    EST_CUDA(cudaGetLastError());
+  } else {
+    rc = e->vg.run(src, n_dev, n_max, e->cfg.surf_filter_size, e->slot_ptr[slot], e->cfg.max_frame_points, e->d_slot_n + slot, nullptr, st, &e->launches);
+    if (rc != LIO_OK) return rc;
+  }
   EST_CUDA(cudaMemcpyAsync(e->d_own_n + slot, e->d_slot_n + slot, sizeof(int), cudaMemcpyDeviceToDevice, st));
-  if (e->lc_on && (rc = lc_push(e, deskew_surf)) != LIO_OK) return rc;
+  if (e->lc_on && (rc = lc_push(e, deskew_surf, cp && cp->corner_filtered)) != LIO_OK) return rc;
   push_shift(e->size_surf_stack, 0);
+  if (cp) predict_state_w(e);
   rc = scan_open_window(e);
   if (rc != LIO_OK || open_only) return rc;
   rc = scan_solve(e, e->cfg.max_num_iterations);

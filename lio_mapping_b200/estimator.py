@@ -352,6 +352,39 @@ class Estimator:
         _lib.check(_lib.lib().lio_est_map_poses(self.h, tobe, aft, ins, info), "lio_est_map_poses")
         return tobe, aft, ins, dict(inserted=bool(info[0]), points=int(info[1]), surround_published=bool(info[2]), surround_size=int(info[3]))
 
+    # ---- imu_factor = 0 from the odometry's clouds (lio_est_attach_mapping)
+    def attach_mapping(self, pm):
+        """Hand a fresh publishing PointMapping (EnablePublish done, no Process yet, same device) to an imu_factor = 0 estimator with
+        local clouds on, before anything else is fed.  From then on process_compact / process_compact_dev run the reference's
+        ProcessCompactData: PointMapping::Process on every message, the window of mapped poses, the start-up once it is full, and
+        afterwards the lidar-only solve with the map insert and publication on pm.  pm is refused its own calls until this
+        estimator is closed; the estimator keeps a reference to it."""
+        _lib.check(_lib.lib().lio_est_attach_mapping(self.h, pm.h), "lio_est_attach_mapping")
+        self._map = pm
+
+    def process_compact(self, corner_last, surf_last, full_cloud, transform_sum7):
+        """One /compact_data message from host arrays (the odometry's /laser_cloud_corner_last, /laser_cloud_surf_last, full cloud
+        and transform_sum_).  Returns compact_status()."""
+        arrs = [np.ascontiguousarray(a, np.float32).reshape(-1, 4) for a in (corner_last, surf_last, full_cloud)]
+        n = [a.shape[0] for a in arrs]
+        arrs = [a if a.shape[0] else np.zeros((1, 4), np.float32) for a in arrs]
+        _lib.check(_lib.lib().lio_est_process_compact_host(self.h, arrs[0], n[0], arrs[1], n[1], arrs[2], n[2],
+                                                           np.ascontiguousarray(transform_sum7, np.float32)), "lio_est_process_compact_host")
+        return self.compact_status()
+
+    def process_compact_dev(self, ptrs, n_dev_ptr: int, n_max, transform_sum7):
+        """The same with the clouds in HBM: exactly what PointOdometry.clouds_dev() returns (ptrs, n_dev_ptr, n_max)."""
+        _lib.check(_lib.lib().lio_est_process_compact_dev(self.h, C.c_void_p(ptrs[0]), C.c_void_p(ptrs[1]), C.c_void_p(ptrs[2]),
+                                                          C.c_void_p(n_dev_ptr), np.ascontiguousarray(n_max, np.int32),
+                                                          np.ascontiguousarray(transform_sum7, np.float32)), "lio_est_process_compact_dev")
+        return self.compact_status()
+
+    def compact_status(self):
+        """{inited, cir_buf_count, pushed, solved} of the last process_compact call."""
+        out = np.zeros(4, np.int32)
+        _lib.check(_lib.lib().lio_est_compact_status(self.h, out), "lio_est_compact_status")
+        return dict(inited=bool(out[0]), cir_buf_count=int(out[1]), pushed=bool(out[2]), solved=bool(out[3]))
+
     def summary(self):
         s = np.zeros(32)
         _lib.check(_lib.lib().lio_est_summary(self.h, s), "lio_est_summary")
