@@ -1,6 +1,6 @@
-// The device estimator's use of a publishing PointMapping's cube map after initialisation (lio_est_attach_map, estimator.cu):
+// The device estimator's use of a publishing PointMapping's cube map after initialisation (lio_est_attach_map, est_map.cu):
 // Estimator.cc:703-721 run UpdateMapDatabase and PublishResults of the PointMapping the estimator is.  The lio_pm handle stays
-// opaque to estimator.cu; these are the only entries it uses (cubemap.cu).
+// opaque to the estimator; these are the only entries it uses (cubemap.cu).
 #pragma once
 #include <cuda_runtime.h>
 #include <vector>

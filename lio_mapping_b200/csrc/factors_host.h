@@ -63,3 +63,8 @@ hm::V3 R2ypr(const hm::M3 &R);
 hm::M3 ypr2R(const hm::V3 &ypr);
 
 }  // namespace lio
+
+// The C-ABI's pre-integration handle (lio_pim_*): lio_est_init_frame takes over its pre-integration
+struct lio_pim {
+  std::shared_ptr<lio::Preintegration> p;
+};

@@ -1,15 +1,19 @@
 // lio_mapping_b200 — C-ABI seams of the host shell's dense fp64 kernels (hostmath.cc), so that the CPU test-suite can pin
 // them against LAPACK without a device: the blocked Cholesky used by the dogleg step (Ceres DENSE_SCHUR equivalent,
 // Estimator.cc:1909-1921) and the symmetric eigen-solver used by the marginalisation (Eigen::SelfAdjointEigenSolver call
-// sites MarginalizationFactor.cc:276, :293).
+// sites MarginalizationFactor.cc:276, :293).  Also the pre-integration handle (lio_pim_*) and the ImuFactor on it
+// (factors_host.cc), which lio_est_init_frame consumes.
 #include <cstring>
 #include "../../include/lio_b200.h"
+#include "factors_host.h"
 #include "hostmath.h"
 #include "solver_host.h"
 #include <cmath>
+#include <new>
 
 void lio_set_last_error(const char *file, int line, const char *msg);  // capi_common.cu
 
+using namespace lio;
 using namespace lio::hm;
 
 extern "C" int lio_host_cholesky_solve(int n, const double *A, const double *b, double *L_out, double *x) {
@@ -92,5 +96,46 @@ extern "C" int lio_host_dogleg_toy(int n, int m, const double *A, const double *
   for (int i = 0; i < n; ++i) x[i] = state[i];
   summary[0] = sum.iterations; summary[1] = sum.successful_steps; summary[2] = sum.termination;
   summary[3] = sum.initial_cost; summary[4] = sum.final_cost; summary[5] = sum.evaluations;
+  return LIO_OK;
+}
+
+// ---- IntegrationBase and ImuFactor (factors_host.cc) on a pre-integration handle
+extern "C" int lio_pim_create(const double a0[3], const double g0[3], const double ba[3], const double bg[3], const double n5[5], lio_pim **out) {
+  if (!a0 || !g0 || !ba || !bg || !n5 || !out) return LIO_ERR_INVALID;
+  ImuNoise nz;
+  nz.acc_n = n5[0]; nz.gyr_n = n5[1]; nz.acc_w = n5[2]; nz.gyr_w = n5[3]; nz.g_norm = n5[4];
+  lio_pim *p = new (std::nothrow) lio_pim();
+  if (!p) return LIO_ERR_INVALID;
+  p->p = std::make_shared<Preintegration>(V3(a0), V3(g0), V3(ba), V3(bg), nz);
+  *out = p;
+  return LIO_OK;
+}
+extern "C" int lio_pim_destroy(lio_pim *p) { delete p; return LIO_OK; }
+extern "C" int lio_pim_push_back(lio_pim *p, double dt, const double a[3], const double g[3]) {
+  if (!p || !a || !g) return LIO_ERR_INVALID;
+  p->p->push_back(dt, V3(a), V3(g));
+  return LIO_OK;
+}
+extern "C" int lio_pim_get(lio_pim *p, double *s, double *jac, double *cov) {
+  if (!p || !s) return LIO_ERR_INVALID;
+  const Preintegration &q = *p->p;
+  s[0] = q.delta_p.x; s[1] = q.delta_p.y; s[2] = q.delta_p.z; s[3] = q.delta_q.x; s[4] = q.delta_q.y; s[5] = q.delta_q.z; s[6] = q.delta_q.w;
+  s[7] = q.delta_v.x; s[8] = q.delta_v.y; s[9] = q.delta_v.z; s[10] = q.sum_dt;
+  if (jac) std::memcpy(jac, q.jac, sizeof(q.jac));
+  if (cov) std::memcpy(cov, q.cov, sizeof(q.cov));
+  return LIO_OK;
+}
+extern "C" int lio_imu_factor_evaluate(lio_pim *p, const double pose_i[7], const double sb_i[9], const double pose_j[7],
+                                       const double sb_j[9], double *res15, double *J0, double *J1, double *J2, double *J3) {
+  if (!p || !pose_i || !sb_i || !pose_j || !sb_j || !res15) return LIO_ERR_INVALID;
+  double Ji[15][6], Jsi[15][9], Jj[15][6], Jsj[15][9];
+  const bool need = J0 || J1 || J2 || J3;
+  imu_factor_evaluate(*p->p, pose_i, sb_i, pose_j, sb_j, res15, need ? Ji : nullptr, Jsi, Jj, Jsj);
+  if (need) {
+    for (int a = 0; a < 15; ++a) {
+      for (int c = 0; c < 7; ++c) { if (J0) J0[a * 7 + c] = c < 6 ? Ji[a][c] : 0.0; if (J2) J2[a * 7 + c] = c < 6 ? Jj[a][c] : 0.0; }
+      for (int c = 0; c < 9; ++c) { if (J1) J1[a * 9 + c] = Jsi[a][c]; if (J3) J3[a * 9 + c] = Jsj[a][c]; }
+    }
+  }
   return LIO_OK;
 }

@@ -1,6 +1,6 @@
 // Device pieces of Estimator::CalculateLaserOdom (src/imu_processor/Estimator.cc:1242-1359) and of the scan-to-map loops
 // built on it (PointMapping.cc:609-715, MapBuilder.cc:873-1011), shared by the stand-alone reduce / solve kernels
-// (estimator.cu) and by the fused tail of the k-NN kernel (knn.cu).  Compile the including unit with -fmad=false.
+// (odom.cu) and by the fused tail of the k-NN kernel (knn.cu).  Compile the including unit with -fmad=false.
 #pragma once
 #include "knn.cuh"
 #include "qr.cuh"
@@ -17,7 +17,7 @@ struct OdomState {
   unsigned counter;
 };
 
-// Workspace + driver of the scan-to-map optimisation on device-resident clouds (estimator.cu); shared by the host-array
+// Workspace + driver of the scan-to-map optimisation on device-resident clouds (odom.cu); shared by the host-array
 // parity entry lio_scan_to_map_host and by the cube-map context (cubemap.cu).
 struct ScanToMapWork {
   CellHash hc, hs;
@@ -35,6 +35,13 @@ struct ScanToMapWork {
 int scan_to_map_run(ScanToMapWork &W, const float4 *d_cmap, int Kc, const float4 *d_smap, int Ks, const float4 *d_corner, const int *d_nc,
                     int Mc_max, const float4 *d_surf, const int *d_ns, int Ms_max, float *tf7, float min_match_sq_dis, float min_plane_dis,
                     int max_iter, double delta_r_abort, double delta_t_abort, int variant, int *n_out, int *iters, int sm, cudaStream_t st);
+
+// Rounds [from, to) of CalculateLaserOdom (Estimator.cc:1242-1359) for the frame cloud surf (*n_dev points, at most n_bound)
+// against the map's hash, refining *tf_dev: the estimator's chain (build_local_map), which lio_laser_odom_host runs as well.  A
+// round after convergence is a no-op on the device (done flag).  `launches` (optional) counts the kernel launches.
+int odom_rounds(const CellHash &h, const float4 *surf, const int *n_dev, int n_bound, TransformF *tf_dev, const FeatureOut &fo,
+                bool keep_features, OdomState *odom, double *partial, KnnWork &work, float min_match_sq_dis, float min_plane_dis,
+                int from, int to, int sm, cudaStream_t q, int *launches);
 
 // rot.toRotationMatrix() of the (possibly un-normalised) float quaternion
 __device__ __forceinline__ void odom_rotation(const TransformF &tf, float (&R)[9]) {
