@@ -357,8 +357,9 @@ int lio_asm_stream_bench(long long n_features, int iters, int device, double out
  * fused kernel (default 1024, i.e. one log per 2048 features and thread). */
 int lio_asm_set_fold_chunks(int chunks);
 
-/* Test seam of the device-resident solver: solves A x = b (A symmetric positive definite, n x n row-major, n <= 216) with
- * the tiled shared-memory Cholesky (fp64 tensor-core MMA trailing update) that the dogleg step of the device solver uses
+/* Test seam of the device-resident solver: solves A x = b (A symmetric positive definite, n x n row-major, n <= 261) with
+ * the tiled shared-memory Cholesky (n <= 216: one CTA, as k_step; 217..261: a cluster of two CTAs whose shared memory holds
+ * the tiles together, as k_step_x2) (fp64 tensor-core MMA trailing update) that the dogleg step of the device solver uses
  * in place of Ceres' dense factorisation (Estimator.cc:1911 DENSE_SCHUR).  *ok = 0 when a pivot is not positive.
  * prof (optional, 4 * ceil(n / 8) + 1 entries): SM cycles per 8-column panel {panel solve, own tile update, diagonal-tile
  * factorisation, trailing update incl. barrier} as seen by the warp that runs the serial chain, then the back substitution. */
@@ -438,7 +439,9 @@ typedef struct lio_est_config {   /* EstimatorConfig (Estimator.h:77-108), lidar
   int max_scan_points;           /* capacity of the incoming laser_cloud_surf_last_ */
   int device_solver;             /* 1 (default): ImuFactor / marginalisation prior / PriorFactor evaluation, the dense normal
                                     equations, the tiled Cholesky and the dogleg controller all resident on the GPU (no host
-                                    sync inside a solve; opt windows up to 13); 0: host controller around the fused kernel */
+                                    sync inside a solve; opt windows up to 16: 14..16 on a two-CTA cluster, where the device
+                                    can hold one; otherwise, or with max_num_iterations > 22, the host controller);
+                                    0: host controller around the fused kernel */
   int overlap_marginalization;   /* 1 (default): the Schur-complement / eigen algebra of scan k's marginalisation runs on a
                                     worker thread beside scan k+1's device front end (started at that call's entry, joined
                                     before its solve); 0: inline at the end of scan k, the reference's order.  Same result. */
@@ -662,8 +665,9 @@ const char *lio_est_last_error(lio_est *est);
  * evaluation; row 16 = SM clock inside the lidar block expansion of evaluation 2 (entry, operands staged, S M, M^T (S M)).
  * Followed by 4 * 28 + 4 entries: the per-panel profile of evaluation 1's Cholesky in the layout of
  * lio_dev_cholesky_solve_host's prof (column 1 = %globaltimer at the start of the panel's diagonal tile), and after the back
- * substitution cycles four %globaltimer stamps (entry, loop start, loop end, exit).  cap >= 24 * 16 + 116.  Zeros when the host
- * controller is in use.  `LIO_BENCH_TRACE=1 python bench.py` prints it. */
+ * substitution cycles four %globaltimer stamps (entry, loop start, loop end, exit).  Opt windows 14..16 (29..33 panels) fill
+ * the 116 entries with panels 0..28 and leave out the back substitution and the four stamps.  cap >= 24 * 16 + 116.  Zeros
+ * when the host controller is in use.  `LIO_BENCH_TRACE=1 python bench.py` prints it. */
 int lio_est_solver_trace(lio_est *est, long long *out, int cap);
 /* CUDA-event timing of the fused residual+Jacobian kernel accumulated since the last reset (events recorded
  * on the estimator's stream around every launch): out[0..3] = {sum ms, launches, features processed, bytes/feature};

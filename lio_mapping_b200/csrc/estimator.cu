@@ -84,7 +84,7 @@ extern "C" void lio_est_default_config(lio_est_config *c) {
   c->acc_n = 0.2; c->gyr_n = 0.02; c->acc_w = 2e-4; c->gyr_w = 2e-5; c->g_norm = 9.805;
   c->max_num_iterations = 10; c->odom_max_iterations = 10;
   c->max_frame_points = 1 << 16; c->max_scan_points = 1 << 18;
-  c->device_solver = 1;   // GPU-resident dogleg loop (solver_dev.cu); 0 keeps the host controller (also used when O > 13)
+  c->device_solver = 1;   // GPU-resident dogleg loop (solver_dev.cu; O = 14..16 on a two-CTA cluster); 0 keeps the host controller
   c->overlap_marginalization = 1;
   c->solver_graph = 1;
   c->init_window_factor = 1;

@@ -19,12 +19,16 @@
 // one panel ahead (look-ahead, overlapped with the trailing update), the panel solve X = A L^-T and the trailing update
 // C -= X X^T are fp64 tensor-core MMAs (mma.sync m8n8k4, DMMA) - the one piece of the solver that is a genuine GEMM.
 // The right-hand side rides along as an extra row, so the forward substitution is free; the back substitution walks the
-// tiles in reverse.  n <= 216 (O <= 13) fits one SM; larger windows keep the host controller.
+// tiles in reverse.  n <= 216 (O <= 13) fits one SM (k_step).  O = 14..16 (n <= 261, 33 tile columns, 299 KiB) runs the
+// same step body as k_step_x2, a cluster of two CTAs: rank 0 computes, rank 1 lends its shared memory for half of the
+// off-diagonal tiles, which rank 0 reaches over DSMEM (OneCta / TwoCta below decide where each tile lives).
 #include "solver_dev.cuh"
 #include <algorithm>
+#include <cooperative_groups.h>
 
 namespace lio {
 using namespace hm;
+namespace cg = cooperative_groups;
 
 constexpr int kDsThreads = 512;   // 128 registers per thread: the serial diagonal-tile chain lives entirely in one lane's registers
 constexpr int kDsWarps = kDsThreads / 32;
@@ -212,6 +216,50 @@ k_factors(DevSolveState *__restrict__ S, const double *__restrict__ Hp, FPtrs F,
 __device__ __forceinline__ int tile_off(int ib, int jb) { return (ib * (ib + 1) / 2 + jb) * 64; }
 __device__ __forceinline__ int swz(int r, int c) { return r * 8 + (c ^ ((r & 2) << 1)); }
 
+// Where tile (ib, jb) of the lower triangle lives: every phase that touches the Cholesky tiles addresses them through one
+// of these two maps.  `tiles` is the CTA's own dynamic shared memory.
+struct OneCta {   // k_step: all tiles packed row by row in the CTA's own shared memory (rows contiguous)
+  static constexpr bool kCluster = false;
+  static constexpr int kRowSlices = 7;    // 32-column slices of an Hpart row (n <= 224)
+  static constexpr int kLidarLoads = 4;   // staged lidar operands per thread: O * 140 <= 4 * 512
+  static constexpr int kBackWarps = 8;    // warps of the back substitution: 8 NB <= 256 rows
+  template <class T> __device__ __forceinline__ static T *at(T *tiles, int ib, int jb) { return tiles + tile_off(ib, jb); }
+  __device__ __forceinline__ static size_t local_doubles(int NB) { return (size_t)(NB * (NB + 1) / 2) * 64; }
+  __device__ __forceinline__ static bool prof_fits(int, int) { return true; }
+};
+
+// Address of tile (ib, jb) under the map TP, in a function whose tile base is `tiles`.  A macro, not a call, so that for
+// OneCta the expression is exactly the one the one-CTA kernels were written with (going through an inline function
+// perturbed their instruction selection).
+#define TILE(ib, jb) (TP::kCluster ? TP::at(tiles, ib, jb) : tiles + tile_off(ib, jb))
+
+// k_step_x2 / k_chol_test_x2 (n <= 261, NB <= 33): rank 0 keeps the diagonal tiles (ib, ib) and the first sub-diagonal
+// tiles (ib + 1, ib) - every tile the serial chain warp touches - and the remaining tiles of the odd tile rows; rank 1 holds
+// the remaining tiles of the even tile rows.  Per CTA at NB = 33: rank 0 33 + 32 + 240 tiles (156 KiB) + the vectors, rank 1
+// 256 tiles (128 KiB).  Layout (fixed, independent of NB), in tiles:
+//   rank 0: [diagonal ib: 0..32][sub-diagonal (jb + 1, jb): 33..64][odd row ib = 2k + 1, jb <= ib - 2: 65 + k (k - 1) + jb]
+//   rank 1: [even row ib = 2k, jb <= ib - 2: (k - 1)^2 + jb]
+// Only rank 0's threads read or write tiles, so the CTA barriers that separate its phases order the remote accesses as well
+// (the PTX memory model scopes a barrier by the threads that take part, not by where the location lives); rank 1's shared
+// memory is live from the cluster barrier at kernel entry to the one at exit.
+struct TwoCta {
+  static constexpr bool kCluster = true;
+  static constexpr int kRowSlices = 9;    // n <= 288
+  static constexpr int kLidarLoads = 5;   // O * 140 <= 5 * 512
+  static constexpr int kBackWarps = 9;    // 8 NB <= 288 rows
+  static constexpr int kMaxNB = 33;
+  static constexpr int kLocalTiles = 2 * kMaxNB - 1 + 240, kPeerTiles = 256;
+  template <class T> __device__ __forceinline__ static T *at(T *tiles, int ib, int jb) {
+    const int d = ib - jb, k = ib >> 1;
+    if (d == 0) return tiles + 64 * ib;
+    if (d == 1) return tiles + 64 * (kMaxNB + jb);
+    if (ib & 1) return tiles + 64 * (2 * kMaxNB - 1 + k * (k - 1) + jb);
+    return cg::this_cluster().map_shared_rank(tiles, 1) + 64 * ((k - 1) * (k - 1) + jb);
+  }
+  __device__ __forceinline__ static size_t local_doubles(int) { return (size_t)kLocalTiles * 64; }
+  __device__ __forceinline__ static bool prof_fits(int slot, int cap) { return slot < cap; }
+};
+
 __device__ __forceinline__ void dmma884(double &d0, double &d1, double a, double b) {
   asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};" : "+d"(d0), "+d"(d1) : "d"(a), "d"(b));
 }
@@ -287,23 +335,25 @@ __device__ __forceinline__ long long clock_after(double v) {
 }
 
 // Factors the tiled matrix in place (strictly-lower tiles: L; diagonal tiles: inv(L_kk)) and overwrites y (padded to
-// 8 NB) with the solution of (L L^T) x = y.  Returns 1 on success; uniform.
-__device__ int chol_solve_tiles(double *tiles, int NB, double *y, int *s_ok, long long *prof = nullptr) {
+// 8 NB) with the solution of (L L^T) x = y.  Returns 1 on success; uniform over the CTA (and, since only rank 0 of a
+// cluster calls it, over the cluster).  TwoCta: profile slots >= prof_cap are not written.
+template <class TP>
+__device__ int chol_solve_tiles(double *tiles, int NB, double *y, int *s_ok, long long *prof = nullptr, int prof_cap = 0) {
   const int tid = threadIdx.x, w = warp_id(), l = lane_id();
   const int fr = l >> 2, fq = l & 3;   // fragment row, fragment quad
-  if (prof && tid == 0) prof[4 * NB + 1] = gtime_ns();
+  if (prof && tid == 0 && TP::prof_fits(4 * NB + 1, prof_cap)) prof[4 * NB + 1] = gtime_ns();
   if (tid == 0) *s_ok = 1;
   __syncthreads();
   // The serial chain (diagonal tiles) runs on the LAST warp: the issue arbiter favours the highest warp id of a
   // scheduler, so the chain is never starved by the seven update warps it shares its scheduler with.
   constexpr int kChainWarp = kDsWarps - 1;
-  if (w == kChainWarp) diag_factor(tiles + tile_off(0, 0), s_ok);
+  if (w == kChainWarp) diag_factor(TILE(0, 0), s_ok);
   __syncthreads();
-  if (prof && w == kChainWarp && l == 0) prof[4 * NB + 2] = gtime_ns();
+  if (prof && w == kChainWarp && l == 0 && TP::prof_fits(4 * NB + 2, prof_cap)) prof[4 * NB + 2] = gtime_ns();
   for (int kb = 0; kb < NB; ++kb) {
     if (!*s_ok) break;
     const long long tp0 = clock_after(y[0]);
-    const double *Li = tiles + tile_off(kb, kb);   // inv(L_kk)
+    const double *Li = TILE(kb, kb);   // inv(L_kk)
     const int m = NB - 1 - kb;
     // ---- panel solve: X = A inv(L)^T for the tiles below the diagonal; y_kb = inv(L) y_kb.  The chain warp takes the first
     // tile and at once applies it to the next diagonal tile, so that after the barrier it can start factoring immediately
@@ -311,14 +361,14 @@ __device__ int chol_solve_tiles(double *tiles, int NB, double *y, int *s_ok, lon
     const double b0 = Li[swz(fr, fq)], b1 = Li[swz(fr, fq + 4)];
     if (w == kChainWarp) {
       if (m > 0) {
-        double *A = tiles + tile_off(kb + 1, kb);
+        double *A = TILE(kb + 1, kb);
         const double a0 = A[swz(fr, fq)], a1 = A[swz(fr, fq + 4)];
         double d0 = 0.0, d1 = 0.0;
         dmma884(d0, d1, a0, b0);
         dmma884(d0, d1, a1, b1);
         *reinterpret_cast<double2 *>(A + swz(fr, 2 * fq)) = make_double2(d0, d1);
         __syncwarp();
-        double *C = tiles + tile_off(kb + 1, kb + 1);
+        double *C = TILE(kb + 1, kb + 1);
         const double x0 = A[swz(fr, fq)], x1 = A[swz(fr, fq + 4)];
         double2 c = *reinterpret_cast<double2 *>(C + swz(fr, 2 * fq));
         dmma884(c.x, c.y, -x0, x0);
@@ -327,7 +377,7 @@ __device__ int chol_solve_tiles(double *tiles, int NB, double *y, int *s_ok, lon
       }
     } else {
       for (int t = 1 + w; t < m; t += kDsWarps - 1) {
-        double *A = tiles + tile_off(kb + 1 + t, kb);
+        double *A = TILE(kb + 1 + t, kb);
         const double a0 = A[swz(fr, fq)], a1 = A[swz(fr, fq + 4)];
         double d0 = 0.0, d1 = 0.0;
         dmma884(d0, d1, a0, b0);
@@ -346,15 +396,15 @@ __device__ int chol_solve_tiles(double *tiles, int NB, double *y, int *s_ok, lon
     }
     __syncthreads();
     const long long tp1 = clock_after(y[8 * kb]);      // y_kb was written by warp 0 before the barrier: really after release
-    if (prof && w == kChainWarp && l == 0) prof[4 * kb + 0] = tp1 - tp0;
+    if (prof && w == kChainWarp && l == 0 && TP::prof_fits(4 * kb + 3, prof_cap)) prof[4 * kb + 0] = tp1 - tp0;
     if (m == 0) break;
     // ---- trailing update C(i, j) -= X_i X_j^T, right-hand side rows, and the next diagonal tile one panel ahead
     const int ntile = m * (m + 1) / 2;
     if (w == kChainWarp) {
-      double *C = tiles + tile_off(kb + 1, kb + 1);
+      double *C = TILE(kb + 1, kb + 1);
       const long long td0 = clock64();
       diag_factor(C, s_ok);
-      if (prof && l == 0) { prof[4 * kb + 1] = gtime_ns(); prof[4 * kb + 2] = clock64() - td0; }
+      if (prof && l == 0 && TP::prof_fits(4 * kb + 3, prof_cap)) { prof[4 * kb + 1] = gtime_ns(); prof[4 * kb + 2] = clock64() - td0; }
     } else if ((w & 3) != (kChainWarp & 3)) {
       // tile tasks p = 1 .. ntile - 1: tile (i, j) with p = i (i + 1) / 2 + j (p = 0 is the next diagonal tile: the chain warp's).
       // The warps that share the chain warp's scheduler (w % 4 == 3) take no tasks: their fp64 MMAs would queue in front of
@@ -367,6 +417,7 @@ __device__ int chol_solve_tiles(double *tiles, int NB, double *y, int *s_ok, lon
       const int ntask = ntile - 1;                               // tile tasks p = 1 .. ntile - 1
       const int per = (ntask + kWorkers - 1) / kWorkers;
       const int p0 = 1 + wi * per, p1 = min(ntile, p0 + per);
+      if constexpr (!TP::kCluster) {
       if (p0 < p1) {
         int i = (int)((sqrt(8.0 * p0 + 1.0) - 1.0) * 0.5);
         while ((i + 1) * (i + 2) / 2 <= p0) ++i;
@@ -402,11 +453,45 @@ __device__ int chol_solve_tiles(double *tiles, int NB, double *y, int *s_ok, lon
           j = 0; ++i;
         }
       }
+      } else if (p0 < p1) {
+        // TwoCta: the same walk, every tile address from the map (a row's tiles are spread over both CTAs)
+        int i = (int)((sqrt(8.0 * p0 + 1.0) - 1.0) * 0.5);
+        while ((i + 1) * (i + 2) / 2 <= p0) ++i;
+        while (i * (i + 1) / 2 > p0) --i;
+        int j = p0 - i * (i + 1) / 2;
+        const int o0 = swz(fr, fq), o1 = swz(fr, fq + 4), oc = swz(fr, 2 * fq);
+        for (int p = p0; p < p1;) {
+          const int jend = min(i, j + (p1 - p) - 1);
+          const double *Xi = TILE(kb + 1 + i, kb);
+          const double a0 = -Xi[o0], a1 = -Xi[o1];
+          double *Cp = TILE(kb + 1 + i, kb + 1 + j) + oc;
+          const double *xp = TILE(kb + 1 + j, kb);
+          double x0 = xp[o0], x1 = xp[o1];
+          double2 c = *reinterpret_cast<double2 *>(Cp);
+          for (int jj = j; jj <= jend; ++jj) {
+            const bool more = jj < jend;
+            double *Cn = Cp;
+            double nx0 = 0.0, nx1 = 0.0;
+            double2 nc = make_double2(0.0, 0.0);
+            if (more) {
+              const double *xn = TILE(kb + 2 + jj, kb);
+              Cn = TILE(kb + 1 + i, kb + 2 + jj) + oc;
+              nx0 = xn[o0]; nx1 = xn[o1]; nc = *reinterpret_cast<double2 *>(Cn);
+            }
+            dmma884(c.x, c.y, a0, x0);
+            dmma884(c.x, c.y, a1, x1);
+            *reinterpret_cast<double2 *>(Cp) = c;
+            Cp = Cn; x0 = nx0; x1 = nx1; c = nc;
+          }
+          p += jend - j + 1;
+          j = 0; ++i;
+        }
+      }
       // right-hand side rows of tile-row r (r = 0 .. m - 1), one per worker in turn
       if (l < 8) {
         for (int r = wi; r < m; r += kWorkers) {
           const int ib = kb + 1 + r;
-          const double *X = tiles + tile_off(ib, kb);
+          const double *X = TILE(ib, kb);
           double s = 0.0;
 #pragma unroll
           for (int k = 0; k < 8; ++k) s += X[swz(l, k)] * y[8 * kb + k];
@@ -415,20 +500,20 @@ __device__ int chol_solve_tiles(double *tiles, int NB, double *y, int *s_ok, lon
       }
     }
     __syncthreads();
-    if (prof && w == kChainWarp && l == 0) prof[4 * kb + 3] = clock_after(y[8 * (kb + 1)]) - tp1;
+    if (prof && w == kChainWarp && l == 0 && TP::prof_fits(4 * kb + 3, prof_cap)) prof[4 * kb + 3] = clock_after(y[8 * (kb + 1)]) - tp1;
   }
   __syncthreads();
   const int ok = *s_ok;
   if (!ok) return 0;
   const long long tb0 = clock64();
-  if (prof && w == kChainWarp && l == 0) prof[4 * NB + 3] = gtime_ns();
-  // ---- back substitution L^T x = y over the tiles in reverse.  Only the first 8 warps take part (8 NB <= 256 rows): the
+  if (prof && w == kChainWarp && l == 0 && TP::prof_fits(4 * NB + 3, prof_cap)) prof[4 * NB + 3] = gtime_ns();
+  // ---- back substitution L^T x = y over the tiles in reverse.  Only the first kBackWarps warps take part (8 NB rows): the
   // 8 threads of tile-row jb turn their finished y into x = inv(L_jj)^T y (they share a warp), one named barrier
   // publishes x, then every thread of the rows above subtracts its tile's contribution.
-  if (w < 8) {
+  if (w < TP::kBackWarps) {
     for (int jb = NB - 1; jb >= 0; --jb) {
       if ((tid >> 3) == jb) {
-        const double *Li = tiles + tile_off(jb, jb);
+        const double *Li = TILE(jb, jb);
         const int c = tid & 7;
         __syncwarp(0xffu << (l & 24));
         double v0 = 0.0, v1 = 0.0;
@@ -442,11 +527,11 @@ __device__ int chol_solve_tiles(double *tiles, int NB, double *y, int *s_ok, lon
       }
       double lt[8];   // this thread's column of tile (jb, ib): independent of x, fetched before the barrier
       if (tid < 8 * jb) {
-        const double *Lt = tiles + tile_off(jb, tid >> 3);
+        const double *Lt = TILE(jb, tid >> 3);
 #pragma unroll
         for (int r = 0; r < 8; ++r) lt[r] = Lt[swz(r, tid & 7)];
       }
-      asm volatile("bar.sync 1, 256;" ::: "memory");
+      asm volatile("bar.sync 1, %0;" :: "n"(32 * TP::kBackWarps) : "memory");
       if (tid < 8 * jb) {
         double s0 = 0.0, s1 = 0.0;
 #pragma unroll
@@ -456,7 +541,7 @@ __device__ int chol_solve_tiles(double *tiles, int NB, double *y, int *s_ok, lon
     }
   }
   __syncthreads();
-  if (prof && tid == 0) { const long long te = clock_after(y[0]); prof[4 * NB] = te - tb0; prof[4 * NB + 4] = gtime_ns(); }
+  if (prof && tid == 0 && TP::prof_fits(4 * NB + 4, prof_cap)) { const long long te = clock_after(y[0]); prof[4 * NB] = te - tb0; prof[4 * NB + 4] = gtime_ns(); }
   return 1;
 }
 
@@ -622,15 +707,16 @@ __device__ __forceinline__ double lidar_g(const GatherCtx &c, int ba, int sa) {
 // (M_i: 108 doubles, S_i: 29) are staged in shared memory first and every product runs from there: the three phases used to
 // fetch their operands from global memory one dependent round trip after the other (4.8 us for 10 frames).
 // scratch: >= O * (108 + 32 + 108 + 342) doubles of shared memory (the Cholesky tiles are not in use yet).
+template <int kLoads>
 __device__ void lidar_blocks(int O, const double *__restrict__ Sblk, const double *__restrict__ FM, double *G, double *G0, double *scratch, long long *marks = nullptr) {
   const int tid = threadIdx.x, T = blockDim.x;
   if (marks && tid == 0) marks[0] = clock64();
   double *sM = scratch, *sS = sM + O * 108, *sSM = sS + O * 32, *sG = sSM + O * 108;
-  {   // all of a thread's loads are issued before the first store (O <= 13: at most four per thread)
-    double v[4];
-    int dst[4];
+  {   // all of a thread's loads are issued before the first store (O * 140 <= kLoads * 512)
+    double v[kLoads];
+    int dst[kLoads];
 #pragma unroll
-    for (int k = 0; k < 4; ++k) {
+    for (int k = 0; k < kLoads; ++k) {
       const int p = tid + k * T;
       dst[k] = -1; v[k] = 0.0;
       if (p < O * 140) {
@@ -640,7 +726,7 @@ __device__ void lidar_blocks(int O, const double *__restrict__ Sblk, const doubl
       }
     }
 #pragma unroll
-    for (int k = 0; k < 4; ++k) if (dst[k] >= 0) scratch[dst[k]] = v[k];
+    for (int k = 0; k < kLoads; ++k) if (dst[k] >= 0) scratch[dst[k]] = v[k];
   }
   __syncthreads();
   if (marks && threadIdx.x == 0) marks[1] = clock_after(scratch[0]);
@@ -705,9 +791,45 @@ __device__ void lidar_blocks(int O, const double *__restrict__ Sblk, const doubl
 }
 
 // y = H v with H the symmetric matrix whose lower triangle sits in the (unfactored) tiles; v, y in shared memory.
-// Two threads per row, each over every other column (needs n <= blockDim.x / 2); the tile address advances
-// incrementally along the row / down the column.
+// Two threads per row, each over every other column; the tile address advances incrementally along the row / down the
+// column.  OneCta: n <= blockDim.x / 2.  TwoCta: rows a and a + blockDim.x / 2, every tile address from the map.
+template <class TP>
 __device__ void symv_tiles(const double *tiles, int n, const double *v, double *y) {
+  if constexpr (TP::kCluster) {
+    const int q = threadIdx.x & 1;
+    for (int a0 = 0; a0 < n; a0 += blockDim.x >> 1) {   // uniform trip count: the shuffle below has every lane
+      const int a = a0 + (threadIdx.x >> 1);
+      double s0 = 0.0, s1 = 0.0;
+      if (a < n) {
+        const int ta = a >> 3, ra = a & 7;
+        for (int jb = 0; jb < ta; ++jb) {
+          const double *row = TILE(ta, jb);
+#pragma unroll
+          for (int c = 0; c < 8; c += 4) {
+            s0 += row[swz(ra, c + q)] * v[8 * jb + c + q];
+            s1 += row[swz(ra, c + 2 + q)] * v[8 * jb + c + 2 + q];
+          }
+        }
+        const double *row = TILE(ta, ta);
+        for (int c = q; c <= ra; c += 2) s0 += row[swz(ra, c)] * v[8 * ta + c];
+        for (int r = ra + 1 + q; r < 8 && 8 * ta + r < n; r += 2) s1 += row[swz(r, ra)] * v[8 * ta + r];
+        const int NB = (n + 7) >> 3;
+        for (int ib = ta + 1; ib < NB; ++ib) {
+          const double *col = TILE(ib, ta);
+#pragma unroll
+          for (int r = 0; r < 8; r += 4) {
+            s0 += col[swz(r + q, ra)] * v[8 * ib + r + q];
+            s1 += col[swz(r + 2 + q, ra)] * v[8 * ib + r + 2 + q];
+          }
+        }
+      }
+      double s = s0 + s1;
+      s += __shfl_xor_sync(0xffffffffu, s, 1);
+      if (a < n && q == 0) y[a] = s;
+    }
+    __syncthreads();
+    return;
+  }
   const int a = threadIdx.x >> 1, q = threadIdx.x & 1;
   double s0 = 0.0, s1 = 0.0;
   if (a < n) {
@@ -753,9 +875,40 @@ __device__ __forceinline__ void copy_tiles(double *__restrict__ dst, const doubl
   }
   for (; k < n2; k += T) d2[k] = s2[k];
 }
+// Copy between a global tile set in the canonical layout (tile_off) and the tiles where TP keeps them.  OneCta: one flat
+// copy.  TwoCta: the same 16-byte accesses, eight in flight, each shared-memory address from the map.
+__device__ __forceinline__ int tile_row(int t) {   // ib of the canonical tile index t = ib (ib + 1) / 2 + jb
+  int ib = (int)((sqrt(8.0 * t + 1.0) - 1.0) * 0.5);
+  while ((ib + 1) * (ib + 2) / 2 <= t) ++ib;
+  while (ib * (ib + 1) / 2 > t) --ib;
+  return ib;
+}
+template <class TP> __device__ __forceinline__ double2 *tile_vec(double *tiles, int k) {   // 16-byte word k of the canonical set
+  const int t = k >> 5, ib = tile_row(t);
+  return reinterpret_cast<double2 *>(TILE(ib, t - ib * (ib + 1) / 2)) + (k & 31);
+}
+template <class TP, bool kLoad>
+__device__ __forceinline__ void copy_tiles_map(double *tiles, double *glob, int ntd) {   // ntd = tiles x 64
+  if constexpr (!TP::kCluster) {
+    if (kLoad) copy_tiles(tiles, glob, ntd); else copy_tiles(glob, tiles, ntd);
+  } else {
+    const int n2 = ntd >> 1, T = blockDim.x;
+    double2 *g2 = reinterpret_cast<double2 *>(glob);
+    int k = threadIdx.x;
+    for (; k + 7 * T < n2; k += 8 * T) {
+      double2 v[8];
+#pragma unroll
+      for (int q = 0; q < 8; ++q) v[q] = kLoad ? g2[k + q * T] : *tile_vec<TP>(tiles, k + q * T);
+#pragma unroll
+      for (int q = 0; q < 8; ++q) { if (kLoad) *tile_vec<TP>(tiles, k + q * T) = v[q]; else g2[k + q * T] = v[q]; }
+    }
+    for (; k < n2; k += T) { if (kLoad) *tile_vec<TP>(tiles, k) = g2[k]; else g2[k] = *tile_vec<TP>(tiles, k); }
+  }
+}
 // (re)load the pure scaled H of the current x (tile layout, saved by the evaluation that built it)
+template <class TP>
 __device__ void refill_tiles(double *tiles, const double *__restrict__ HsT, int ntd) {
-  copy_tiles(tiles, HsT, ntd);
+  copy_tiles_map<TP, true>(tiles, const_cast<double *>(HsT), ntd);
   __syncthreads();
 }
 
@@ -774,6 +927,7 @@ struct StepShared {
   int flag[4], ok, pim_valid[kMaxOpt];
 };
 
+template <class TP>
 __device__ void step_body(DevSolveState *S, StepShared &sh, double *dsm, double *Hs, const double *__restrict__ Hp, double *H0, double *g0,
                           const double *__restrict__ Sblk, FPtrs F, const double *__restrict__ Hpart, const double *__restrict__ HpartT, double *Rt,
                           int eval_index) {
@@ -787,7 +941,7 @@ __device__ void step_body(DevSolveState *S, StepShared &sh, double *dsm, double 
   const int O = sc.O, n = sc.n;
   const int NB = (n + 7) / 8, NP = NB * 8, ntd = (NB * (NB + 1) / 2) * 64;
   double *tiles = dsm;
-  double *v_g = dsm + (size_t)(NB * (NB + 1) / 2) * 64;   // scaled gradient of the current x
+  double *v_g = dsm + TP::local_doubles(NB);   // scaled gradient of the current x
   double *v_scale = v_g + NP, *v_diag = v_scale + NP, *v_grad = v_diag + NP, *v_gn = v_grad + NP, *v_step = v_gn + NP;
   double *v_tmp = v_step + NP, *v_y = v_tmp + NP, *v_hsg = v_y + NP;
   const double min_diagonal = 1e-6, max_diagonal = 1e32, min_mu = 1e-8, max_mu = 1.0, mu_factor = 10.0;
@@ -885,7 +1039,7 @@ __device__ void step_body(DevSolveState *S, StepShared &sh, double *dsm, double 
 
   if (build) {
     // ---------------- normal equations at the new current point ----------------
-    if (gc.lidar) lidar_blocks(O, Sblk, F.M, G, G0, tiles, eval_index == 2 ? &S->dbg[16][0] : nullptr);
+    if (gc.lidar) lidar_blocks<TP::kLidarLoads>(O, Sblk, F.M, G, G0, tiles, eval_index == 2 ? &S->dbg[16][0] : nullptr);
     DS_MARK(3);
     // unscaled diagonal, gradient; Jacobi scaling is fixed at iteration zero
     // k_hpart's gather is usable when it assumed the structure that is in force now (the gates may have changed it)
@@ -931,7 +1085,7 @@ __device__ void step_body(DevSolveState *S, StepShared &sh, double *dsm, double 
     if (fast && eval_index >= 1 && gpart[n + 2] != 0.0) {
       // k_hpart left the scaled lidar-independent share in tile layout: one coalesced copy, then the lidar entries (pose rows
       // and the free extrinsic only: <= 72 x 72 / 2 candidates) are added in place
-      copy_tiles(tiles, HpartT, ntd);
+      copy_tiles_map<TP, true>(tiles, const_cast<double *>(HpartT), ntd);
       __syncthreads();
       if (gc.lidar) {
         // the structurally non-zero lidar entries only: per frame the 6 pose_i rows against [pose_0 | pose_i | extrinsic]
@@ -939,7 +1093,7 @@ __device__ void step_body(DevSolveState *S, StepShared &sh, double *dsm, double 
         // their loads independent
         const int total = O * 108 + 144;
 #pragma unroll
-        for (int k = 0; k < 4; ++k) {   // O <= 13: 1548 candidates <= 4 x 512
+        for (int k = 0; k < 4; ++k) {   // O <= 16: 1872 candidates <= 4 x 512
           const int e = tid + k * kDsThreads;
           if (e >= total) continue;
           int a, b;
@@ -958,12 +1112,12 @@ __device__ void step_body(DevSolveState *S, StepShared &sh, double *dsm, double 
           int sa = 0;
           const int ba = lidar_block(gc, a, sa);
           const double lh = lidar_h(gc, ba, sa, b);
-          if (lh != 0.0) tiles[tile_off(a >> 3, b >> 3) + swz(a & 7, b & 7)] += lh * v_scale[a] * v_scale[b];
+          if (lh != 0.0) TILE(a >> 3, b >> 3)[swz(a & 7, b & 7)] += lh * v_scale[a] * v_scale[b];
         }
         __syncthreads();
       }
       for (int a = tid; a < n; a += T) {
-        const double d = sqrt(fmin(fmax(tiles[tile_off(a >> 3, a >> 3) + swz(a & 7, a & 7)], min_diagonal), max_diagonal));
+        const double d = sqrt(fmin(fmax(TILE(a >> 3, a >> 3)[swz(a & 7, a & 7)], min_diagonal), max_diagonal));
         v_diag[a] = d; S->diagonal[a] = d;
       }
     } else if (fast) {
@@ -971,17 +1125,17 @@ __device__ void step_body(DevSolveState *S, StepShared &sh, double *dsm, double 
       const int l = lane_id();
       for (int a = warp_id(); a < NP; a += kDsWarps) {
         if (a >= n) {   // padding rows: identity
-          for (int b2 = l; b2 <= a; b2 += 32) tiles[tile_off(a >> 3, b2 >> 3) + swz(a & 7, b2 & 7)] = (a == b2) ? 1.0 : 0.0;
+          for (int b2 = l; b2 <= a; b2 += 32) TILE(a >> 3, b2 >> 3)[swz(a & 7, b2 & 7)] = (a == b2) ? 1.0 : 0.0;
           continue;
         }
         int sa = 0;
         const int ba = gc.lidar ? lidar_block(gc, a, sa) : -1;
         const double sca = v_scale[a];
-        double hq[7];
+        double hq[TP::kRowSlices];
 #pragma unroll
-        for (int q = 0; q < 7; ++q) { const int b = l + 32 * q; hq[q] = (b <= a) ? Hpart[(size_t)a * n + b] : 0.0; }
+        for (int q = 0; q < TP::kRowSlices; ++q) { const int b = l + 32 * q; hq[q] = (b <= a) ? Hpart[(size_t)a * n + b] : 0.0; }
 #pragma unroll
-        for (int q = 0; q < 7; ++q) {
+        for (int q = 0; q < TP::kRowSlices; ++q) {
           const int b = l + 32 * q;
           if (b > a) continue;
           const double h = hq[q] + (ba >= 0 ? lidar_h(gc, ba, sa, b) : 0.0);
@@ -991,7 +1145,7 @@ __device__ void step_body(DevSolveState *S, StepShared &sh, double *dsm, double 
             const double d = sqrt(fmin(fmax(hs, min_diagonal), max_diagonal));
             v_diag[a] = d; S->diagonal[a] = d;
           }
-          tiles[tile_off(a >> 3, b >> 3) + swz(a & 7, b & 7)] = hs;
+          TILE(a >> 3, b >> 3)[swz(a & 7, b & 7)] = hs;
         }
       }
     } else {
@@ -1049,15 +1203,15 @@ __device__ void step_body(DevSolveState *S, StepShared &sh, double *dsm, double 
             const double d = sqrt(fmin(fmax(hs, min_diagonal), max_diagonal));
             v_diag[ga] = d; S->diagonal[ga] = d;
           }
-          tiles[tile_off(ga >> 3, gb >> 3) + swz(ga & 7, gb & 7)] = hs;
+          TILE(ga >> 3, gb >> 3)[swz(ga & 7, gb & 7)] = hs;
         }
       }
       for (int a2 = n + warp_id(); a2 < NP; a2 += kDsWarps)   // padding rows: identity
-        for (int b2 = l; b2 <= a2; b2 += 32) tiles[tile_off(a2 >> 3, b2 >> 3) + swz(a2 & 7, b2 & 7)] = (a2 == b2) ? 1.0 : 0.0;
+        for (int b2 = l; b2 <= a2; b2 += 32) TILE(a2 >> 3, b2 >> 3)[swz(a2 & 7, b2 & 7)] = (a2 == b2) ? 1.0 : 0.0;
     }
     tiles_ready = 1;
     __syncthreads();
-    copy_tiles(Hs, tiles, ntd);   // kept for a mu retry / an invalid step of a later evaluation (plain stores, nobody waits for them)
+    copy_tiles_map<TP, false>(tiles, Hs, ntd);   // kept for a mu retry / an invalid step of a later evaluation (plain stores, nobody waits for them)
     for (int i = tid; i < n; i += T) { v_grad[i] = v_g[i] / v_diag[i]; S->gradient[i] = v_grad[i]; }
     __syncthreads();
     DS_MARK(5);
@@ -1078,10 +1232,10 @@ __device__ void step_body(DevSolveState *S, StepShared &sh, double *dsm, double 
     int linear_ok = 1;
     if (!s_flag[3]) {
       // Cauchy point scale: alpha = |gradient|^2 / (sg^T H sg), sg = gradient / D; H sg is kept (model cost change)
-      if (!tiles_ready) refill_tiles(tiles, Hs, ntd);
+      if (!tiles_ready) refill_tiles<TP>(tiles, Hs, ntd);
       for (int i = tid; i < NP; i += T) v_tmp[i] = i < n ? v_g[i] / (v_diag[i] * v_diag[i]) : 0.0;
       __syncthreads();
-      symv_tiles(tiles, n, v_tmp, v_hsg);
+      symv_tiles<TP>(tiles, n, v_tmp, v_hsg);
       double pa = 0, pb = 0, pc = 0;
       for (int i = tid; i < n; i += T) { pa += v_grad[i] * v_grad[i]; pb += v_tmp[i] * v_hsg[i]; S->hsg[i] = v_hsg[i]; }
       block_sum3(pa, pb, pc, sred);
@@ -1092,14 +1246,14 @@ __device__ void step_body(DevSolveState *S, StepShared &sh, double *dsm, double 
       bool pure = true;   // the tiles hold the pure H
       while (mu < max_mu) {
         // tiles of H + mu D^2 (lower triangle; identity on the padding), right-hand side g
-        if (!pure) refill_tiles(tiles, Hs, ntd);
-        for (int i = tid; i < n; i += T) tiles[tile_off(i >> 3, i >> 3) + swz(i & 7, i & 7)] += mu * v_diag[i] * v_diag[i];
+        if (!pure) refill_tiles<TP>(tiles, Hs, ntd);
+        for (int i = tid; i < n; i += T) TILE(i >> 3, i >> 3)[swz(i & 7, i & 7)] += mu * v_diag[i] * v_diag[i];
         pure = false;
         tiles_ready = 0;
         for (int i = tid; i < NP; i += T) v_y[i] = i < n ? v_g[i] : 0.0;
         __syncthreads();
         DS_MARK(7);
-        int ok = chol_solve_tiles(tiles, NB, v_y, &s_ok, eval_index == 1 ? S->chol_prof : nullptr);
+        int ok = chol_solve_tiles<TP>(tiles, NB, v_y, &s_ok, eval_index == 1 ? S->chol_prof : nullptr, 4 * 28 + 4);
         DS_MARK(8);
         if (ok) {
           double bad = 0;
@@ -1202,9 +1356,37 @@ k_step(DevSolveState *S, double *Hs, const double *__restrict__ Hp, double *H0, 
   if (tid >= 64 && tid < 64 + kMaxOpt) sh.pim_valid[tid - 64] = S->pim_valid[tid - 64];
   if (tid == 128) sh.zero = 0.0;
   __syncthreads();
-  step_body(S, sh, dsm, Hs, Hp, H0, g0, Sblk, F, Hpart, HpartT, Rt, eval_index);
+  step_body<OneCta>(S, sh, dsm, Hs, Hp, H0, g0, Sblk, F, Hpart, HpartT, Rt, eval_index);
   __syncthreads();
   if (tid < (int)(sizeof(DevScalars) / 8)) reinterpret_cast<long long *>(&S->sc)[tid] = reinterpret_cast<const long long *>(&sh.sc)[tid];
+}
+
+// Opt windows 14..16: the same step on a cluster of two CTAs.  Rank 0 runs k_step's body with the tiles mapped by TwoCta;
+// rank 1 only lends its shared memory.  Exits are uniform over the cluster by construction: no thread returns from this
+// kernel before the final cluster barrier.  Rank 1 does nothing between the two barriers; rank 0's early exits (sc.done at
+// entry, the verdict / gradient / iteration stops and the failed-step limit inside step_body) all return to the code below,
+// and a failed pivot only raises mu inside step_body.  The entry barrier orders rank 1's start before rank 0's first remote
+// access; the exit barrier keeps rank 1's shared memory alive until rank 0's last one (its stores are complete: arrive has
+// release semantics, wait acquire).
+__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kDsThreads, 1)
+k_step_x2(DevSolveState *S, double *Hs, const double *__restrict__ Hp, double *H0, double *g0, const double *__restrict__ Sblk,
+          FPtrs F, const double *__restrict__ Hpart, const double *__restrict__ HpartT, double *Rt, int eval_index) {
+  extern __shared__ __align__(16) double dsm[];
+  __shared__ StepShared sh;
+  cg::cluster_group cluster = cg::this_cluster();
+  cluster.sync();
+  // uniform over rank 0: nothing writes S->sc before every thread of rank 0 has passed the barrier behind this read
+  if (cluster.block_rank() == 0 && !S->sc.done) {
+    const int tid = threadIdx.x;
+    if (tid < (int)(sizeof(DevScalars) / 8)) reinterpret_cast<long long *>(&sh.sc)[tid] = reinterpret_cast<const long long *>(&S->sc)[tid];
+    if (tid >= 64 && tid < 64 + kMaxOpt) sh.pim_valid[tid - 64] = S->pim_valid[tid - 64];
+    if (tid == 128) sh.zero = 0.0;
+    __syncthreads();
+    step_body<TwoCta>(S, sh, dsm, Hs, Hp, H0, g0, Sblk, F, Hpart, HpartT, Rt, eval_index);
+    __syncthreads();
+    if (tid < (int)(sizeof(DevScalars) / 8)) reinterpret_cast<long long *>(&S->sc)[tid] = reinterpret_cast<const long long *>(&sh.sc)[tid];
+  }
+  cluster.sync();
 }
 
 // =====================================================================================================
@@ -1213,12 +1395,33 @@ static size_t step_smem_bytes(int O) {
   return sizeof(double) * ((size_t)(NB * (NB + 1) / 2) * 64 + 9 * (size_t)NB * 8);
 }
 
-bool DevSolver::supports(int O_) const { return O_ >= 1 && O_ <= kDsMaxOpt && step_smem_bytes(O_) <= 225 * 1024; }
+// k_step_x2: each CTA of the pair gets rank 0's share (fixed TwoCta layout: local tiles + the nine vectors at NB = 33)
+static size_t step_x2_smem_bytes() {
+  return sizeof(double) * ((size_t)TwoCta::kLocalTiles * 64 + 9 * (size_t)TwoCta::kMaxNB * 8);
+}
+static_assert(TwoCta::kPeerTiles * 64 <= TwoCta::kLocalTiles * 64 + 9 * TwoCta::kMaxNB * 8, "rank 1's tiles fit the same allocation");
+
+// The cluster kernel's shared-memory size is set and one two-CTA cluster must be able to be resident on the current device.
+static bool cluster_step_resident() {
+  const size_t smem = step_x2_smem_bytes();
+  if (cudaFuncSetAttribute(k_step_x2, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) { cudaGetLastError(); return false; }
+  cudaLaunchConfig_t lc = {};
+  lc.gridDim = dim3(2); lc.blockDim = dim3(kDsThreads); lc.dynamicSmemBytes = smem;
+  int nc = 0;
+  if (cudaOccupancyMaxActiveClusters(&nc, k_step_x2, &lc) != cudaSuccess) { cudaGetLastError(); return false; }
+  return nc >= 1;
+}
+
+// O <= 13: one CTA; O = 14..16: the two-CTA cluster, when the device can hold one (decided once, at estimator creation)
+bool DevSolver::supports(int O_) const {
+  if (O_ >= 1 && O_ <= kDsMaxOpt1) return step_smem_bytes(O_) <= 225 * 1024;
+  return O_ > kDsMaxOpt1 && O_ <= kDsMaxOpt && cluster_step_resident();
+}
 
 int DevSolver::init(int O_) {
   O = O_;
   const int n = 15 * (O + 1) + 6, np = 15 * O + 6;
-  smem_bytes = step_smem_bytes(O);
+  smem_bytes = O <= kDsMaxOpt1 ? step_smem_bytes(O) : step_x2_smem_bytes();
   if (cudaMalloc(&st, sizeof(DevSolveState)) != cudaSuccess) return -1;
   if (cudaMalloc(&Hs, sizeof(double) * n * n) != cudaSuccess) return -1;
   if (cudaMalloc(&H0, sizeof(double) * n * n) != cudaSuccess) return -1;
@@ -1235,7 +1438,11 @@ int DevSolver::init(int O_) {
   if (cudaMallocHost((void **)&h_st, sizeof(DevSolveState)) != cudaSuccess) return -1;
   if (cudaMemset(st, 0, sizeof(DevSolveState)) != cudaSuccess) return -1;
   if (cudaMemset(F, 0, sizeof(double) * f_doubles()) != cudaSuccess) return -1;
-  if (cudaFuncSetAttribute(k_step, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes) != cudaSuccess) return -1;
+  if (O <= kDsMaxOpt1) {
+    if (cudaFuncSetAttribute(k_step, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes) != cudaSuccess) return -1;
+  } else if (cudaFuncSetAttribute(k_step_x2, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes) != cudaSuccess) {
+    return -1;
+  }
   if (cudaStreamCreateWithFlags(&aux, cudaStreamNonBlocking) != cudaSuccess) return -1;
   if (cudaEventCreateWithFlags(&ev_fork, cudaEventDisableTiming) != cudaSuccess) return -1;
   if (cudaEventCreateWithFlags(&ev_join, cudaEventDisableTiming) != cudaSuccess) return -1;
@@ -1275,7 +1482,10 @@ int dev_solver_factors(DevSolver &ds, int eval_index, cudaStream_t st, int *laun
 int dev_solver_step(DevSolver &ds, const double *S_dev, double *Rt_dev, int eval_index, cudaStream_t st, int *launches) {
   cudaError_t e = cudaStreamWaitEvent(st, ds.ev_join, 0);
   if (e == cudaSuccess) {
-    k_step<<<1, kDsThreads, ds.smem_bytes, st>>>(ds.st, ds.Hs, ds.Hp, ds.H0, ds.g0, S_dev, fptrs(ds), ds.Hpart, ds.HpartT, Rt_dev, eval_index);
+    if (ds.O <= kDsMaxOpt1)
+      k_step<<<1, kDsThreads, ds.smem_bytes, st>>>(ds.st, ds.Hs, ds.Hp, ds.H0, ds.g0, S_dev, fptrs(ds), ds.Hpart, ds.HpartT, Rt_dev, eval_index);
+    else   // one cluster of two CTAs (__cluster_dims__)
+      k_step_x2<<<2, kDsThreads, ds.smem_bytes, st>>>(ds.st, ds.Hs, ds.Hp, ds.H0, ds.g0, S_dev, fptrs(ds), ds.Hpart, ds.HpartT, Rt_dev, eval_index);
     e = cudaGetLastError();
   }
   if (launches) *launches += 1;
@@ -1287,14 +1497,12 @@ int dev_solver_step(DevSolver &ds, const double *S_dev, double *Rt_dev, int eval
 
 // ---- test seam: the tiled shared-memory Cholesky alone, on an explicit host system ------------------------------------
 namespace lio {
-__global__ void __launch_bounds__(kDsThreads, 1)
-k_chol_test(const double *__restrict__ A, const double *__restrict__ b, int n, double *__restrict__ x, int *__restrict__ ok_out,
-            long long *__restrict__ prof) {
-  extern __shared__ __align__(16) double dsm[];
-  __shared__ int s_ok;
+template <class TP>
+__device__ void chol_test_body(double *dsm, int &s_ok, const double *__restrict__ A, const double *__restrict__ b, int n,
+                               double *__restrict__ x, int *__restrict__ ok_out, long long *__restrict__ prof) {
   const int tid = threadIdx.x, T = blockDim.x;
   const int NB = (n + 7) / 8, NP = NB * 8;
-  double *tiles = dsm, *y = dsm + (size_t)(NB * (NB + 1) / 2) * 64;
+  double *tiles = dsm, *y = dsm + TP::local_doubles(NB);
   for (int p = tid; p < (NB * (NB + 1) / 2) * 64; p += T) {
     const int t = p >> 6, e = p & 63, r = e >> 3, cs = e & 7, c = cs ^ ((r & 2) << 1);
     int ib = (int)((sqrt(8.0 * t + 1.0) - 1.0) * 0.5);
@@ -1302,24 +1510,48 @@ k_chol_test(const double *__restrict__ A, const double *__restrict__ b, int n, d
     while (ib * (ib + 1) / 2 > t) --ib;
     const int jb = t - ib * (ib + 1) / 2;
     const int a = 8 * ib + r, bb = 8 * jb + c;
-    tiles[p] = (a < n && bb < n) ? A[(size_t)a * n + bb] : (a == bb ? 1.0 : 0.0);
+    const double v = (a < n && bb < n) ? A[(size_t)a * n + bb] : (a == bb ? 1.0 : 0.0);
+    if constexpr (TP::kCluster) TILE(ib, jb)[e] = v; else tiles[p] = v;
   }
   for (int i = tid; i < NP; i += T) y[i] = i < n ? b[i] : 0.0;
   __syncthreads();
-  const int ok = chol_solve_tiles(tiles, NB, y, &s_ok, prof);
+  const int ok = chol_solve_tiles<TP>(tiles, NB, y, &s_ok, prof, 4 * NB + 5);
   for (int i = tid; i < n; i += T) x[i] = y[i];
   if (tid == 0) *ok_out = ok;
 }
+
+__global__ void __launch_bounds__(kDsThreads, 1)
+k_chol_test(const double *__restrict__ A, const double *__restrict__ b, int n, double *__restrict__ x, int *__restrict__ ok_out,
+            long long *__restrict__ prof) {
+  extern __shared__ __align__(16) double dsm[];
+  __shared__ int s_ok;
+  chol_test_body<OneCta>(dsm, s_ok, A, b, n, x, ok_out, prof);
+}
+
+// n = 217..261 on a cluster of two CTAs, as k_step_x2: rank 1 lends its shared memory between the two cluster barriers, and
+// no thread leaves before the second (a failed pivot ends chol_solve_tiles on all of rank 0 together).
+__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kDsThreads, 1)
+k_chol_test_x2(const double *__restrict__ A, const double *__restrict__ b, int n, double *__restrict__ x, int *__restrict__ ok_out,
+               long long *__restrict__ prof) {
+  extern __shared__ __align__(16) double dsm[];
+  __shared__ int s_ok;
+  cg::cluster_group cluster = cg::this_cluster();
+  cluster.sync();
+  if (cluster.block_rank() == 0) chol_test_body<TwoCta>(dsm, s_ok, A, b, n, x, ok_out, prof);
+  cluster.sync();
+}
 }  // namespace lio
 
-// Solves A x = b (A symmetric positive definite, n x n row-major, n <= 216) with the device solver's tiled Cholesky.
+// Solves A x = b (A symmetric positive definite, n x n row-major, n <= 261) with the device solver's tiled Cholesky: one CTA
+// for n <= 216 (k_step's), the two-CTA cluster above (k_step_x2's).
 extern "C" int lio_dev_cholesky_solve_host(const double *A, const double *b, int n, double *x, int *ok, long long *prof, int device) {
   using namespace lio;
   if (!A || !b || !x || !ok || n < 1 || n > 15 * (kDsMaxOpt + 1) + 6) return LIO_ERR_INVALID;
   if (lio_device_count() <= 0) return LIO_ERR_NO_DEVICE;
   LIO_CUDA_OK(cudaSetDevice(device));
   const int NB = (n + 7) / 8;
-  const size_t smem = sizeof(double) * ((size_t)(NB * (NB + 1) / 2) * 64 + (size_t)NB * 8);
+  const bool one = n <= 15 * (kDsMaxOpt1 + 1) + 6;
+  const size_t smem = sizeof(double) * ((one ? (size_t)(NB * (NB + 1) / 2) * 64 : (size_t)TwoCta::kLocalTiles * 64) + (size_t)NB * 8);
   DevBufs d;
   double *dA = nullptr, *db = nullptr, *dx = nullptr;
   int *dok = nullptr;
@@ -1327,10 +1559,12 @@ extern "C" int lio_dev_cholesky_solve_host(const double *A, const double *b, int
   const size_t nprof = 4 * (size_t)NB + 1, nprof_dev = nprof + 4;   // + 4 in-kernel phase stamps (not returned)
   if (!d.alloc(&dA, (size_t)n * n) || !d.alloc(&db, n) || !d.alloc(&dx, n) || !d.alloc(&dok, 1) || !d.alloc(&dprof, nprof_dev) ||
       !d.up(dA, A, (size_t)n * n) || !d.up(db, b, n) ||
-      !d.ok(cudaFuncSetAttribute(k_chol_test, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) ||
+      !d.ok(cudaFuncSetAttribute(one ? k_chol_test : k_chol_test_x2, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) ||
       !d.ok(cudaMemset(dprof, 0, sizeof(long long) * nprof_dev)))
     return LIO_ERR_CUDA;
-  k_chol_test<<<1, kDsThreads, smem>>>(dA, db, n, dx, dok, prof ? dprof : nullptr);
+  if (one) k_chol_test<<<1, kDsThreads, smem>>>(dA, db, n, dx, dok, prof ? dprof : nullptr);
+  else k_chol_test_x2<<<2, kDsThreads, smem>>>(dA, db, n, dx, dok, prof ? dprof : nullptr);
+  if (!d.ok(cudaGetLastError())) return LIO_ERR_CUDA;
   if (!d.down(x, dx, n) || (prof && !d.down(prof, dprof, nprof))) return LIO_ERR_CUDA;
   if (prof) {   // the four %globaltimer stamps become durations (ns) appended behind the per-panel cycles when the caller left room
     long long st[4];

@@ -9,7 +9,8 @@ constexpr int kDsMaxN = 15 * (kMaxOpt + 1) + 6;  // 261
 constexpr int kDsMaxNp = 15 * kMaxOpt + 6;       // 246
 constexpr int kFPriorCtas = 13;                  // CTAs of k_factors that share the prior's matrix-vector product
 constexpr int kDsXDim = 16 * (kMaxOpt + 1) + 7;
-constexpr int kDsMaxOpt = 13;                    // largest opt window whose Cholesky tiles fit one SM's shared memory
+constexpr int kDsMaxOpt1 = 13;                   // largest opt window whose Cholesky tiles fit one SM's shared memory (k_step)
+constexpr int kDsMaxOpt = kMaxOpt;               // larger windows (14..16) spread the tiles over a two-CTA cluster (k_step_x2)
 
 // Scalar part of the solver state.  k_step keeps a copy in shared memory for the duration of a launch (thread 0 runs the
 // trust-region bookkeeping on it without global round trips) and writes it back on exit.
@@ -43,7 +44,8 @@ struct DevSolveState {
   // device-side timeline (layout documented at lio_est_solver_trace in lio_b200.h): rows 0..11 k_step phases + gap kernels per
   // evaluation, rows 12..14 asm_ppp stamps, row 16 lidar block expansion
   long long dbg[24][16];
-  long long chol_prof[4 * 28 + 4];   // per-panel cycles of the Cholesky of evaluation 1 (see lio_dev_cholesky_solve_host)
+  long long chol_prof[4 * 28 + 4];   // per-panel cycles of the Cholesky of evaluation 1 (see lio_dev_cholesky_solve_host); opt
+                                     // windows 14..16 (29..33 tile columns) record panels 0..28 only and no tail stamps
 };
 
 // Scratch written by k_factors (state-dependent, lidar-independent terms at the state being evaluated) and read by
