@@ -722,6 +722,54 @@ int lio_xyzi_to_pcl32(const float *xyzi, int n, uint8_t *out32);
 int lio_pcl32_to_xyzi(const uint8_t *in32, int n, float *xyzi);
 
 /* ------------------------------------------------------------------------------------------
+ * The map of a whole drive (src/save_bag_to_pcd.cc): the registered clouds accumulated in HBM, written as one PCD.
+ * ---------------------------------------------------------------------------------------- */
+/* save_bag_to_pcd.cc appends every /cloud_registered message to one cloud (`map_points += transformed_cloud`, :111-115; its
+ * transform is the identity, :95-109) and writes it with pcl::PCDWriter::writeBinary (:156-160).  An lio_rm handle does the same
+ * in HBM, one insert per publishing step:
+ *   leaf == 0   raw mode, the tool's behaviour: the concatenation of every inserted point in insert order, non-finite points kept;
+ *               capacity counts points.
+ *   leaf > 0    voxel mode; capacity counts voxels.  A point's voxel is (int64) floorf(c * (1.0f / leaf)) per axis in float32
+ *               (PCL's VoxelGrid arithmetic without its 32-bit voxel index).  Points with a non-finite x, y or z, or a voxel
+ *               coordinate outside [-2^20, 2^20), are dropped.  Each voxel keeps fp64 sums of x, y, z, intensity and a count, and
+ *               every point is added to them one at a time in arrival order (insert order, then index in the cloud): the sums
+ *               equal np.add.at on float64 arrays.  A voxel's id is given when its first point arrives.
+ * The handle owns HBM for the map (raw: 16 B per point; voxel: about 80 B per voxel) and grows its per-insert scratch with
+ * stream-ordered allocations.  All work runs on cuda_stream (0 = the legacy default stream).
+ * Bad arguments return LIO_ERR_INVALID (voxel mode takes capacity <= 2^30), no device LIO_ERR_NO_DEVICE. */
+typedef struct lio_rm lio_rm;
+int lio_rm_create(float leaf, long long capacity, int device, void *cuda_stream, lio_rm **out);
+int lio_rm_destroy(lio_rm *rm);
+/* Insert one cloud of n float4 {x, y, z, intensity} (save_bag_to_pcd.cc:111-115).  _dev takes a device array and the host count,
+ * e.g. what lio_mb_full_dev returns on a publishing lio_pm, a map-builder handle or the map attached to an estimator.  It is
+ * stream-ordered on the handle's stream and never waits on the host: the cloud is written by stream-ordered work on the mapping's
+ * stream, so create the handle on that stream or order the two streams with an event.  Work enqueued on the handle's stream after
+ * the call may reuse the caller's buffer.  _host copies a host array before it returns.
+ * An insert that would exceed the capacity changes nothing and sets a sticky overflow flag; every later insert is then a no-op
+ * until lio_rm_reset.  A voxel-mode insert is 17 stream operations whatever n is (one more for the upload of _host), a raw-mode
+ * insert one copy. */
+int lio_rm_insert_dev(lio_rm *rm, const float *xyzi_dev, int n);
+int lio_rm_insert_host(lio_rm *rm, const float *xyzi, int n);
+/* out8 = {insert calls, points offered by them, map size (points or voxels), overflow flag, points accepted, points dropped (voxel
+ * mode: non-finite or out of range), host waits of the handle so far (this call's included), stream operations of the last insert}.
+ * Synchronises the handle's stream. */
+int lio_rm_stats(lio_rm *rm, long long out8[8]);
+/* The map as float4, raw points in insert order or voxels in id order as float(sum / count) per channel.  _dev synchronises for
+ * the size, then gathers into a stable export buffer on the stream; the pointer is valid until the next insert or reset.
+ * _download copies it to out (cap float4 records; LIO_ERR_CAPACITY with *n set when the map is larger). */
+int lio_rm_export_dev(lio_rm *rm, const float **ptr, long long *n);
+int lio_rm_download(lio_rm *rm, float *out_xyzi, long long cap, long long *n);
+/* Empties the map and clears the overflow flag (stream-ordered); the counters of lio_rm_stats keep counting. */
+int lio_rm_reset(lio_rm *rm);
+/* A binary PCD v0.7 file in the layout pcl::PCDWriter::writeBinary gives pcl::PointXYZI (save_bag_to_pcd.cc:156-160), restated
+ * from PCL's published format: the header lines "# .PCD v0.7 - Point Cloud Data file format", "VERSION 0.7",
+ * "FIELDS x y z intensity", "SIZE 4 4 4 4", "TYPE F F F F", "COUNT 1 1 1 1", "WIDTH n", "HEIGHT 1", "VIEWPOINT 0 0 0 1 0 0 0",
+ * "POINTS n", "DATA binary", each ended by '\n', then n records of 16 bytes (x, y, z, intensity; no padding fields).
+ * lio_pcd_write_xyzi is host only and needs no device; a path that cannot be written returns LIO_ERR_INVALID. */
+int lio_pcd_write_xyzi(const char *path, const float *xyzi_host, long long n);
+int lio_rm_write_pcd(lio_rm *rm, const char *path);
+
+/* ------------------------------------------------------------------------------------------
  * Dense fp64 kernels of the host shell (host only; test seams).
  * ---------------------------------------------------------------------------------------- */
 /* Lower Cholesky A = L L^T (blocked, the factorisation behind every dogleg step: Ceres DENSE_SCHUR at n <= 261,

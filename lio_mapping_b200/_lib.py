@@ -211,6 +211,17 @@ def lib():
     L.lio_pm_update_map_database_host.argtypes = [vp, f32p, ip, f32p, ip, np.ctypeslib.ndpointer(np.int64, flags="C_CONTIGUOUS"), ip,
                                                   f32p, i32p]
     L.lio_pm_update_stats.argtypes = [vp, i32p]
+    ll, i64p = C.c_longlong, np.ctypeslib.ndpointer(np.int64, flags="C_CONTIGUOUS")
+    L.lio_rm_create.argtypes = [C.c_float, ll, ip, vp, C.POINTER(vp)]
+    L.lio_rm_destroy.argtypes = [vp]
+    L.lio_rm_insert_dev.argtypes = [vp, vp, ip]
+    L.lio_rm_insert_host.argtypes = [vp, f32p, ip]
+    L.lio_rm_stats.argtypes = [vp, i64p]
+    L.lio_rm_export_dev.argtypes = [vp, C.POINTER(vp), C.POINTER(ll)]
+    L.lio_rm_download.argtypes = [vp, f32p, ll, C.POINTER(ll)]
+    L.lio_rm_reset.argtypes = [vp]
+    L.lio_pcd_write_xyzi.argtypes = [C.c_char_p, f32p, ll]
+    L.lio_rm_write_pcd.argtypes = [vp, C.c_char_p]
     _LIB = L
     return L
 
