@@ -411,6 +411,16 @@ int lio_pim_get(lio_pim *p, double *state11, double *jac225, double *cov225);
 /* ImuFactor::Evaluate (include/factor/ImuFactor.h:53-167): J blocks 15x7, 15x9, 15x7, 15x9 row-major or NULL */
 int lio_imu_factor_evaluate(lio_pim *p, const double pose_i[7], const double sb_i[9], const double pose_j[7],
                             const double sb_j[9], double *res15, double *J0, double *J1, double *J2, double *J3);
+/* Estimator::RunInitialization (src/imu_processor/Estimator.cc:858-958) with ImuInitializer::Initialization (ImuInitializer.cc:35-308,
+ * :421-452) on host arrays: the arithmetic the imu_factor = 1 estimator runs on its full window (lio_est_attach_imu_mapping).
+ * W >= 5 (ApproximateGravity needs it; LIO_ERR_INVALID otherwise); laser_tf7 (W+1) x 7 float transforms (x y z w, px py pz), pims W + 1
+ * handles (frame i's pre-integration ends at frame i; the excitation check reads 1..W), tlb7 transform_lb_; bas / bgs / vs (W+1) x 3,
+ * R_WI9 row-major.  outcome: 0 excitation below 0.25 (nothing changes), 1 gravity norm check failed, 2 success.  With 1 and 2 the
+ * reference's side effects all happen: bgs += delta_bg, pims 1..W repropagated with (0, bgs[0]) and then pims 0..W with (bas[i], bgs[i]),
+ * ps / rs (row-major 3x3 each) from the laser transforms, R0 = ypr2R(-yaw, 0, 0) R_WI^T applied to ps, rs, vs, R_WI9 = R0^T and
+ * g3 = R0 g_in_laser; vs is the refined velocities only on success.  A non-finite result returns LIO_ERR_NUMERIC. */
+int lio_imu_run_initialization_host(int W, const float *laser_tf7, lio_pim *const *pims, const float tlb7[7], double g_norm, const double *bas,
+                                    double *bgs, double *vs, double R_WI9[9], double *ps, double *rs, double g3[3], int *outcome);
 
 /* ------------------------------------------------------------------------------------------
  * Stages B+C+D — lio::Estimator in steady state (stage_flag_ == INITED)
@@ -634,6 +644,35 @@ int lio_est_process_compact_dev(lio_est *est, const float *corner_dev, const flo
 int lio_est_process_compact_host(lio_est *est, const float *corner, int nc, const float *surf, int ns, const float *full, int nf,
                                  const float transform_sum7[7]);
 int lio_est_compact_status(lio_est *est, int info4[4]);
+/* ---- imu_factor = 1 from the odometry's clouds and the IMU: the estimator starts itself with ImuInitializer (ProcessLaserOdom NOT_INITED
+ * :505-602, RunInitialization :858-958) and then runs the lio_est_attach_map path.
+ *   lio_est_attach_imu_mapping   as lio_est_attach_mapping, with imu_factor = 1 and W >= 5; estimate_extrinsic = 2 is refused.  Refusals
+ *                                return LIO_ERR_INVALID and change nothing.
+ *   lio_est_process_compact_stamped_dev / _host
+ *                                the compact entries with the message's header.stamp, which the 0.1 s gate between attempts (:533-536)
+ *                                compares; feed the IMU samples up to that stamp before the call.  On an imu_factor = 0 mapping they
+ *                                equal the unstamped entries; on an IMU mapping the unstamped entries return LIO_ERR_INVALID.
+ *                                NOT_INITED: as under lio_est_attach_mapping.  The push that fills the window, and every later push
+ *                                until one succeeds, runs RunInitialization when stamp - (stamp of the last attempt) > 0.1 (the first
+ *                                always).  Success: the rotated states, Vs, Bgs and g_vec_ are taken, pm switches to its IMU-inited mode,
+ *                                the first solve runs (no insert or publication), then SlideWindow.  Otherwise SlideWindow's state copy and
+ *                                the attempt's side effects stay (see lio_imu_run_initialization_host); a non-finite result returns
+ *                                LIO_ERR_NUMERIC and poisons the context.
+ *                                INITED: no Process; tobe is predicted as lio_est_attach_map predicts it, the INITED push rules take the
+ *                                message's clouds (without a de-skew flag PointMapping's last stacks, which no longer change), from the
+ *                                (O+1)-th INITED message on the oldest optimised frame is inserted with the frozen valid list, then
+ *                                PublishResults.  With a de-skew flag the caller turns its odometry into a pass-through once
+ *                                lio_est_imu_init_status reports inited (lio_po_set_enable_odom(po, 0); the reference's /enable_odom).
+ *   lio_est_imu_init_status      info4 = {attempts, outcome of the last (-1 none, 0 excitation, 1 gravity check, 2 success), whether the
+ *                                last message ran an attempt, inited}; g3 = g_vec_, R_WI9 = R_WI_ row-major; states16 (W+1) x 16 in the
+ *                                lio_est_get_states layout as the last attempt left them (on success: before the first solve; untouched
+ *                                before the first attempt).  g3, R_WI9 and states16 may be NULL. */
+int lio_est_attach_imu_mapping(lio_est *est, lio_pm *pm);
+int lio_est_process_compact_stamped_dev(lio_est *est, const float *corner_dev, const float *surf_dev, const float *full_dev, const int *n3_dev,
+                                        const int n3_max[3], const float transform_sum7[7], double stamp);
+int lio_est_process_compact_stamped_host(lio_est *est, const float *corner, int nc, const float *surf, int ns, const float *full, int nf,
+                                         const float transform_sum7[7], double stamp);
+int lio_est_imu_init_status(lio_est *est, int info4[4], double g3[3], double R_WI9[9], double *states16);
 /* window states: (W+1) x 16 doubles (layout of state16) */
 int lio_est_get_states(lio_est *est, double *out);
 /* summary[32]: see lio_mapping_b200/estimator.py SUMMARY_KEYS */

@@ -203,6 +203,12 @@ def lib():
     L.lio_est_process_compact_dev.argtypes = [vp, vp, vp, vp, vp, i32p, f32p]
     L.lio_est_process_compact_host.argtypes = [vp, f32p, ip, f32p, ip, f32p, ip, f32p]
     L.lio_est_compact_status.argtypes = [vp, i32p]
+    L.lio_est_attach_imu_mapping.argtypes = [vp, vp]
+    L.lio_est_process_compact_stamped_dev.argtypes = [vp, vp, vp, vp, vp, i32p, f32p, C.c_double]
+    L.lio_est_process_compact_stamped_host.argtypes = [vp, f32p, ip, f32p, ip, f32p, ip, f32p, C.c_double]
+    L.lio_est_imu_init_status.argtypes = [vp, i32p, f64p, f64p, f64p]
+    L.lio_imu_run_initialization_host.argtypes = [ip, f32p, C.POINTER(vp), f32p, C.c_double, f64p, f64p, f64p, f64p, f64p, f64p, f64p,
+                                                  C.POINTER(ip)]
     L.lio_mb_process_map_dev.argtypes = [vp, vp, vp, vp, vp, i32p, f32p, f32p, f32p, i32p]
     L.lio_po_process_dev.argtypes = [vp, C.POINTER(vp), C.POINTER(vp), i32p, f32p, f32p, i32p]
     L.lio_po_clouds_dev.argtypes = [vp, C.POINTER(vp), C.POINTER(vp), i32p]

@@ -206,9 +206,9 @@ static lio::TwistF lb_twist(const lio_est *e) {
 
 // Scan entry: join the previous scan's map work (it reads frame slots the push below may reuse, and the staged full cloud), predict
 // transform_tobe_mapped_ (ProcessCompactData :776-809, imu_factor: tobe * lb * (prev^-1 * curr) * lb^-1 in float Twist, prev / curr
-// the float casts of the states W - 1 and W) and, when W == O with de-skew, keep the clouds of the frame that leaves the window:
-// they are the ones this scan inserts (see map_step).
-int map_scan_entry(lio_est *e) {
+// the float casts of the states W - 1 and W; only on INITED messages: predict is false for the start-up's) and, when W == O with
+// de-skew, keep the clouds of the frame that leaves the window: they are the ones this scan inserts (see map_step).
+int map_scan_entry(lio_est *e, bool predict) {
   const int W = e->W, O = e->O;
   cudaStream_t st = e->stream;
   if (e->map.pending) { LIO_CUDA_OK(cudaStreamWaitEvent(st, e->map.ev_done, 0)); e->map.pending = false; }
@@ -216,7 +216,7 @@ int map_scan_entry(lio_est *e) {
     const Q q = fromR(R);
     return lio::TwistF{(float)q.x, (float)q.y, (float)q.z, (float)q.w, (float)P.x, (float)P.y, (float)P.z};
   };
-  if (e->cfg.imu_factor) {   // imu_factor = 0: TransformAssociateToMap, run by the mapping's Process (:804)
+  if (e->cfg.imu_factor && predict) {   // imu_factor = 0: TransformAssociateToMap, run by the mapping's Process (:804)
     const lio::TwistF d = lio::twist_mul(lio::twist_inverse(twist_of(e->Rs[W - 1], e->Ps[W - 1])), twist_of(e->Rs[W], e->Ps[W]));
     const lio::TwistF lb = lb_twist(e);
     lio::TwistF *tobe = pm_tobe(e->map.pm);
@@ -266,9 +266,11 @@ int map_step(lio_est *e) {
   LIO_CUDA_OK(cudaEventRecord(e->map.ev_in, e->stream));
   LIO_CUDA_OK(cudaStreamWaitEvent(ms, e->map.ev_in, 0));
   e->map.pending = true;
-  // imu_factor = 0: the frame's own valid list and the cube centre it was computed with (opt_valid_idx_ / opt_cube_centers_.first())
-  const std::vector<size_t> *valid = e->mapping.on ? &e->mapping.opt_valid[pivot] : nullptr;
-  const int *centre = e->mapping.on ? e->mapping.opt_centre[pivot].data() : nullptr;
+  // imu_factor = 0: the frame's own valid list and the cube centre it was computed with (opt_valid_idx_ / opt_cube_centers_.first());
+  // imu_factor = 1: the lists of the last Process, frozen since
+  const bool own = e->mapping.on && !e->cfg.imu_factor;
+  const std::vector<size_t> *valid = own ? &e->mapping.opt_valid[pivot] : nullptr;
+  const int *centre = own ? e->mapping.opt_centre[pivot].data() : nullptr;
   const int rc = pm_est_step(e->map.pm, insert, src, n_dev, bound, e->map.insert, valid, centre, e->lc.d_stage[1], e->lc.d_stage_n + 1, e->h_counts[W + 13],
                              e->map.info);
   if (rc != LIO_OK) return rc;
@@ -349,14 +351,17 @@ void predict_state_w(lio_est *e) {
   e->Rs[W] = e->Rs[W - 1] * toR(Q((double)inc.qw, (double)inc.qx, (double)inc.qy, (double)inc.qz));
 }
 
-extern "C" int lio_est_attach_mapping(lio_est *e, lio_pm *pm) {
+static int attach_mapping(lio_est *e, lio_pm *pm, bool imu) {
   if (!e || !pm) return LIO_ERR_INVALID;
   const char *why = nullptr;
-  if (e->map.pm) why = "lio_est_attach_mapping: a map is attached already";
-  else if (e->frames_started || e->tmp_pre) why = "lio_est_attach_mapping: call it before lio_est_init_frame / lio_est_finish_init and the first scan";
-  else if (!e->lc.on) why = "lio_est_attach_mapping: local clouds are off (lio_est_enable_local_clouds)";
-  else if (e->cfg.imu_factor) why = "lio_est_attach_mapping: needs imu_factor = 0";
-  else if (e->world > 1 || e->px.npeers || e->px.fpeers) why = "lio_est_attach_mapping: not supported on a sharded context";
+  if (e->map.pm) why = "a map is attached already";
+  else if (e->frames_started || e->tmp_pre) why = "call it before lio_est_init_frame / lio_est_finish_init and the first scan";
+  else if (!e->lc.on) why = "local clouds are off (lio_est_enable_local_clouds)";
+  else if (!imu && e->cfg.imu_factor) why = "lio_est_attach_mapping needs imu_factor = 0 (lio_est_attach_imu_mapping takes imu_factor = 1)";
+  else if (imu && !e->cfg.imu_factor) why = "lio_est_attach_imu_mapping needs imu_factor = 1";
+  else if (imu && e->W < 5) why = "lio_est_attach_imu_mapping: ImuInitializer needs window_size >= 5 (ApproximateGravity)";
+  else if (imu && e->extrinsic_stage == 2) why = "lio_est_attach_imu_mapping: estimate_extrinsic = 2 (EstimateExtrinsicRotation) is not supported";
+  else if (e->world > 1 || e->px.npeers || e->px.fpeers) why = "not supported on a sharded context";
   if (why) { lio_set_last_error(__FILE__, __LINE__, why); return LIO_ERR_INVALID; }
   const int rc = attach_common(e, pm, true);
   if (rc != LIO_OK) return rc;
@@ -370,21 +375,50 @@ extern "C" int lio_est_attach_mapping(lio_est *e, lio_pm *pm) {
   return LIO_OK;
 }
 
-// ProcessCompactData (:776-856) with update_laser_imu: PointMapping::Process on the mapping's stream, then ProcessLaserOdom.  corner /
-// surf / full and n3_dev are the message's clouds and counts, n_max their bounds (already capped by the mapping's capacities).
-static int compact_body(lio_est *e, const float4 *const src[3], const int *n3_dev, const int n_max[3], const float sum7[7]) {
+extern "C" int lio_est_attach_mapping(lio_est *e, lio_pm *pm) { return attach_mapping(e, pm, false); }
+extern "C" int lio_est_attach_imu_mapping(lio_est *e, lio_pm *pm) { return attach_mapping(e, pm, true); }
+
+// RunInitialization (:858-958) on the window the push has just filled: all_laser_transforms_ 0..W and their pre-integrations, which are
+// pre_[1..W] and tmp_pre (the push moves them one place later; the objects, which the attempt repropagates, are the same)
+static int imu_attempt(lio_est *e, double stamp) {
+  const int W = e->W;
+  std::vector<Preintegration *> pre(W + 1);
+  for (int i = 0; i < W; ++i) pre[i] = e->pre[i + 1].get();
+  pre[W] = e->tmp_pre.get();
+  const int rc = run_initialization(W, e->mapping.laser_tf.data(), pre.data(), lb_twist(e), e->noise.g_norm, e->Bas.data(), e->Bgs.data(),
+                                    e->Vs.data(), e->mapping.R_WI, e->Ps.data(), e->Rs.data(), e->g_vec);
+  ++e->mapping.attempts;
+  e->mapping.attempted = true;
+  e->mapping.attempt_states.resize(16 * (W + 1));
+  lio_est_get_states(e, e->mapping.attempt_states.data());
+  e->mapping.initial_time = stamp;   // :536
+  if (rc == kInitNotFinite) {
+    lio_set_last_error(__FILE__, __LINE__, "RunInitialization: non-finite result (TangentBasis of a gravity exactly along +z)");
+    return LIO_ERR_NUMERIC;
+  }
+  e->mapping.outcome = rc;
+  return LIO_OK;
+}
+
+// ProcessCompactData (:776-856) with update_laser_imu: PointMapping::Process on the mapping's stream (not once imu_factor = 1 is
+// inited, :810-812), then ProcessLaserOdom.  corner / surf / full and n3_dev are the message's clouds and counts, n_max their bounds
+// (already capped by the mapping's capacities); stamp is header.stamp (imu_factor = 1 only).
+static int compact_body(lio_est *e, const float4 *const src[3], const int *n3_dev, const int n_max[3], const float sum7[7], double stamp) {
   const int W = e->W;
   cudaStream_t st = e->stream, ms = pm_stream(e->map.pm);
-  // Process overwrites the handle's stacks and full cloud, which the estimator's previous pushes read on its own stream
+  const bool process = !(e->mapping.inited && e->cfg.imu_factor);
+  // Process overwrites the handle's stacks and full cloud, which the estimator's previous pushes read on its own stream; without it
+  // the estimator's stream still waits for the host entry's upload on the mapping's stream
   LIO_CUDA_OK(cudaEventRecord(e->map.ev_in, st));
   LIO_CUDA_OK(cudaStreamWaitEvent(ms, e->map.ev_in, 0));
-  int rc = pm_est_process(e->map.pm, src, src[2], n3_dev, n_max, sum7);
+  int rc = process ? pm_est_process(e->map.pm, src, src[2], n3_dev, n_max, sum7) : LIO_OK;
   if (rc != LIO_OK) return rc;
   LIO_CUDA_OK(cudaEventRecord(e->map.ev_done, ms));
   LIO_CUDA_OK(cudaStreamWaitEvent(st, e->map.ev_done, 0));
   e->map.pending = false;
   ++e->mapping.recv_count;
   e->mapping.compact_info[0] = e->mapping.inited ? 1 : 0; e->mapping.compact_info[1] = e->mapping.cir_count; e->mapping.compact_info[2] = e->mapping.compact_info[3] = 0;
+  e->mapping.attempted = false;
   if (!e->mapping.inited && e->mapping.recv_count % e->cfg.init_window_factor != 0) return LIO_OK;   // :436-439
   // the push (:441-487): the laser transform is transform_aft_mapped_, the stacks PointMapping's down-sampled ones unless the INITED
   // de-skew rules push their own (:474-480, :628-693)
@@ -395,12 +429,13 @@ static int compact_body(lio_est *e, const float4 *const src[3], const int *n3_de
     return LIO_ERR_CAPACITY;
   }
   const int *cnt = pm_counts_dev(e->map.pm);   // {corner in, surf in, corner ds, surf ds, full}
+  const int *n_in = process ? cnt : n3_dev;     // the message's counts: Process's copies, or the caller's own
   rc = lc_stage_wait(e);
   if (rc != LIO_OK) return rc;
   {
-    const float4 *sc[2] = {pm_stacks ? pm_ds(e->map.pm, 0) : src[0], pm_full_in(e->map.pm)};
-    const int *nc[2] = {pm_stacks ? cnt + 2 : cnt, cnt + 4};
-    const int nb[2] = {e->lc.cap[0], n_max[2]};
+    const float4 *sc[2] = {pm_stacks ? pm_ds(e->map.pm, 0) : src[0], process ? pm_full_in(e->map.pm) : src[2]};
+    const int *nc[2] = {pm_stacks ? cnt + 2 : n_in, process ? cnt + 4 : n3_dev + 2};
+    const int nb[2] = {process || pm_stacks ? e->lc.cap[0] : n_max[0], n_max[2]};
     for (int w = 0; w < 2; ++w) copy_cloud(sc[w], nc[w], nb[w], e->lc.d_stage[w], e->lc.d_stage_n + w, e->sm_count * 2, st);
     LIO_CUDA_OK(cudaGetLastError());
     e->lc.staged = true;
@@ -414,9 +449,18 @@ static int compact_body(lio_est *e, const float4 *const src[3], const int *n3_de
   }
   e->mapping.compact_info[2] = 1;
   const int c = e->mapping.cir_count;
-  if (!e->mapping.inited && c < W) {   // NOT_INITED, window not full: push, SlideWindow's state copy, ++cir_buf_count_ (:603-614)
+  const V3 tmp_bg = e->Bgs[c];
+  bool startup = !e->mapping.inited && c == W;
+  if (startup && e->cfg.imu_factor) {   // :533-537
+    startup = false;
+    if (stamp - e->mapping.initial_time > 0.1) {
+      if ((rc = imu_attempt(e, stamp)) != LIO_OK) return rc;
+      startup = e->mapping.outcome == kInitSuccess;
+    }
+  }
+  if (!e->mapping.inited && !startup) {   // NOT_INITED without a start-up: push, then SlideWindow's state copy (:600-614)
     push_shift(e->pre, e->tmp_pre);
-    e->tmp_pre = std::make_shared<Preintegration>(e->acc_last, e->gyr_last, e->Bas[c], e->Bgs[c], e->noise);
+    e->tmp_pre = std::make_shared<Preintegration>(e->acc_last, e->gyr_last, e->Bas[c], tmp_bg, e->noise);
     const int freed = e->slot_of[0];
     e->slot_of.erase(e->slot_of.begin());
     e->slot_of.push_back(freed);
@@ -428,13 +472,18 @@ static int compact_body(lio_est *e, const float4 *const src[3], const int *n3_de
     LIO_CUDA_OK(cudaMemcpyAsync(e->d_own_n + slot, e->d_slot_n + slot, sizeof(int), cudaMemcpyDeviceToDevice, st));
     e->lc.staged = false;
     push_shift(e->size_surf_stack, nds[1]);
-    e->Ps[c + 1] = e->Ps[c]; e->Vs[c + 1] = e->Vs[c]; e->Rs[c + 1] = e->Rs[c]; e->Bas[c + 1] = e->Bas[c]; e->Bgs[c + 1] = e->Bgs[c];
-    e->mapping.compact_info[1] = ++e->mapping.cir_count;
+    if (c < W) {   // ++cir_buf_count_ (:613)
+      e->Ps[c + 1] = e->Ps[c]; e->Vs[c + 1] = e->Vs[c]; e->Rs[c + 1] = e->Rs[c]; e->Bas[c + 1] = e->Bas[c]; e->Bgs[c + 1] = e->Bgs[c];
+      e->mapping.compact_info[1] = ++e->mapping.cir_count;
+    } else {       // imu_factor = 1, full window, no successful attempt (:600-602): the buffers move on, state W is kept
+      push_shift(e->Ps, e->Ps[W]); push_shift(e->Vs, e->Vs[W]); push_shift(e->Rs, e->Rs[W]); push_shift(e->Bas, e->Bas[W]);
+      push_shift(e->Bgs, e->Bgs[W]);
+    }
     return LIO_OK;
   }
-  CompactPush cp{nullptr, nullptr, pm_stacks, !e->mapping.inited};
+  CompactPush cp{nullptr, nullptr, pm_stacks, !e->mapping.inited, tmp_bg};
   if (pm_stacks) { cp.surf_ds = pm_ds(e->map.pm, 1); cp.surf_ds_n = cnt + 3; }
-  if (!e->mapping.inited) {   // the start-up (:505-517): states 0..W from the W + 1 pushed laser transforms, then the first solve and slide
+  if (!e->mapping.inited && !e->cfg.imu_factor) {   // the start-up (:505-517): states 0..W from the W + 1 pushed laser transforms
     const lio::TwistF lb = lb_twist(e);
     for (int i = 0; i <= W; ++i) {
       const lio::TwistF tb = lio::twist_mul(e->mapping.laser_tf[i], lb);
@@ -443,18 +492,20 @@ static int compact_body(lio_est *e, const float4 *const src[3], const int *n3_de
       e->Ps[i] = V3((double)tb.px, (double)tb.py, (double)tb.pz);
       for (int a = 0; a < 3; ++a) for (int b = 0; b < 3; ++b) e->Rs[i](a, b) = (double)R[3 * a + b];
     }
+  }
+  if (!e->mapping.inited) {   // then (either mode) the first solve and SlideWindow
     e->mapping.inited = true;
     pm_set_imu_inited(e->map.pm);   // SetInitFlag(true) (:544)
     e->mapping.quiet = true;
   }
-  rc = process_scan_body(e, src[1], cnt + 1, std::max(1, std::min(n_max[1], e->cfg.max_scan_points)), false, &cp);
+  rc = process_scan_body(e, src[1], n_in + 1, std::max(1, std::min(n_max[1], e->cfg.max_scan_points)), false, &cp);
   e->mapping.quiet = false;
   if (rc != LIO_OK) return rc;
   e->mapping.compact_info[0] = 1; e->mapping.compact_info[3] = 1;
   return LIO_OK;
 }
 
-static int compact_common(lio_est *e, const float4 *const src[3], const int *n3_dev, const int n_max[3], const float sum7[7]) {
+static int compact_common(lio_est *e, const float4 *const src[3], const int *n3_dev, const int n_max[3], const float sum7[7], double stamp) {
   if (e->poisoned) return refuse_poisoned(e);
   // the full cloud is pushed into a local full slot, and with a de-skew flag the raw corner cloud is staged after initialisation:
   // bounds above those capacities are refused before anything changes, as lio_est_set_scan_clouds_* refuses them
@@ -464,7 +515,7 @@ static int compact_common(lio_est *e, const float4 *const src[3], const int *n3_
   }
   e->frames_started = true;
   e->scanned = true;
-  const int rc = compact_body(e, src, n3_dev, n_max, sum7);
+  const int rc = compact_body(e, src, n3_dev, n_max, sum7, stamp);
   return rc != LIO_OK ? scan_failed(e, rc) : rc;
 }
 
@@ -473,29 +524,40 @@ static int compact_check(lio_est *e) {
   return LIO_OK;
 }
 
-extern "C" int lio_est_process_compact_dev(lio_est *e, const float *corner_dev, const float *surf_dev, const float *full_dev, const int *n3_dev,
-                                           const int n3_max[3], const float transform_sum7[7]) {
+// The unstamped entries pass a NaN stamp, which an IMU mapping refuses: its attempts are gated on the stamps
+static int compact_check(lio_est *e, double stamp) {
+  const int rc = compact_check(e);
+  if (rc != LIO_OK) return rc;
+  if (e->cfg.imu_factor && std::isnan(stamp)) {
+    lio_set_last_error(__FILE__, __LINE__, "an IMU mapping takes the message stamps: lio_est_process_compact_stamped_*");
+    return LIO_ERR_INVALID;
+  }
+  return LIO_OK;
+}
+
+static int compact_dev(lio_est *e, const float *corner_dev, const float *surf_dev, const float *full_dev, const int *n3_dev, const int n3_max[3],
+                       const float transform_sum7[7], double stamp) {
   if (!e || !n3_dev || !n3_max || !transform_sum7 || n3_max[0] < 0 || n3_max[1] < 0 || n3_max[2] < 0 || (n3_max[0] > 0 && !corner_dev) ||
       (n3_max[1] > 0 && !surf_dev) || (n3_max[2] > 0 && !full_dev))
     return LIO_ERR_INVALID;
-  int rc = compact_check(e);
+  int rc = compact_check(e, stamp);
   if (rc != LIO_OK) return rc;
   LIO_CUDA_OK(cudaSetDevice(e->device));
   int n_max[3];
   pm_est_caps(e->map.pm, n3_max, n_max);
   const float4 *src[3] = {reinterpret_cast<const float4 *>(corner_dev), reinterpret_cast<const float4 *>(surf_dev), reinterpret_cast<const float4 *>(full_dev)};
-  return compact_common(e, src, n3_dev, n_max, transform_sum7);
+  return compact_common(e, src, n3_dev, n_max, transform_sum7, stamp);
 }
 
-extern "C" int lio_est_process_compact_host(lio_est *e, const float *corner, int nc, const float *surf, int ns, const float *full, int nf,
-                                            const float transform_sum7[7]) {
+static int compact_host(lio_est *e, const float *corner, int nc, const float *surf, int ns, const float *full, int nf, const float transform_sum7[7],
+                        double stamp) {
   if (!e || !transform_sum7 || nc < 0 || ns < 0 || nf < 0 || (nc > 0 && !corner) || (ns > 0 && !surf) || (nf > 0 && !full)) return LIO_ERR_INVALID;
-  int rc = compact_check(e);
+  int rc = compact_check(e, stamp);
   if (rc != LIO_OK) return rc;
   LIO_CUDA_OK(cudaSetDevice(e->device));
   if (e->poisoned || nf > e->lc.cap[1] || (map_deskew(e) && nc > e->lc.cap[0])) {
     const int n_max[3] = {nc, ns, nf};
-    return compact_common(e, nullptr, nullptr, n_max, transform_sum7);
+    return compact_common(e, nullptr, nullptr, n_max, transform_sum7, stamp);
   }
   // the handle's input buffers are rewritten: the previous message's pushes (on the estimator's stream) read them
   LIO_CUDA_OK(cudaStreamSynchronize(e->stream));
@@ -503,7 +565,26 @@ extern "C" int lio_est_process_compact_host(lio_est *e, const float *corner, int
   const int *n3_dev = nullptr;
   if ((rc = pm_est_upload(e->map.pm, corner, nc, surf, ns, full, nf, src, &n3_dev)) != LIO_OK) return rc;
   const int n_max[3] = {nc, ns, nf};
-  return compact_common(e, src, n3_dev, n_max, transform_sum7);
+  return compact_common(e, src, n3_dev, n_max, transform_sum7, stamp);
+}
+
+extern "C" int lio_est_process_compact_dev(lio_est *e, const float *corner_dev, const float *surf_dev, const float *full_dev, const int *n3_dev,
+                                           const int n3_max[3], const float transform_sum7[7]) {
+  return compact_dev(e, corner_dev, surf_dev, full_dev, n3_dev, n3_max, transform_sum7, std::nan(""));
+}
+extern "C" int lio_est_process_compact_host(lio_est *e, const float *corner, int nc, const float *surf, int ns, const float *full, int nf,
+                                            const float transform_sum7[7]) {
+  return compact_host(e, corner, nc, surf, ns, full, nf, transform_sum7, std::nan(""));
+}
+extern "C" int lio_est_process_compact_stamped_dev(lio_est *e, const float *corner_dev, const float *surf_dev, const float *full_dev,
+                                                   const int *n3_dev, const int n3_max[3], const float transform_sum7[7], double stamp) {
+  if (std::isnan(stamp)) return LIO_ERR_INVALID;
+  return compact_dev(e, corner_dev, surf_dev, full_dev, n3_dev, n3_max, transform_sum7, stamp);
+}
+extern "C" int lio_est_process_compact_stamped_host(lio_est *e, const float *corner, int nc, const float *surf, int ns, const float *full, int nf,
+                                                    const float transform_sum7[7], double stamp) {
+  if (std::isnan(stamp)) return LIO_ERR_INVALID;
+  return compact_host(e, corner, nc, surf, ns, full, nf, transform_sum7, stamp);
 }
 
 extern "C" int lio_est_compact_status(lio_est *e, int info4[4]) {
@@ -511,5 +592,17 @@ extern "C" int lio_est_compact_status(lio_est *e, int info4[4]) {
   int rc = compact_check(e);
   if (rc != LIO_OK) return rc;
   for (int k = 0; k < 4; ++k) info4[k] = e->mapping.compact_info[k];
+  return LIO_OK;
+}
+
+extern "C" int lio_est_imu_init_status(lio_est *e, int info4[4], double g3[3], double R_WI9[9], double *states16) {
+  if (!e || !info4) return LIO_ERR_INVALID;
+  int rc = compact_check(e);
+  if (rc != LIO_OK) return rc;
+  info4[0] = e->mapping.attempts; info4[1] = e->mapping.outcome; info4[2] = e->mapping.attempted ? 1 : 0; info4[3] = e->mapping.inited ? 1 : 0;
+  if (g3) for (int k = 0; k < 3; ++k) g3[k] = e->g_vec[k];
+  if (R_WI9) for (int a = 0; a < 3; ++a) for (int b = 0; b < 3; ++b) R_WI9[3 * a + b] = e->mapping.R_WI(a, b);
+  if (states16 && !e->mapping.attempt_states.empty())
+    std::memcpy(states16, e->mapping.attempt_states.data(), sizeof(double) * e->mapping.attempt_states.size());
   return LIO_OK;
 }

@@ -414,11 +414,12 @@ int process_scan_body(lio_est *e, const float4 *scan_dev, const int *n_dev, int 
   e->have_H0 = false;
   if (!e->tmp_pre) { lio_set_last_error(__FILE__, __LINE__, "process_scan before finish_init"); return LIO_ERR_INVALID; }
   if (e->map.pm) {
-    const int rc0 = map_scan_entry(e);
+    const int rc0 = map_scan_entry(e, !(cp && cp->startup));
     if (rc0 != LIO_OK) return rc0;
   }
   push_shift(e->pre, e->tmp_pre);
-  e->tmp_pre = std::make_shared<Preintegration>(e->acc_last, e->gyr_last, e->Bas[W], e->Bgs[W], e->noise);
+  e->tmp_pre = std::make_shared<Preintegration>(e->acc_last, e->gyr_last, e->Bas[W], cp ? cp->tmp_bg : e->Bgs[W], e->noise);
+  e->tmp_pre->keep_samples = false;   // from here on the window is INITED: only RunInitialization repropagates
   // frame slot rotation (CircularBuffer push): the dropped logical frame 0 becomes the new frame W
   {
     const int freed = e->slot_of[0];
@@ -476,7 +477,7 @@ int process_scan_body(lio_est *e, const float4 *scan_dev, const int *n_dev, int 
   LIO_CUDA_OK(cudaMemcpyAsync(e->d_own_n + slot, e->d_slot_n + slot, sizeof(int), cudaMemcpyDeviceToDevice, st));
   if (e->lc.on && (rc = lc_push(e, deskew_surf, cp && cp->corner_filtered)) != LIO_OK) return rc;
   push_shift(e->size_surf_stack, 0);
-  if (cp) predict_state_w(e);
+  if (cp && !e->cfg.imu_factor) predict_state_w(e);
   rc = scan_open_window(e);
   if (rc != LIO_OK || open_only) return rc;
   rc = scan_solve(e, e->cfg.max_num_iterations);

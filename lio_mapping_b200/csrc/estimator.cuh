@@ -14,6 +14,7 @@
 #include <thread>
 #include "factors_host.h"
 #include "factors_impl.h"
+#include "imu_init.h"
 #include "knn.cuh"
 #include "odom.cuh"
 #include "qr.cuh"
@@ -169,7 +170,8 @@ struct AttachedMap {
 };
 
 // imu_factor = 0 from the odometry's clouds (lio_est_attach_mapping): the estimator's own PointMapping::Process on every message,
-// the NOT_INITED window of the mapped poses and the start-up (ProcessCompactData / ProcessLaserOdom, Estimator.cc:430-856)
+// the NOT_INITED window of the mapped poses and the start-up (ProcessCompactData / ProcessLaserOdom, Estimator.cc:430-856).
+// imu_factor = 1 (lio_est_attach_imu_mapping): the same window, started by RunInitialization (:505-602, :858-958).
 struct Mapping {
   bool on = false;
   bool inited = false;                // stage_flag_ == INITED
@@ -179,6 +181,12 @@ struct Mapping {
   std::vector<std::vector<size_t>> opt_valid;   // opt_valid_idx_, logical frames
   std::vector<std::array<int, 3>> opt_centre;   // opt_cube_centers_, logical frames
   int compact_info[4] = {0, 0, 0, 0}; // inited, cir_buf_count_, pushed by the last call, solved by the last call
+  // imu_factor = 1
+  double initial_time = -1;           // initial_time_: the stamp of the last attempt
+  int attempts = 0, outcome = -1;     // RunInitialization calls, result of the last (kInit*)
+  bool attempted = false;             // the last message ran an attempt
+  M3 R_WI = M3::I();                  // R_WI_
+  std::vector<double> attempt_states; // (W+1) x 16 (lio_est_get_states layout) as the last attempt left them, before any solve
   void release() { *this = Mapping(); }
 };
 
@@ -340,7 +348,8 @@ int refuse_poisoned(lio_est *e);   // sets the "context poisoned" error, returns
 // A push of lio_est_process_compact_* (imu_factor = 0): surf_ds / surf_ds_n, when set, is PointMapping's down-sampled surf stack, copied
 // into the frame slot instead of the VoxelGrid of the scan (:474-480); corner_filtered: the staged corner cloud is that stack's corner
 // cloud, copied likewise; startup: the NOT_INITED push that reaches a full window (:505-517), no transform_es_.
-struct CompactPush { const float4 *surf_ds; const int *surf_ds_n; bool corner_filtered, startup; };
+// tmp_bg: Bgs_[W] as it was when the push made tmp_pre_integration_ (:453), before RunInitialization moved it.
+struct CompactPush { const float4 *surf_ds; const int *surf_ds_n; bool corner_filtered, startup; V3 tmp_bg; };
 int process_scan_body(lio_est *e, const float4 *scan_dev, const int *n_dev, int n_max, bool open_only, const CompactPush *cp = nullptr);
 
 // ---- est_solve.cu
@@ -360,6 +369,6 @@ int slide_window(lio_est *e);
 // ---- est_map.cu
 int lc_push(lio_est *e, bool deskew_corner, bool corner_filtered = false);
 int lc_join(lio_est *e);
-int map_scan_entry(lio_est *e);
+int map_scan_entry(lio_est *e, bool predict);
 int map_step(lio_est *e);
 void predict_state_w(lio_est *e);

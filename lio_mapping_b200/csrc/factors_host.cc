@@ -21,6 +21,24 @@ Preintegration::Preintegration(const V3 &a0, const V3 &g0, const V3 &ba, const V
 }
 
 void Preintegration::push_back(double dt, const V3 &acc1, const V3 &gyr1) {
+  if (keep_samples) { dt_buf.push_back(dt); acc_buf.push_back(acc1); gyr_buf.push_back(gyr1); }
+  propagate(dt, acc1, gyr1);
+}
+
+void Preintegration::repropagate(const V3 &ba, const V3 &bg) {
+  sum_dt = 0;
+  acc0 = lin_acc; gyr0 = lin_gyr;
+  delta_p = V3(); delta_q = Q(); delta_v = V3();
+  lin_ba = ba; lin_bg = bg;
+  std::memset(jac, 0, sizeof(jac));
+  std::memset(cov, 0, sizeof(cov));
+  for (int i = 0; i < 15; ++i) jac[i][i] = 1.0;
+  for (size_t i = 0; i < dt_buf.size(); ++i) propagate(dt_buf[i], acc_buf[i], gyr_buf[i]);
+  sqrt_info_valid = false;
+  cache.reset();
+}
+
+void Preintegration::propagate(double dt, const V3 &acc1, const V3 &gyr1) {
   sqrt_info_valid = false;
   cache.reset();
   const V3 un_acc_0 = rotate(delta_q, acc0 - lin_ba);

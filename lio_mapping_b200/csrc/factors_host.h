@@ -26,8 +26,14 @@ struct Preintegration {
   // whitening matrix LLT(cov^-1).matrixL()^T, cached after the last push_back
   double sqrt_info[15][15];
   bool sqrt_info_valid = false;
+  bool keep_samples = true;         // false: repropagate is never called (the estimator's INITED pre-integrations)
+  std::vector<double> dt_buf;       // the samples pushed so far, for repropagate
+  std::vector<hm::V3> acc_buf, gyr_buf;
   Preintegration(const hm::V3 &acc0, const hm::V3 &gyr0, const hm::V3 &ba, const hm::V3 &bg, const ImuNoise &n);
   void push_back(double dt, const hm::V3 &acc, const hm::V3 &gyr);
+  // IntegrationBase::Repropagate (IntegrationBase.h:110-125): start over from the first sample with new linearisation biases
+  void repropagate(const hm::V3 &ba, const hm::V3 &bg);
+  void propagate(double dt, const hm::V3 &acc, const hm::V3 &gyr);   // one mid-point step (Propagate :278-307)
   void ensure_sqrt_info();
   void to_data(struct PimData &d);
   const struct PimData &data();  // cached plain-data view (valid until the next push_back)

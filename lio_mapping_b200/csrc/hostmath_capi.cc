@@ -7,6 +7,7 @@
 #include "../../include/lio_b200.h"
 #include "factors_host.h"
 #include "hostmath.h"
+#include "imu_init.h"
 #include "solver_host.h"
 #include <cmath>
 #include <new>
@@ -137,5 +138,41 @@ extern "C" int lio_imu_factor_evaluate(lio_pim *p, const double pose_i[7], const
       for (int c = 0; c < 9; ++c) { if (J1) J1[a * 9 + c] = Jsi[a][c]; if (J3) J3[a * 9 + c] = Jsj[a][c]; }
     }
   }
+  return LIO_OK;
+}
+
+extern "C" int lio_imu_run_initialization_host(int W, const float *laser_tf7, lio_pim *const *pims, const float tlb7[7], double g_norm,
+                                               const double *bas, double *bgs, double *vs, double R_WI9[9], double *ps, double *rs, double g3[3],
+                                               int *outcome) {
+  if (W < 5 || !laser_tf7 || !pims || !tlb7 || !bas || !bgs || !vs || !R_WI9 || !ps || !rs || !g3 || !outcome) return LIO_ERR_INVALID;
+  std::vector<TwistF> tf(W + 1);
+  std::vector<Preintegration *> pre(W + 1);
+  std::vector<V3> Ba(W + 1), Bg(W + 1), Vs(W + 1), Ps(W + 1);
+  std::vector<M3> Rs(W + 1);
+  for (int i = 0; i <= W; ++i) {
+    if (!pims[i]) return LIO_ERR_INVALID;
+    const float *t = laser_tf7 + 7 * i;
+    tf[i] = TwistF{t[0], t[1], t[2], t[3], t[4], t[5], t[6]};
+    pre[i] = pims[i]->p.get();
+    Ba[i] = V3(bas + 3 * i); Bg[i] = V3(bgs + 3 * i); Vs[i] = V3(vs + 3 * i);
+  }
+  M3 R_WI;
+  for (int a = 0; a < 3; ++a) for (int b = 0; b < 3; ++b) R_WI(a, b) = R_WI9[3 * a + b];
+  V3 g;
+  const TwistF tlb{tlb7[0], tlb7[1], tlb7[2], tlb7[3], tlb7[4], tlb7[5], tlb7[6]};
+  const int rc = run_initialization(W, tf.data(), pre.data(), tlb, g_norm, Ba.data(), Bg.data(), Vs.data(), R_WI, Ps.data(), Rs.data(), g);
+  if (rc == kInitNotFinite) {
+    lio_set_last_error(__FILE__, __LINE__, "RunInitialization: non-finite result");
+    return LIO_ERR_NUMERIC;
+  }
+  *outcome = rc;
+  if (rc == kInitLowExcitation) return LIO_OK;
+  for (int i = 0; i <= W; ++i)
+    for (int k = 0; k < 3; ++k) {
+      bgs[3 * i + k] = Bg[i][k]; vs[3 * i + k] = Vs[i][k]; ps[3 * i + k] = Ps[i][k];
+      for (int c = 0; c < 3; ++c) rs[9 * i + 3 * k + c] = Rs[i](k, c);
+    }
+  for (int a = 0; a < 3; ++a) for (int b = 0; b < 3; ++b) R_WI9[3 * a + b] = R_WI(a, b);
+  for (int k = 0; k < 3; ++k) g3[k] = g[k];
   return LIO_OK;
 }

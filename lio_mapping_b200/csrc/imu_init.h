@@ -1,0 +1,17 @@
+// lio_mapping_b200 — Estimator::RunInitialization with ImuInitializer::Initialization on the host (imu_init.cc)
+#pragma once
+#include "factors_host.h"
+#include "twistf.h"
+
+namespace lio {
+
+enum { kInitLowExcitation = 0, kInitGravityFailed = 1, kInitSuccess = 2, kInitNotFinite = -1 };
+
+// One attempt on a full window of W + 1 frames (W >= 5): laser transforms tf[0..W] (transform_aft_mapped_ of each push), their
+// pre-integrations pre[0..W] (repropagated in place), transform_lb_.  Bgs, Vs and R_WI are read and written, Ps / Rs / g_vec written.
+// Returns kInitLowExcitation with nothing changed, else kInitGravityFailed / kInitSuccess with the side effects the reference has
+// either way, or kInitNotFinite when a result is not finite.
+int run_initialization(int W, const TwistF *tf, Preintegration *const *pre, const TwistF &tlb, double g_norm, const hm::V3 *Bas,
+                       hm::V3 *Bgs, hm::V3 *Vs, hm::M3 &R_WI, hm::V3 *Ps, hm::M3 *Rs, hm::V3 &g_vec);
+
+}  // namespace lio

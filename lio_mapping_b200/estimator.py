@@ -99,6 +99,23 @@ class Pim:
             pass
 
 
+def run_initialization(laser_tf7, pims, tlb7, g_norm, bas, bgs, vs, R_WI):
+    """Estimator::RunInitialization on host arrays (lio_imu_run_initialization_host): W + 1 laser transforms (tf7), W + 1 Pim objects
+    (repropagated in place), transform_lb_ (tf7), g_norm, biases / velocities (W+1) x 3 and R_WI_ (3 x 3).  Returns a dict with the
+    outcome (0 excitation too low, 1 gravity check failed, 2 success) and the states, biases, velocities, g_vec and R_WI after the
+    attempt (unchanged inputs for outcome 0)."""
+    tf = np.ascontiguousarray(laser_tf7, np.float32).reshape(-1, 7)
+    W = tf.shape[0] - 1
+    bgs = np.array(bgs, np.float64).reshape(W + 1, 3); vs = np.array(vs, np.float64).reshape(W + 1, 3)
+    R = np.array(R_WI, np.float64).reshape(3, 3).copy()
+    ps = np.zeros((W + 1, 3)); rs = np.zeros((W + 1, 3, 3)); g = np.zeros(3); out = C.c_int(-1)
+    handles = (C.c_void_p * (W + 1))(*[p.h.value for p in pims])
+    _lib.check(_lib.lib().lio_imu_run_initialization_host(W, tf, handles, np.ascontiguousarray(tlb7, np.float32), float(g_norm),
+                                                          _d(np.asarray(bas, np.float64).reshape(-1)), bgs, vs, R, ps, rs, g, C.byref(out)),
+               "lio_imu_run_initialization_host")
+    return dict(outcome=out.value, Ps=ps, Rs=rs, Vs=vs, Bgs=bgs, g_vec=g, R_WI=R)
+
+
 class Estimator:
     def __init__(self, device: int = 0, stream: int = 0, **cfg):
         L = _lib.lib()
@@ -362,22 +379,46 @@ class Estimator:
         _lib.check(_lib.lib().lio_est_attach_mapping(self.h, pm.h), "lio_est_attach_mapping")
         self._map = pm
 
-    def process_compact(self, corner_last, surf_last, full_cloud, transform_sum7):
+    def attach_imu_mapping(self, pm):
+        """The same for an imu_factor = 1 estimator (window_size >= 5, estimate_extrinsic != 2): the window of mapped poses is started by
+        ImuInitializer on the IMU fed through process_imu, after which the estimator runs the attach_map path.  Feed it with
+        process_compact(..., stamp=) / process_compact_dev(..., stamp=); imu_init_status() reports the attempts."""
+        _lib.check(_lib.lib().lio_est_attach_imu_mapping(self.h, pm.h), "lio_est_attach_imu_mapping")
+        self._map = pm
+
+    def process_compact(self, corner_last, surf_last, full_cloud, transform_sum7, stamp=None):
         """One /compact_data message from host arrays (the odometry's /laser_cloud_corner_last, /laser_cloud_surf_last, full cloud
-        and transform_sum_).  Returns compact_status()."""
+        and transform_sum_); stamp is the message's header.stamp in seconds, which an IMU mapping needs.  Returns compact_status()."""
         arrs = [np.ascontiguousarray(a, np.float32).reshape(-1, 4) for a in (corner_last, surf_last, full_cloud)]
         n = [a.shape[0] for a in arrs]
         arrs = [a if a.shape[0] else np.zeros((1, 4), np.float32) for a in arrs]
-        _lib.check(_lib.lib().lio_est_process_compact_host(self.h, arrs[0], n[0], arrs[1], n[1], arrs[2], n[2],
-                                                           np.ascontiguousarray(transform_sum7, np.float32)), "lio_est_process_compact_host")
+        t = np.ascontiguousarray(transform_sum7, np.float32)
+        L = _lib.lib()
+        if stamp is None:
+            _lib.check(L.lio_est_process_compact_host(self.h, arrs[0], n[0], arrs[1], n[1], arrs[2], n[2], t), "lio_est_process_compact_host")
+        else:
+            _lib.check(L.lio_est_process_compact_stamped_host(self.h, arrs[0], n[0], arrs[1], n[1], arrs[2], n[2], t, float(stamp)),
+                       "lio_est_process_compact_stamped_host")
         return self.compact_status()
 
-    def process_compact_dev(self, ptrs, n_dev_ptr: int, n_max, transform_sum7):
+    def process_compact_dev(self, ptrs, n_dev_ptr: int, n_max, transform_sum7, stamp=None):
         """The same with the clouds in HBM: exactly what PointOdometry.clouds_dev() returns (ptrs, n_dev_ptr, n_max)."""
-        _lib.check(_lib.lib().lio_est_process_compact_dev(self.h, C.c_void_p(ptrs[0]), C.c_void_p(ptrs[1]), C.c_void_p(ptrs[2]),
-                                                          C.c_void_p(n_dev_ptr), np.ascontiguousarray(n_max, np.int32),
-                                                          np.ascontiguousarray(transform_sum7, np.float32)), "lio_est_process_compact_dev")
+        args = (self.h, C.c_void_p(ptrs[0]), C.c_void_p(ptrs[1]), C.c_void_p(ptrs[2]), C.c_void_p(n_dev_ptr),
+                np.ascontiguousarray(n_max, np.int32), np.ascontiguousarray(transform_sum7, np.float32))
+        L = _lib.lib()
+        if stamp is None:
+            _lib.check(L.lio_est_process_compact_dev(*args), "lio_est_process_compact_dev")
+        else:
+            _lib.check(L.lio_est_process_compact_stamped_dev(*args, float(stamp)), "lio_est_process_compact_stamped_dev")
         return self.compact_status()
+
+    def imu_init_status(self):
+        """{attempts, outcome (-1 none, 0 excitation too low, 1 gravity check failed, 2 success), attempted by the last message, inited,
+        g_vec (g_vec_), R_WI (R_WI_), states ((W+1) x 16 as the last attempt left them, before any solve; NaN before the first)}."""
+        info = np.zeros(4, np.int32); g = np.zeros(3); R = np.zeros(9); s = np.full((self.W + 1) * 16, np.nan)
+        _lib.check(_lib.lib().lio_est_imu_init_status(self.h, info, g, R, s), "lio_est_imu_init_status")
+        return dict(attempts=int(info[0]), outcome=int(info[1]), attempted=bool(info[2]), inited=bool(info[3]), g_vec=g, R_WI=R.reshape(3, 3),
+                    states=s.reshape(-1, 16))
 
     def compact_status(self):
         """{inited, cir_buf_count, pushed, solved} of the last process_compact call."""
