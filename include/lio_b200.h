@@ -421,6 +421,12 @@ int lio_imu_factor_evaluate(lio_pim *p, const double pose_i[7], const double sb_
  * g3 = R0 g_in_laser; vs is the refined velocities only on success.  A non-finite result returns LIO_ERR_NUMERIC. */
 int lio_imu_run_initialization_host(int W, const float *laser_tf7, lio_pim *const *pims, const float tlb7[7], double g_norm, const double *bas,
                                     double *bgs, double *vs, double R_WI9[9], double *ps, double *rs, double g3[3], int *outcome);
+/* ImuInitializer::EstimateExtrinsicRotation (src/imu_processor/ImuInitializer.cc:353-419) on host arrays: the calibration the imu_factor = 1
+ * estimator runs before RunInitialization with estimate_extrinsic = 2 (lio_est_enable_extrinsic_calibration).  W >= 1; laser_tf7 and pims as
+ * for lio_imu_run_initialization_host (pims 1..W are read, none is changed); tlb7 transform_lb_ in / out.  The rotation of tlb7 is overwritten
+ * whether or not the call succeeds, its position never.  sv4 = the singular values of the 4W x 4 system, descending; ok = 1 iff sv4[2] > 0.25.
+ * Needs no device. */
+int lio_imu_estimate_extrinsic_rotation_host(int W, const float *laser_tf7, lio_pim *const *pims, float tlb7[7], double sv4[4], int *ok);
 
 /* ------------------------------------------------------------------------------------------
  * Stages B+C+D — lio::Estimator in steady state (stage_flag_ == INITED)
@@ -646,8 +652,8 @@ int lio_est_process_compact_host(lio_est *est, const float *corner, int nc, cons
 int lio_est_compact_status(lio_est *est, int info4[4]);
 /* ---- imu_factor = 1 from the odometry's clouds and the IMU: the estimator starts itself with ImuInitializer (ProcessLaserOdom NOT_INITED
  * :505-602, RunInitialization :858-958) and then runs the lio_est_attach_map path.
- *   lio_est_attach_imu_mapping   as lio_est_attach_mapping, with imu_factor = 1 and W >= 5; estimate_extrinsic = 2 is refused.  Refusals
- *                                return LIO_ERR_INVALID and change nothing.
+ *   lio_est_attach_imu_mapping   as lio_est_attach_mapping, with imu_factor = 1 and W >= 5; estimate_extrinsic = 2 is refused unless
+ *                                lio_est_enable_extrinsic_calibration was called.  Refusals return LIO_ERR_INVALID and change nothing.
  *   lio_est_process_compact_stamped_dev / _host
  *                                the compact entries with the message's header.stamp, which the 0.1 s gate between attempts (:533-536)
  *                                compares; feed the IMU samples up to that stamp before the call.  On an imu_factor = 0 mapping they
@@ -666,8 +672,24 @@ int lio_est_compact_status(lio_est *est, int info4[4]);
  *   lio_est_imu_init_status      info4 = {attempts, outcome of the last (-1 none, 0 excitation, 1 gravity check, 2 success), whether the
  *                                last message ran an attempt, inited}; g3 = g_vec_, R_WI9 = R_WI_ row-major; states16 (W+1) x 16 in the
  *                                lio_est_get_states layout as the last attempt left them (on success: before the first solve; untouched
- *                                before the first attempt).  g3, R_WI9 and states16 may be NULL. */
+ *                                before the first attempt).  g3, R_WI9 and states16 may be NULL.
+ *   lio_est_enable_extrinsic_calibration
+ *                                opt-in for estimate_extrinsic = 2 (the reference's extrinsic stage 2, Estimator.cc:520-531): accepted only
+ *                                on an imu_factor = 1, estimate_extrinsic = 2 context, once, before lio_est_attach_imu_mapping and before
+ *                                any frame; anything else returns LIO_ERR_INVALID and changes nothing.  With it, every full-window
+ *                                NOT_INITED push runs EstimateExtrinsicRotation (lio_imu_estimate_extrinsic_rotation_host) on the window,
+ *                                with no stamp gate, before the gated RunInitialization, until one succeeds.  Each call overwrites the
+ *                                rotation of transform_lb_ (lio_est_get_extrinsic; the position never changes), which the attempt, the
+ *                                start-up states, the prediction, de-skew and the solve then use.  While no call has succeeded no
+ *                                RunInitialization runs and the push ends in SlideWindow's state copy; after a success the extrinsic
+ *                                stage is 1 and the same message goes on to the gate.
+ *   lio_est_extrinsic_calib_status
+ *                                info4 = {calibrations run, result of the last (-1 none, 0 failed, 1 success), whether the last message
+ *                                ran one, current extrinsic stage}; sv4 = the last call's singular values, descending (may be NULL).
+ *                                lio_est_imu_init_status's attempts count RunInitialization calls only. */
 int lio_est_attach_imu_mapping(lio_est *est, lio_pm *pm);
+int lio_est_enable_extrinsic_calibration(lio_est *est);
+int lio_est_extrinsic_calib_status(lio_est *est, int info4[4], double sv4[4]);
 int lio_est_process_compact_stamped_dev(lio_est *est, const float *corner_dev, const float *surf_dev, const float *full_dev, const int *n3_dev,
                                         const int n3_max[3], const float transform_sum7[7], double stamp);
 int lio_est_process_compact_stamped_host(lio_est *est, const float *corner, int nc, const float *surf, int ns, const float *full, int nf,

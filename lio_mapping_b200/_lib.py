@@ -209,6 +209,9 @@ def lib():
     L.lio_est_imu_init_status.argtypes = [vp, i32p, f64p, f64p, f64p]
     L.lio_imu_run_initialization_host.argtypes = [ip, f32p, C.POINTER(vp), f32p, C.c_double, f64p, f64p, f64p, f64p, f64p, f64p, f64p,
                                                   C.POINTER(ip)]
+    L.lio_imu_estimate_extrinsic_rotation_host.argtypes = [ip, f32p, C.POINTER(vp), f32p, f64p, C.POINTER(ip)]
+    L.lio_est_enable_extrinsic_calibration.argtypes = [vp]
+    L.lio_est_extrinsic_calib_status.argtypes = [vp, i32p, f64p]
     L.lio_mb_process_map_dev.argtypes = [vp, vp, vp, vp, vp, i32p, f32p, f32p, f32p, i32p]
     L.lio_po_process_dev.argtypes = [vp, C.POINTER(vp), C.POINTER(vp), i32p, f32p, f32p, i32p]
     L.lio_po_clouds_dev.argtypes = [vp, C.POINTER(vp), C.POINTER(vp), i32p]

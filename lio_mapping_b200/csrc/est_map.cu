@@ -360,7 +360,8 @@ static int attach_mapping(lio_est *e, lio_pm *pm, bool imu) {
   else if (!imu && e->cfg.imu_factor) why = "lio_est_attach_mapping needs imu_factor = 0 (lio_est_attach_imu_mapping takes imu_factor = 1)";
   else if (imu && !e->cfg.imu_factor) why = "lio_est_attach_imu_mapping needs imu_factor = 1";
   else if (imu && e->W < 5) why = "lio_est_attach_imu_mapping: ImuInitializer needs window_size >= 5 (ApproximateGravity)";
-  else if (imu && e->extrinsic_stage == 2) why = "lio_est_attach_imu_mapping: estimate_extrinsic = 2 (EstimateExtrinsicRotation) is not supported";
+  else if (imu && e->extrinsic_stage == 2 && !e->calib.on)
+    why = "lio_est_attach_imu_mapping: estimate_extrinsic = 2 needs lio_est_enable_extrinsic_calibration first";
   else if (e->world > 1 || e->px.npeers || e->px.fpeers) why = "not supported on a sharded context";
   if (why) { lio_set_last_error(__FILE__, __LINE__, why); return LIO_ERR_INVALID; }
   const int rc = attach_common(e, pm, true);
@@ -378,13 +379,44 @@ static int attach_mapping(lio_est *e, lio_pm *pm, bool imu) {
 extern "C" int lio_est_attach_mapping(lio_est *e, lio_pm *pm) { return attach_mapping(e, pm, false); }
 extern "C" int lio_est_attach_imu_mapping(lio_est *e, lio_pm *pm) { return attach_mapping(e, pm, true); }
 
-// RunInitialization (:858-958) on the window the push has just filled: all_laser_transforms_ 0..W and their pre-integrations, which are
-// pre_[1..W] and tmp_pre (the push moves them one place later; the objects, which the attempt repropagates, are the same)
-static int imu_attempt(lio_est *e, double stamp) {
+extern "C" int lio_est_enable_extrinsic_calibration(lio_est *e) {
+  if (!e) return LIO_ERR_INVALID;
+  const char *why = nullptr;
+  if (!e->cfg.imu_factor || e->extrinsic_stage != 2) why = "lio_est_enable_extrinsic_calibration needs imu_factor = 1 and estimate_extrinsic = 2";
+  else if (e->calib.on) why = "lio_est_enable_extrinsic_calibration: call it once";
+  else if (e->mapping.on || e->map.pm || e->frames_started || e->tmp_pre) why = "lio_est_enable_extrinsic_calibration: call it before the attach and any frame";
+  if (why) { lio_set_last_error(__FILE__, __LINE__, why); return LIO_ERR_INVALID; }
+  e->calib.on = true;
+  return LIO_OK;
+}
+
+// all_laser_transforms_ 0..W's pre-integrations on the window the push has just filled: pre_[1..W] and tmp_pre (the push moves them one
+// place later; the objects, which an attempt repropagates, are the same)
+static std::vector<Preintegration *> window_pre(lio_est *e) {
   const int W = e->W;
   std::vector<Preintegration *> pre(W + 1);
   for (int i = 0; i < W; ++i) pre[i] = e->pre[i + 1].get();
   pre[W] = e->tmp_pre.get();
+  return pre;
+}
+
+// EstimateExtrinsicRotation (:520-531) on that window, with no stamp gate: transform_lb_'s rotation is overwritten whether or not it
+// succeeds; a success ends extrinsic stage 2
+static void calib_attempt(lio_est *e) {
+  const std::vector<Preintegration *> pre = window_pre(e);
+  lio::TwistF tlb = lb_twist(e);
+  const bool ok = estimate_extrinsic_rotation(e->W, e->mapping.laser_tf.data(), pre.data(), tlb, e->calib.sv);
+  e->tlb_q[0] = tlb.qx; e->tlb_q[1] = tlb.qy; e->tlb_q[2] = tlb.qz; e->tlb_q[3] = tlb.qw;
+  ++e->calib.runs;
+  e->calib.result = ok ? 1 : 0;
+  e->calib.ran = true;
+  if (ok) e->extrinsic_stage = 1;
+}
+
+// RunInitialization (:858-958) on the same window
+static int imu_attempt(lio_est *e, double stamp) {
+  const int W = e->W;
+  const std::vector<Preintegration *> pre = window_pre(e);
   const int rc = run_initialization(W, e->mapping.laser_tf.data(), pre.data(), lb_twist(e), e->noise.g_norm, e->Bas.data(), e->Bgs.data(),
                                     e->Vs.data(), e->mapping.R_WI, e->Ps.data(), e->Rs.data(), e->g_vec);
   ++e->mapping.attempts;
@@ -419,6 +451,7 @@ static int compact_body(lio_est *e, const float4 *const src[3], const int *n3_de
   ++e->mapping.recv_count;
   e->mapping.compact_info[0] = e->mapping.inited ? 1 : 0; e->mapping.compact_info[1] = e->mapping.cir_count; e->mapping.compact_info[2] = e->mapping.compact_info[3] = 0;
   e->mapping.attempted = false;
+  e->calib.ran = false;
   if (!e->mapping.inited && e->mapping.recv_count % e->cfg.init_window_factor != 0) return LIO_OK;   // :436-439
   // the push (:441-487): the laser transform is transform_aft_mapped_, the stacks PointMapping's down-sampled ones unless the INITED
   // de-skew rules push their own (:474-480, :628-693)
@@ -451,9 +484,10 @@ static int compact_body(lio_est *e, const float4 *const src[3], const int *n3_de
   const int c = e->mapping.cir_count;
   const V3 tmp_bg = e->Bgs[c];
   bool startup = !e->mapping.inited && c == W;
-  if (startup && e->cfg.imu_factor) {   // :533-537
+  if (startup && e->cfg.imu_factor) {   // :520-537
     startup = false;
-    if (stamp - e->mapping.initial_time > 0.1) {
+    if (e->extrinsic_stage == 2) calib_attempt(e);
+    if (e->extrinsic_stage != 2 && stamp - e->mapping.initial_time > 0.1) {
       if ((rc = imu_attempt(e, stamp)) != LIO_OK) return rc;
       startup = e->mapping.outcome == kInitSuccess;
     }
@@ -604,5 +638,12 @@ extern "C" int lio_est_imu_init_status(lio_est *e, int info4[4], double g3[3], d
   if (R_WI9) for (int a = 0; a < 3; ++a) for (int b = 0; b < 3; ++b) R_WI9[3 * a + b] = e->mapping.R_WI(a, b);
   if (states16 && !e->mapping.attempt_states.empty())
     std::memcpy(states16, e->mapping.attempt_states.data(), sizeof(double) * e->mapping.attempt_states.size());
+  return LIO_OK;
+}
+
+extern "C" int lio_est_extrinsic_calib_status(lio_est *e, int info4[4], double sv4[4]) {
+  if (!e || !info4) return LIO_ERR_INVALID;
+  info4[0] = e->calib.runs; info4[1] = e->calib.result; info4[2] = e->calib.ran ? 1 : 0; info4[3] = e->extrinsic_stage;
+  if (sv4) for (int k = 0; k < 4; ++k) sv4[k] = e->calib.sv[k];
   return LIO_OK;
 }

@@ -190,6 +190,14 @@ struct Mapping {
   void release() { *this = Mapping(); }
 };
 
+// estimate_extrinsic = 2 on an IMU mapping (lio_est_enable_extrinsic_calibration): EstimateExtrinsicRotation before RunInitialization
+struct ExtrinsicCalib {
+  bool on = false;
+  int runs = 0, result = -1;          // calls, result of the last (0 failed, 1 success)
+  bool ran = false;                   // the last message ran one
+  double sv[4] = {0, 0, 0, 0};        // the last call's singular values, descending
+};
+
 // Peer memory of a sharded context.  Rows exchange: one device allocation per rank, laid out as
 //   [2 parities][kMaxOpt * kAsmStride doubles] | unsigned flag[kMaxPeers] | int err
 // Feature exchange: all feature buffers (xyz+score, coefficients, counts) live in ONE allocation with two parities, so that a sharded
@@ -248,6 +256,7 @@ struct lio_est {
   bool convergence_flag = false, init_local_map = false;
   int extrinsic_stage = 1;
   bool ex_constant = false;
+  ExtrinsicCalib calib;
   // ---- device
   std::vector<float4 *> slot_ptr;    // physical slots
   std::vector<int> slot_of;          // logical frame -> physical slot

@@ -176,3 +176,19 @@ extern "C" int lio_imu_run_initialization_host(int W, const float *laser_tf7, li
   for (int k = 0; k < 3; ++k) g3[k] = g[k];
   return LIO_OK;
 }
+
+extern "C" int lio_imu_estimate_extrinsic_rotation_host(int W, const float *laser_tf7, lio_pim *const *pims, float tlb7[7], double sv4[4], int *ok) {
+  if (W < 1 || !laser_tf7 || !pims || !tlb7 || !sv4 || !ok) return LIO_ERR_INVALID;
+  std::vector<TwistF> tf(W + 1);
+  std::vector<Preintegration *> pre(W + 1);
+  for (int i = 0; i <= W; ++i) {
+    if (!pims[i]) return LIO_ERR_INVALID;
+    const float *t = laser_tf7 + 7 * i;
+    tf[i] = TwistF{t[0], t[1], t[2], t[3], t[4], t[5], t[6]};
+    pre[i] = pims[i]->p.get();
+  }
+  TwistF tlb{tlb7[0], tlb7[1], tlb7[2], tlb7[3], tlb7[4], tlb7[5], tlb7[6]};
+  *ok = estimate_extrinsic_rotation(W, tf.data(), pre.data(), tlb, sv4) ? 1 : 0;
+  tlb7[0] = tlb.qx; tlb7[1] = tlb.qy; tlb7[2] = tlb.qz; tlb7[3] = tlb.qw;
+  return LIO_OK;
+}

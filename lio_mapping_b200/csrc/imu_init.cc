@@ -1,8 +1,10 @@
 // lio_mapping_b200 — the IMU start-up of the imu_factor = 1 estimator on the host: Estimator::RunInitialization
 // (src/imu_processor/Estimator.cc:858-958) with ImuInitializer::Initialization (src/imu_processor/ImuInitializer.cc:35-308,
-// :421-452).  One attempt solves a 3 x 3 gyro-bias system, a 3 x 3 gravity system and five (3(W+1)+2)^2 refinements; every
-// input (the mapped laser poses, the pre-integrations) is host state, so it runs here and not on the device.
+// :421-452), and the extrinsic-rotation calibration before it, ImuInitializer::EstimateExtrinsicRotation (:353-419).  One attempt
+// solves a 3 x 3 gyro-bias system, a 3 x 3 gravity system and five (3(W+1)+2)^2 refinements, one calibration a 4W x 4 least-squares
+// system; every input (the mapped laser poses, the pre-integrations) is host state, so both run here and not on the device.
 #include "imu_init.h"
+#include <algorithm>
 #include <cmath>
 #include <limits>
 
@@ -64,18 +66,21 @@ void tangent_basis(const V3 &g0, V3 &b, V3 &c) {
   c = cross(a, b);
 }
 
+// (q_i^* q_j).cast<double>() with the product in float: the laser rotation between two pushes (:58-60, :369-370)
+Q laser_delta_q(const TwistF &ti, const TwistF &tj) {
+  const float cx = -ti.qx, cy = -ti.qy, cz = -ti.qz, cw = ti.qw;
+  const float wx = cw * tj.qx + cx * tj.qw + cy * tj.qz - cz * tj.qy;
+  const float wy = cw * tj.qy + cy * tj.qw + cz * tj.qx - cx * tj.qz;
+  const float wz = cw * tj.qz + cz * tj.qw + cx * tj.qy - cy * tj.qx;
+  const float ww = cw * tj.qw - cx * tj.qx - cy * tj.qy - cz * tj.qz;
+  return Q((double)ww, (double)wx, (double)wy, (double)wz);
+}
+
 // EstimateGyroBias (:49-90)
 void estimate_gyro_bias(int W, const TwistF *tf, Preintegration *const *pre, V3 *Bgs) {
   std::vector<double> A(9, 0.0), b(3, 0.0), dbg;
   for (int i = 0; i < W; ++i) {
-    // Quaterniond(q_i^* q_j) with the product in float
-    const TwistF &ti = tf[i], &tj = tf[i + 1];
-    const float cx = -ti.qx, cy = -ti.qy, cz = -ti.qz, cw = ti.qw;
-    const float wx = cw * tj.qx + cx * tj.qw + cy * tj.qz - cz * tj.qy;
-    const float wy = cw * tj.qy + cy * tj.qw + cz * tj.qx - cx * tj.qz;
-    const float wz = cw * tj.qz + cz * tj.qw + cx * tj.qy - cy * tj.qx;
-    const float ww = cw * tj.qw - cx * tj.qx - cy * tj.qy - cz * tj.qz;
-    const Q q_ij((double)ww, (double)wx, (double)wy, (double)wz);
+    const Q q_ij = laser_delta_q(tf[i], tf[i + 1]);
     const Preintegration &p = *pre[i + 1];
     const V3 tb = (conj(p.delta_q) * q_ij).vec() * 2.0;
     for (int r = 0; r < 3; ++r) {
@@ -232,6 +237,56 @@ int run_initialization(int W, const TwistF *tf, Preintegration *const *pre, cons
   for (int i = 0; i <= W; ++i) finite = finite && finite3(Ps[i]) && finite3(Vs[i]) && finite3(Bgs[i]);
   if (!finite) return kInitNotFinite;
   return ok ? kInitSuccess : kInitGravityFailed;
+}
+
+// EstimateExtrinsicRotation (ImuInitializer.cc:353-419).  Row block i of A is huber_i (LeftQuatMatrix(q_laser) - RightQuatMatrix(q_imu))
+// (math_utils.h:140-161, coefficient order x y z w).  The reference takes Eigen::JacobiSVD of A; here the singular values and V come
+// from the symmetric eigen-decomposition of the 4 x 4 A^T A (hm::sym_eigen: Householder tridiagonalisation, then implicit QL), with
+// sigma_k = sqrt(lambda_k) and x the eigenvector of the smallest eigenvalue.  Every block row has norm <= 2 huber, and a success needs
+// sigma_2 > 0.25, so there the gap below it bounds x's error to about 1e-13; on a failure x is what the reference would write to the
+// same accuracy only when the two smallest singular values are apart.
+bool estimate_extrinsic_rotation(int W, const TwistF *tf, Preintegration *const *pre, TwistF &tlb, double sv[4]) {
+  const TwistF bl = twist_inverse(tlb);   // transform_lb.inverse(), rot cast to double (:356-357)
+  const Q rot_bl((double)bl.qw, (double)bl.qx, (double)bl.qy, (double)bl.qz);
+  Mat AtA(4, 4);
+  for (int i = 0; i < W; ++i) {
+    const Q q_imu = pre[i + 1]->delta_q;                 // :367
+    const Q q_laser = laser_delta_q(tf[i], tf[i + 1]);   // :369-370
+    const Q q_from_imu = conj(rot_bl) * q_imu * rot_bl;  // :372
+    const Q d = q_laser * conj(q_from_imu);              // Eigen angularDistance, in degrees (:374)
+    const double deg = 180 / M_PI * (2.0 * std::atan2(std::sqrt(d.x * d.x + d.y * d.y + d.z * d.z), std::fabs(d.w)));
+    const double huber = deg > 5.0 ? 5.0 / deg : 1.0;   // :378
+    const double lv[3] = {q_laser.x, q_laser.y, q_laser.z}, rv[3] = {q_imu.x, q_imu.y, q_imu.z};
+    double L[4][4] = {}, R[4][4] = {}, B[4][4];
+    const double ls[3][3] = {{0, -lv[2], lv[1]}, {lv[2], 0, -lv[0]}, {-lv[1], lv[0], 0}};
+    const double rs[3][3] = {{0, -rv[2], rv[1]}, {rv[2], 0, -rv[0]}, {-rv[1], rv[0], 0}};
+    for (int a = 0; a < 3; ++a) {
+      for (int c = 0; c < 3; ++c) {
+        L[a][c] = (a == c ? q_laser.w : 0.0) + ls[a][c];
+        R[a][c] = (a == c ? q_imu.w : 0.0) - rs[a][c];
+      }
+      L[3][a] = -lv[a]; L[a][3] = lv[a];
+      R[3][a] = -rv[a]; R[a][3] = rv[a];
+    }
+    L[3][3] = q_laser.w; R[3][3] = q_imu.w;
+    for (int a = 0; a < 4; ++a) for (int c = 0; c < 4; ++c) B[a][c] = huber * (L[a][c] - R[a][c]);   // :383
+    for (int a = 0; a < 4; ++a)
+      for (int c = 0; c < 4; ++c) for (int k = 0; k < 4; ++k) AtA(a, c) += B[k][a] * B[k][c];
+  }
+  Vec lambda;
+  Mat V;
+  sym_eigen(AtA, lambda, V, 1);   // ascending
+  for (int k = 0; k < 4; ++k) sv[k] = std::sqrt(std::max(lambda[3 - k], 0.0));
+  // Quaterniond(x) with x = V.col(3) (coefficients x y z w), then transform_lb.rot = x.cast<float>().toRotationMatrix() (:399-402):
+  // Eigen's quaternion-to-matrix formula without normalisation, then its matrix-to-quaternion.  The sign of x cancels.
+  const float qx = (float)V(0, 0), qy = (float)V(1, 0), qz = (float)V(2, 0), qw = (float)V(3, 0);
+  const float tx = 2.f * qx, ty = 2.f * qy, tz = 2.f * qz;
+  const float twx = tx * qw, twy = ty * qw, twz = tz * qw, txx = tx * qx, txy = ty * qx, txz = tz * qx, tyy = ty * qy, tyz = tz * qy, tzz = tz * qz;
+  const float M[9] = {1.f - (tyy + tzz), txy - twz, txz + twy, txy + twz, 1.f - (txx + tzz), tyz - twx, txz - twy, tyz + twx, 1.f - (txx + tyy)};
+  float q[4];
+  matrix_to_quat(M, q);
+  tlb.qx = q[0]; tlb.qy = q[1]; tlb.qz = q[2]; tlb.qw = q[3];
+  return sv[2] > 0.25;   // singularValues().tail<3>()(1) > 0.25 (:404-413)
 }
 
 }  // namespace lio

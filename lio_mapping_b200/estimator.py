@@ -116,6 +116,19 @@ def run_initialization(laser_tf7, pims, tlb7, g_norm, bas, bgs, vs, R_WI):
     return dict(outcome=out.value, Ps=ps, Rs=rs, Vs=vs, Bgs=bgs, g_vec=g, R_WI=R)
 
 
+def estimate_extrinsic_rotation(laser_tf7, pims, tlb7):
+    """ImuInitializer::EstimateExtrinsicRotation on host arrays (lio_imu_estimate_extrinsic_rotation_host): W + 1 laser transforms (tf7),
+    W + 1 Pim objects (frame i's ends at frame i; read only) and transform_lb_ (tf7).  Returns (ok, tlb7 with the new rotation and the
+    same position, the four singular values descending); the rotation is replaced whether or not ok."""
+    tf = np.ascontiguousarray(laser_tf7, np.float32).reshape(-1, 7)
+    W = tf.shape[0] - 1
+    t = np.array(tlb7, np.float32).reshape(7).copy()
+    sv = np.zeros(4); ok = C.c_int(-1)
+    handles = (C.c_void_p * (W + 1))(*[p.h.value for p in pims])
+    _lib.check(_lib.lib().lio_imu_estimate_extrinsic_rotation_host(W, tf, handles, t, sv, C.byref(ok)), "lio_imu_estimate_extrinsic_rotation_host")
+    return bool(ok.value), t, sv
+
+
 class Estimator:
     def __init__(self, device: int = 0, stream: int = 0, **cfg):
         L = _lib.lib()
@@ -380,11 +393,25 @@ class Estimator:
         self._map = pm
 
     def attach_imu_mapping(self, pm):
-        """The same for an imu_factor = 1 estimator (window_size >= 5, estimate_extrinsic != 2): the window of mapped poses is started by
-        ImuInitializer on the IMU fed through process_imu, after which the estimator runs the attach_map path.  Feed it with
-        process_compact(..., stamp=) / process_compact_dev(..., stamp=); imu_init_status() reports the attempts."""
+        """The same for an imu_factor = 1 estimator (window_size >= 5): the window of mapped poses is started by ImuInitializer on the IMU
+        fed through process_imu, after which the estimator runs the attach_map path.  Feed it with process_compact(..., stamp=) /
+        process_compact_dev(..., stamp=); imu_init_status() reports the attempts.  estimate_extrinsic = 2 is accepted only after
+        enable_extrinsic_calibration()."""
         _lib.check(_lib.lib().lio_est_attach_imu_mapping(self.h, pm.h), "lio_est_attach_imu_mapping")
         self._map = pm
+
+    def enable_extrinsic_calibration(self):
+        """estimate_extrinsic = 2 on an imu_factor = 1 estimator, before attach_imu_mapping and any frame: every full-window push before
+        initialisation then calibrates the extrinsic rotation (EstimateExtrinsicRotation), with no stamp gate, until one call succeeds;
+        RunInitialization runs only from that message on.  Each call replaces the rotation of extrinsic(); its position stays."""
+        _lib.check(_lib.lib().lio_est_enable_extrinsic_calibration(self.h), "lio_est_enable_extrinsic_calibration")
+
+    def extrinsic_calib_status(self):
+        """{runs, result of the last (-1 none, 0 failed, 1 success), ran by the last message, stage (the current extrinsic stage),
+        sv (the last call's four singular values, descending)}."""
+        info = np.zeros(4, np.int32); sv = np.zeros(4)
+        _lib.check(_lib.lib().lio_est_extrinsic_calib_status(self.h, info, sv), "lio_est_extrinsic_calib_status")
+        return dict(runs=int(info[0]), result=int(info[1]), ran=bool(info[2]), stage=int(info[3]), sv=sv)
 
     def process_compact(self, corner_last, surf_last, full_cloud, transform_sum7, stamp=None):
         """One /compact_data message from host arrays (the odometry's /laser_cloud_corner_last, /laser_cloud_surf_last, full cloud
