@@ -92,6 +92,10 @@ int lio_pp_process_dev(lio_pp *pp, const float *xyzi_dev, int n);
  * Round-1 status: restated in the oracle and pinned by a CPU test; the device path was written after the round's GPU
  * budget was spent and is exercised by a non-strict xfail test until it has run on hardware. */
 int lio_pp_process_host_ring(lio_pp *pp, const float *xyzi, const uint16_t *rings, int n);
+/* The same with xyzi (n x float4) and rings (n x uint16) already on the device, e.g. a sensor driver's DMA target: the kernels of
+ * lio_pp_process_host_ring without its uploads (which is "upload, then this entry").  Stream rule and count accessors as for
+ * lio_pp_process_dev: asynchronous on the stream, the inputs are read by work enqueued there; lio_pp_cloud_sizes waits. */
+int lio_pp_process_dev_ring(lio_pp *pp, const float *xyzi_dev, const uint16_t *rings_dev, int n);
 /* Sizes of the six output clouds (synchronises the stream). */
 int lio_pp_cloud_sizes(lio_pp *pp, int sizes[LIO_PP_NUM_CLOUDS]);
 /* Copy one output cloud to the host (cap in points).  Returns the point count via *n. */
@@ -829,6 +833,89 @@ int lio_rm_reset(lio_rm *rm);
  * lio_pcd_write_xyzi is host only and needs no device; a path that cannot be written returns LIO_ERR_INVALID. */
 int lio_pcd_write_xyzi(const char *path, const float *xyzi_host, long long n);
 int lio_rm_write_pcd(lio_rm *rm, const char *path);
+
+/* ------------------------------------------------------------------------------------------
+ * lio_node — lio_processor_node + lio_estimator_node (src/processor_node.cc, src/estimator_node.cc; the graph of the
+ * launch/test_*.launch files) as one device-resident handle: raw sweeps and IMU messages in, everything else inside.
+ * ---------------------------------------------------------------------------------------- */
+/* The pairing the reference's measurement thread runs, as a host seam that needs no device.  Arrivals i = 0..n-1 in order: kind[i] 0 an
+ * IMU message (stamp[i], acc3 / gyr3 row i), 1 a /compact_data message (stamp[i]; its acc / gyr rows are ignored).  After every arrival
+ * MeasurementManager::GetMeasurements (MeasurementManager.cc:54-108, enable_imu = true as MeasurementManager.h:79 leaves it) runs until it
+ * waits:
+ *   - an IMU message not later than the last accepted one is dropped and counted (ImuHandler :110-116);
+ *   - it waits while the newest IMU stamp <= front stamp + msg_time_delay, drops the front message while the oldest IMU stamp >= its stamp
+ *     + delay, and otherwise pops it with every IMU message stamped < stamp + delay, then appends the next IMU message WITHOUT popping it;
+ *   - each released message runs Estimator::ProcessEstimation's loop (Estimator.cc:2682-2736) with curr_time_ kept across messages from -1:
+ *     a sample at or before stamp + delay is integrated with dt = t - curr_time_; the one after it is replaced by w1 * previous + w2 * sample
+ *     (dt_1 = laser - curr, w1 = dt_2 / (dt_1 + dt_2), w2 = dt_1 / (dt_1 + dt_2), no FP contraction) with dt = dt_1.  Every call carries the
+ *     IMU message's own stamp.  A sample stamped exactly at stamp + delay is integrated, stays queued and is integrated again with dt = 0
+ *     at the start of the next message.
+ * Outputs: calls8 = the ProcessImu calls {dt, acc xyz, gyr xyz, stamp} (cap_calls rows); events3 = one row per decided message in decision
+ * order {arrival index, 1 processed / 0 dropped, index of its first call}; imu_dropped = out-of-order IMU messages.  Messages still waiting at
+ * the end have no row.  LIO_ERR_CAPACITY when a capacity is too small. */
+int lio_measure_replay(double msg_time_delay, int n, const int *kind, const double *stamp, const double *acc3, const double *gyr3,
+                       double *calls8, int cap_calls, int *n_calls, int *events3, int cap_events, int *n_events, int *imu_dropped);
+
+typedef struct lio_node_config {
+  int sensor_type;                /* 16, 32, 64 or 320: the presets of processor_node.cc:66-74 (VLP-16 -15..15 deg, HDL-32 -30.67..10.67,
+                                     HDL-64 -24.9..2, 320 = RS-32 -25..15 with the ring field of every point) */
+  lio_pp_config pp;               /* PointProcessorConfig; lower_bound / upper_bound / num_rings come from sensor_type */
+  int odom_io;                    /* odom_io (estimator_node.cc:145-147): PointOdometry(0.1, odom_io)'s io_ratio */
+  double msg_time_delay;          /* msg_time_delay (estimator_node.cc:138-139) */
+  lio_est_config est;             /* the EstimatorConfig subset; imu_factor picks the start-up, estimate_extrinsic = 2 calibrates */
+  float tf_lb7[7];                /* transform_lb_ {qx,qy,qz,qw,px,py,pz} (extrinsic_rotation / extrinsic_translation) */
+  float corner_filter_size;       /* PointMapping leaves (corner_filter_size / surf_filter_size: surf must equal est.surf_filter_size) */
+  float surf_filter_size;
+  float map_filter_size;          /* the surround map's leaf */
+  int max_points;                 /* capacity of one raw sweep (and of the full cloud) */
+  int max_feature_points;         /* capacity of one feature cloud of a sweep (odometry, mapping, the local corner cloud) */
+  int max_pending;                /* depth of the /compact_data queue: published messages waiting for their IMU */
+} lio_node_config;
+typedef struct lio_node lio_node;
+typedef struct lio_node_status {
+  long long sweeps;               /* sweeps run through stage A and the odometry */
+  long long published;            /* /compact_data messages the io_ratio gate published (PointOdometry.cc:725) */
+  long long processed;            /* messages paired and processed by the estimator */
+  long long dropped;              /* messages the pairing dropped (no IMU before stamp + delay, MeasurementManager.cc:73-78) */
+  long long imu_dropped;          /* IMU messages dropped as out of order (MeasurementManager.cc:111-114) */
+  int pending;                    /* messages waiting for IMU */
+  int odom_enabled;               /* 0 once the /enable_odom call has switched the odometry to its pass-through */
+  int inited;                     /* the estimator's stage is INITED */
+  int poisoned;                   /* an estimator failure poisoned the node */
+  double last_stamp;              /* header.stamp of the last processed message (-1 before the first) */
+} lio_node_info;
+void lio_node_default_config(lio_node_config *cfg);
+/* Creates lio_pp (sensor preset), lio_po (scan period 0.1, odom_io, 25 iterations), a publishing lio_pm (the YAML's leaves, 10 iterations,
+ * min_match_sq_dis / min_plane_dis of est) and an estimator with local clouds on, all on cuda_stream; sets tf_lb7, calls
+ * lio_est_enable_extrinsic_calibration when imu_factor = 1 and estimate_extrinsic = 2 (Estimator.cc:520-531), then attaches the mapping
+ * with lio_est_attach_imu_mapping (imu_factor = 1) or lio_est_attach_mapping (imu_factor = 0), and allocates max_pending queue slots in
+ * HBM.  A refusal of any inner create / attach is returned as its status, and nothing stays allocated. */
+int lio_node_create(const lio_node_config *cfg, int device, void *cuda_stream, lio_node **out);
+int lio_node_destroy(lio_node *node);
+/* One IMU message (ImuHandler): dropped and counted when not later than the last accepted one; then every message that GetMeasurements now
+ * releases is processed, in order (see lio_node_push_sweep_dev).  _batch: n messages, stamp[n], acc3 / gyr3 n x 3. */
+int lio_node_push_imu(lio_node *node, double stamp, const double acc[3], const double gyr[3]);
+int lio_node_push_imu_batch(lio_node *node, int n, const double *stamp, const double *acc3, const double *gyr3);
+/* One raw sweep (xyzi n x float4, rings n x uint16 - required with sensor_type 320, refused otherwise - and its stamp): stage A
+ * (lio_pp_process_dev / lio_pp_process_dev_ring), then lio_po_process_dev.  When the io_ratio gate publishes (PointOdometry.cc:725-727) the
+ * three clouds are copied, count-guarded, into a queue slot in HBM with transform_sum_, their host counts and the stamp; then the pairing
+ * runs as after an IMU push.  Processing one message: its ProcessImu calls (lio_est_process_imu), then lio_est_process_compact_stamped_dev
+ * on the slot.  When that message initialised an imu_factor = 1 estimator and enable_deskew or cutoff_deskew is set, the node turns the
+ * odometry into its pass-through (lio_po_set_enable_odom(po, 0), the /enable_odom call of Estimator.cc:542-560, made only on the
+ * RunInitialization success path: the imu_factor = 0 start-up, :505-517, leaves the odometry on).  It takes effect from the next sweep,
+ * exactly once; the reference's service call is asynchronous, so there the switch lands at a sweep that depends on thread timing.
+ * Refusals, before anything changes: a sweep the gate would publish while max_pending messages wait returns LIO_ERR_CAPACITY, n above
+ * max_points LIO_ERR_CAPACITY, rings on the wrong sensor type LIO_ERR_INVALID.  Inner failures return their status; an estimator failure
+ * poisons the node as it poisons the estimator: every later push returns LIO_ERR_INVALID.
+ * Waits: the odometry's one or two (lio_po_process_dev) and the estimator's per processed message; the node adds none to the device
+ * entry.  _dev is stream-ordered (the caller's buffers are read by work on the stream); _host uploads, runs the same and synchronises once. */
+int lio_node_push_sweep_dev(lio_node *node, const float *xyzi_dev, const uint16_t *rings_dev, int n, double stamp);
+int lio_node_push_sweep_host(lio_node *node, const float *xyzi, const uint16_t *rings, int n, double stamp);
+int lio_node_status(lio_node *node, lio_node_info *status);
+/* The inner handles, for the existing getters and _dev accessors (lio_est_get_states, lio_est_map_poses, lio_est_imu_init_status,
+ * lio_est_extrinsic_calib_status, lio_est_local_clouds_dev, lio_mb_surround_dev / lio_mb_full_dev for lio_rm_insert_dev, lio_pp_cloud_dev,
+ * ...).  Their process, set-up, attach and destroy entries must not be called: the node owns them.  Any pointer may be NULL. */
+int lio_node_handles(lio_node *node, lio_pp **pp, lio_po **po, lio_est **est, lio_pm **pm);
 
 /* ------------------------------------------------------------------------------------------
  * Dense fp64 kernels of the host shell (host only; test seams).

@@ -60,6 +60,20 @@ class PPConfig(C.Structure):
                 ("max_surf_flat", C.c_int), ("less_flat_filter_size", C.c_float)]
 
 
+class NodeConfig(C.Structure):
+    """lio_node_config (include/lio_b200.h): processor_node + estimator_node parameters."""
+    _fields_ = [("sensor_type", C.c_int), ("pp", PPConfig), ("odom_io", C.c_int), ("msg_time_delay", C.c_double), ("est", EstConfig),
+                ("tf_lb7", C.c_float * 7), ("corner_filter_size", C.c_float), ("surf_filter_size", C.c_float), ("map_filter_size", C.c_float),
+                ("max_points", C.c_int), ("max_feature_points", C.c_int), ("max_pending", C.c_int)]
+
+
+class NodeInfo(C.Structure):
+    """lio_node_info (include/lio_b200.h)."""
+    _fields_ = [("sweeps", C.c_longlong), ("published", C.c_longlong), ("processed", C.c_longlong), ("dropped", C.c_longlong),
+                ("imu_dropped", C.c_longlong), ("pending", C.c_int), ("odom_enabled", C.c_int), ("inited", C.c_int), ("poisoned", C.c_int),
+                ("last_stamp", C.c_double)]
+
+
 def lib():
     global _LIB
     if _LIB is not None:
@@ -231,6 +245,18 @@ def lib():
     L.lio_rm_reset.argtypes = [vp]
     L.lio_pcd_write_xyzi.argtypes = [C.c_char_p, f32p, ll]
     L.lio_rm_write_pcd.argtypes = [vp, C.c_char_p]
+    L.lio_pp_process_dev_ring.argtypes = [vp, vp, vp, ip]
+    L.lio_measure_replay.argtypes = [C.c_double, ip, i32p, f64p, f64p, f64p, f64p, ip, C.POINTER(ip), i32p, ip, C.POINTER(ip), C.POINTER(ip)]
+    L.lio_node_default_config.argtypes = [C.POINTER(NodeConfig)]
+    L.lio_node_default_config.restype = None
+    L.lio_node_create.argtypes = [C.POINTER(NodeConfig), ip, vp, C.POINTER(vp)]
+    L.lio_node_destroy.argtypes = [vp]
+    L.lio_node_push_imu.argtypes = [vp, C.c_double, f64p, f64p]
+    L.lio_node_push_imu_batch.argtypes = [vp, ip, f64p, f64p, f64p]
+    L.lio_node_push_sweep_dev.argtypes = [vp, vp, vp, ip, C.c_double]
+    L.lio_node_push_sweep_host.argtypes = [vp, f32p, vp, ip, C.c_double]
+    L.lio_node_status.argtypes = [vp, C.POINTER(NodeInfo)]
+    L.lio_node_handles.argtypes = [vp, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]
     _LIB = L
     return L
 

@@ -1,0 +1,306 @@
+// lio_node: the reference's test_*.launch graph - lio_processor_node (src/processor_node.cc) and lio_estimator_node
+// (src/estimator_node.cc: PointOdometry on its own thread, Estimator::ProcessEstimation on the measurement thread) - as one handle on
+// one stream.  Stage A, the odometry, the estimator and its attached PointMapping are the existing handles; this unit only restates
+// the glue between them: the /compact_data queue (the odometry's published clouds copied into HBM slots), MeasurementManager's
+// pairing and ProcessEstimation's IMU loop (measure.cc), and the /enable_odom call.  No kernel of its own: the slot copies are the
+// count-guarded copy_cloud of the estimator.
+#include <cmath>
+#include <cstring>
+#include <new>
+#include <vector>
+#include "estimator.cuh"
+#include "measure.h"
+
+namespace {
+
+struct Slot {                 // one published /compact_data message waiting for its IMU
+  float4 *cloud[3] = {};      // /laser_cloud_corner_last, /laser_cloud_surf_last, the full cloud
+  int *d_n = nullptr;         // their device counts
+  int n[3] = {};              // the same counts as the host knows them (the bounds handed on)
+  float sum7[7] = {};         // transform_sum_
+  double stamp = 0;           // header.stamp
+};
+
+}  // namespace
+
+struct lio_node {
+  lio_node_config cfg{};
+  int device = 0;
+  int sm_count = 132;
+  cudaStream_t stream = nullptr;
+  lio_pp *pp = nullptr;
+  lio_po *po = nullptr;
+  lio_pm *pm = nullptr;
+  lio_est *est = nullptr;
+  float4 *d_in = nullptr;              // upload target of lio_node_push_sweep_host
+  uint16_t *d_rings = nullptr;
+  std::vector<Slot> slots;
+  std::vector<int> free_slots;
+  lio::MeasurementPairing pairing{0};
+  std::vector<lio::ImuMsg> list;
+  std::vector<lio::ImuCall> calls;
+  long long po_calls = 0;              // successful odometry calls (the io_ratio gate follows from them)
+  long long sweeps = 0, published = 0, processed = 0, dropped = 0;
+  bool odom_on = true, inited = false, poisoned = false;
+  double last_stamp = -1;
+};
+
+static bool ring_sensor(const lio_node *nd) { return nd->cfg.sensor_type == 320; }
+
+// processor_node.cc:72-73: only the 320 preset reads the ring field (an empty sweep may come without it)
+static int check_rings(const lio_node *nd, bool has_rings, int n) {
+  if (ring_sensor(nd) ? (has_rings || n == 0) : !has_rings) return LIO_OK;
+  lio_set_last_error(__FILE__, __LINE__, "lio_node: rings are required with sensor_type 320 and refused otherwise");
+  return LIO_ERR_INVALID;
+}
+
+static void node_free(lio_node *nd) {
+  if (!nd) return;
+  cudaSetDevice(nd->device);
+  if (nd->est) lio_est_destroy(nd->est);   // releases the attached map first
+  if (nd->pm) lio_pm_destroy(nd->pm);
+  if (nd->po) lio_po_destroy(nd->po);
+  if (nd->pp) lio_pp_destroy(nd->pp);
+  for (Slot &s : nd->slots) {
+    for (float4 *c : s.cloud) if (c) cudaFree(c);
+    if (s.d_n) cudaFree(s.d_n);
+  }
+  if (nd->d_in) cudaFree(nd->d_in);
+  if (nd->d_rings) cudaFree(nd->d_rings);
+  delete nd;
+}
+
+extern "C" void lio_node_default_config(lio_node_config *c) {
+  if (!c) return;
+  std::memset(c, 0, sizeof(*c));
+  c->sensor_type = 16;
+  lio_pp_default_config(&c->pp);
+  c->odom_io = 2;                       // PointOdometry(scan_period, io_ratio = 2) default
+  c->msg_time_delay = 0;                // MeasurementManager.h:78
+  lio_est_default_config(&c->est);
+  c->tf_lb7[3] = 1.0f;
+  c->corner_filter_size = 0.2f;         // PointMapping leaves (config/*.yaml)
+  c->surf_filter_size = 0.4f;
+  c->map_filter_size = 0.6f;
+  c->max_points = 1 << 18;
+  c->max_feature_points = 1 << 16;
+  c->max_pending = 16;
+}
+
+extern "C" int lio_node_create(const lio_node_config *cfg, int device, void *cuda_stream, lio_node **out) {
+  if (!cfg || !out) return LIO_ERR_INVALID;
+  *out = nullptr;
+  const int st = cfg->sensor_type;
+  if ((st != 16 && st != 32 && st != 64 && st != 320) || cfg->odom_io < 1 || !(cfg->msg_time_delay >= 0) || cfg->max_points <= 0 ||
+      cfg->max_feature_points <= 0 || cfg->max_pending < 1 || !(cfg->map_filter_size > 0)) {
+    lio_set_last_error(__FILE__, __LINE__, "lio_node_create: sensor_type must be 16, 32, 64 or 320; odom_io, capacities and max_pending >= 1");
+    return LIO_ERR_INVALID;
+  }
+  if (lio_device_count() <= 0) return LIO_ERR_NO_DEVICE;
+  LIO_CUDA_OK(cudaSetDevice(device));
+  lio_node *nd = new (std::nothrow) lio_node();
+  if (!nd) return LIO_ERR_INVALID;
+  nd->cfg = *cfg;
+  nd->device = device;
+  nd->stream = (cudaStream_t)cuda_stream;
+  cudaDeviceGetAttribute(&nd->sm_count, cudaDevAttrMultiProcessorCount, device);
+  nd->pairing = lio::MeasurementPairing(cfg->msg_time_delay);
+  auto fail = [&](int rc) { node_free(nd); return rc; };
+  // processor_node.cc:64-74: the sensor presets (320 = RS-32 with the ring field)
+  lio_pp_config pc = cfg->pp;
+  if (st == 16) { pc.lower_bound = -15.f; pc.upper_bound = 15.f; pc.num_rings = 16; }
+  else if (st == 32) { pc.lower_bound = -30.67f; pc.upper_bound = 10.67f; pc.num_rings = 32; }
+  else if (st == 64) { pc.lower_bound = -24.9f; pc.upper_bound = 2.f; pc.num_rings = 64; }
+  else { pc.lower_bound = -25.f; pc.upper_bound = 15.f; pc.num_rings = 32; }
+  const int F = cfg->max_feature_points, N = cfg->max_points;
+  const lio_est_config &ec = cfg->est;
+  int rc;
+  if ((rc = lio_pp_create(&pc, N, device, cuda_stream, &nd->pp)) != LIO_OK) return fail(rc);
+  // estimator_node.cc:145-147: PointOdometry(0.1, odom_io) with its default 25 iterations
+  if ((rc = lio_po_create(0.1f, cfg->odom_io, 25, F, N, device, cuda_stream, &nd->po)) != LIO_OK) return fail(rc);
+  // the Estimator is a PointMapping (num_max_iterations_ 10, PointMapping.h:171) with the YAML's leaves
+  if ((rc = lio_pm_create(F, cfg->corner_filter_size, cfg->surf_filter_size, ec.min_match_sq_dis, ec.min_plane_dis, 10, device, cuda_stream,
+                          &nd->pm)) != LIO_OK)
+    return fail(rc);
+  if ((rc = lio_pm_enable_publish(nd->pm, cfg->map_filter_size, N)) != LIO_OK) return fail(rc);
+  if ((rc = lio_est_create(&ec, device, cuda_stream, &nd->est)) != LIO_OK) return fail(rc);
+  if ((rc = lio_est_set_extrinsic(nd->est, cfg->tf_lb7)) != LIO_OK) return fail(rc);
+  if ((rc = lio_est_enable_local_clouds(nd->est, cfg->corner_filter_size, F, N)) != LIO_OK) return fail(rc);
+  if (ec.imu_factor && ec.estimate_extrinsic == 2 && (rc = lio_est_enable_extrinsic_calibration(nd->est)) != LIO_OK) return fail(rc);
+  rc = ec.imu_factor ? lio_est_attach_imu_mapping(nd->est, nd->pm) : lio_est_attach_mapping(nd->est, nd->pm);
+  if (rc != LIO_OK) return fail(rc);
+  nd->slots.resize(cfg->max_pending);
+  for (int k = cfg->max_pending - 1; k >= 0; --k) {
+    Slot &s = nd->slots[k];
+    if (cudaMalloc(&s.cloud[0], sizeof(float4) * F) != cudaSuccess || cudaMalloc(&s.cloud[1], sizeof(float4) * F) != cudaSuccess ||
+        cudaMalloc(&s.cloud[2], sizeof(float4) * N) != cudaSuccess || cudaMalloc(&s.d_n, sizeof(int) * 3) != cudaSuccess) {
+      lio_set_last_error(__FILE__, __LINE__, "lio_node_create: cudaMalloc of a queue slot failed");
+      return fail(LIO_ERR_CUDA);
+    }
+    nd->free_slots.push_back(k);
+  }
+  *out = nd;
+  return LIO_OK;
+}
+
+extern "C" int lio_node_destroy(lio_node *nd) {
+  node_free(nd);
+  return LIO_OK;
+}
+
+// One released message: ProcessEstimation's ProcessImu calls, then ProcessCompactData on its slot (Estimator.cc:2682-2736), then the
+// /enable_odom call of the RunInitialization success path (:542-560).  Any failure poisons the node.
+static int process_message(lio_node *nd, const Slot &s) {
+  nd->calls.clear();
+  nd->pairing.integrate(s.stamp, nd->list, &nd->calls);
+  int rc = LIO_OK;
+  for (const lio::ImuCall &c : nd->calls)
+    if ((rc = lio_est_process_imu(nd->est, c.dt, c.acc, c.gyr, c.stamp)) != LIO_OK) break;
+  if (rc == LIO_OK) rc = lio_est_process_compact_stamped_dev(nd->est, (const float *)s.cloud[0], (const float *)s.cloud[1], (const float *)s.cloud[2],
+                                                            s.d_n, s.n, s.sum7, s.stamp);
+  int info[4] = {};
+  if (rc == LIO_OK) rc = lio_est_compact_status(nd->est, info);
+  if (rc != LIO_OK) { nd->poisoned = true; return rc; }
+  ++nd->processed;
+  nd->last_stamp = s.stamp;
+  const bool now_inited = info[0] != 0;
+  const lio_est_config &ec = nd->cfg.est;
+  if (ec.imu_factor && !nd->inited && now_inited && (ec.enable_deskew || ec.cutoff_deskew)) {
+    if ((rc = lio_po_set_enable_odom(nd->po, 0)) != LIO_OK) { nd->poisoned = true; return rc; }
+    nd->odom_on = false;
+  }
+  nd->inited = now_inited;
+  return LIO_OK;
+}
+
+// GetMeasurements until it waits: every message it releases is processed, every one it drops frees its slot.
+static int drain(lio_node *nd) {
+  for (;;) {
+    int id = -1;
+    double t = 0;
+    const lio::MeasurementPairing::Decision d = nd->pairing.next(&id, &t, &nd->list);
+    if (d == lio::MeasurementPairing::kWait) return LIO_OK;
+    nd->free_slots.push_back(id);
+    if (d == lio::MeasurementPairing::kDropped) { ++nd->dropped; continue; }
+    const int rc = process_message(nd, nd->slots[id]);
+    if (rc != LIO_OK) return rc;
+  }
+}
+
+static int refuse_poisoned(lio_node *nd) {
+  if (!nd->poisoned) return LIO_OK;
+  lio_set_last_error(__FILE__, __LINE__, "lio_node: an earlier estimator failure poisoned the node; destroy and re-create it");
+  return LIO_ERR_INVALID;
+}
+
+extern "C" int lio_node_push_imu_batch(lio_node *nd, int n, const double *stamp, const double *acc3, const double *gyr3) {
+  if (!nd || n < 0 || (n > 0 && (!stamp || !acc3 || !gyr3))) return LIO_ERR_INVALID;
+  int rc = refuse_poisoned(nd);
+  if (rc != LIO_OK) return rc;
+  LIO_CUDA_OK(cudaSetDevice(nd->device));
+  for (int k = 0; k < n; ++k) {
+    lio::ImuMsg m{stamp[k], {acc3[3 * k], acc3[3 * k + 1], acc3[3 * k + 2]}, {gyr3[3 * k], gyr3[3 * k + 1], gyr3[3 * k + 2]}};
+    if (nd->pairing.push_imu(m) && (rc = drain(nd)) != LIO_OK) return rc;
+  }
+  return LIO_OK;
+}
+
+extern "C" int lio_node_push_imu(lio_node *nd, double stamp, const double acc[3], const double gyr[3]) {
+  if (!acc || !gyr) return LIO_ERR_INVALID;
+  return lio_node_push_imu_batch(nd, 1, &stamp, acc, gyr);
+}
+
+extern "C" int lio_node_push_sweep_dev(lio_node *nd, const float *xyzi_dev, const uint16_t *rings_dev, int n, double stamp) {
+  if (!nd || n < 0 || (n > 0 && !xyzi_dev) || std::isnan(stamp)) return LIO_ERR_INVALID;
+  int rc = check_rings(nd, rings_dev != nullptr, n);
+  if (rc != LIO_OK) return rc;
+  if ((rc = refuse_poisoned(nd)) != LIO_OK) return rc;
+  if (rc != LIO_OK) return rc;
+  if (n > nd->cfg.max_points) return LIO_ERR_CAPACITY;
+  // the io_ratio gate of the coming odometry call (PointOdometry.cc:302-310, :725): the first call never publishes
+  const long long c = nd->po_calls;
+  const bool will_publish = c >= 1 && (nd->cfg.odom_io < 2 || c % nd->cfg.odom_io == 1);
+  if (will_publish && nd->free_slots.empty()) {
+    lio_set_last_error(__FILE__, __LINE__, "lio_node: the /compact_data queue is full (max_pending messages wait for IMU)");
+    return LIO_ERR_CAPACITY;
+  }
+  LIO_CUDA_OK(cudaSetDevice(nd->device));
+  rc = ring_sensor(nd) ? lio_pp_process_dev_ring(nd->pp, xyzi_dev, rings_dev, n) : lio_pp_process_dev(nd->pp, xyzi_dev, n);
+  if (rc != LIO_OK) return rc;
+  static const int which[5] = {LIO_PP_CORNER_SHARP, LIO_PP_CORNER_LESS_SHARP, LIO_PP_SURF_FLAT, LIO_PP_SURF_LESS_FLAT, LIO_PP_CLOUD_IN_RINGS};
+  const float *clouds[5];
+  const int *counts[5];
+  for (int k = 0; k < 5; ++k) {
+    if ((rc = lio_pp_cloud_dev(nd->pp, which[k], &clouds[k])) != LIO_OK) return rc;
+    if ((rc = lio_pp_cloud_count_dev(nd->pp, which[k], &counts[k])) != LIO_OK) return rc;
+  }
+  const int F = nd->cfg.max_feature_points;
+  const int n_max[5] = {F, F, F, F, nd->cfg.max_points};
+  float sum7[7], es7[7];
+  int info4[4];
+  if ((rc = lio_po_process_dev(nd->po, clouds, counts, n_max, sum7, es7, info4)) != LIO_OK) return rc;
+  ++nd->po_calls;
+  ++nd->sweeps;
+  if (info4[1]) {   // published (:727): copy the three clouds, transform_sum_ and the stamp into a queue slot
+    const float *ptr[3];
+    const int *n_dev;
+    int n_host[3];
+    if ((rc = lio_po_clouds_dev(nd->po, ptr, &n_dev, n_host)) != LIO_OK) return rc;
+    const int id = nd->free_slots.back();
+    nd->free_slots.pop_back();
+    Slot &s = nd->slots[id];
+    for (int w = 0; w < 3; ++w) {
+      copy_cloud(reinterpret_cast<const float4 *>(ptr[w]), n_dev + w, n_host[w], s.cloud[w], s.d_n + w, 2 * nd->sm_count, nd->stream);
+      s.n[w] = n_host[w];
+    }
+    LIO_CUDA_OK(cudaGetLastError());
+    std::memcpy(s.sum7, sum7, sizeof(sum7));
+    s.stamp = stamp;
+    nd->pairing.push_message(id, stamp);
+    ++nd->published;
+  }
+  return drain(nd);
+}
+
+extern "C" int lio_node_push_sweep_host(lio_node *nd, const float *xyzi, const uint16_t *rings, int n, double stamp) {
+  if (!nd || n < 0 || (n > 0 && !xyzi) || std::isnan(stamp)) return LIO_ERR_INVALID;
+  int rc = check_rings(nd, rings != nullptr, n);
+  if (rc != LIO_OK) return rc;
+  if ((rc = refuse_poisoned(nd)) != LIO_OK) return rc;
+  if (n > nd->cfg.max_points) return LIO_ERR_CAPACITY;
+  LIO_CUDA_OK(cudaSetDevice(nd->device));
+  if (!nd->d_in) LIO_CUDA_OK(cudaMalloc(&nd->d_in, sizeof(float4) * nd->cfg.max_points));
+  if (rings && !nd->d_rings) LIO_CUDA_OK(cudaMalloc(&nd->d_rings, sizeof(uint16_t) * nd->cfg.max_points));
+  if (n > 0) {
+    LIO_CUDA_OK(cudaMemcpyAsync(nd->d_in, xyzi, sizeof(float4) * n, cudaMemcpyHostToDevice, nd->stream));
+    if (rings) LIO_CUDA_OK(cudaMemcpyAsync(nd->d_rings, rings, sizeof(uint16_t) * n, cudaMemcpyHostToDevice, nd->stream));
+  }
+  rc = lio_node_push_sweep_dev(nd, (const float *)nd->d_in, rings ? nd->d_rings : nullptr, n, stamp);
+  const cudaError_t e = cudaStreamSynchronize(nd->stream);   // the caller's buffers may be reused on return
+  if (rc == LIO_OK && e != cudaSuccess) { lio_set_last_error(__FILE__, __LINE__, cudaGetErrorString(e)); return LIO_ERR_CUDA; }
+  return rc;
+}
+
+extern "C" int lio_node_status(lio_node *nd, lio_node_info *s) {
+  if (!nd || !s) return LIO_ERR_INVALID;
+  s->sweeps = nd->sweeps;
+  s->published = nd->published;
+  s->processed = nd->processed;
+  s->dropped = nd->dropped;
+  s->pending = nd->pairing.pending();
+  s->imu_dropped = nd->pairing.imu_dropped();
+  s->odom_enabled = nd->odom_on ? 1 : 0;
+  s->inited = nd->inited ? 1 : 0;
+  s->poisoned = nd->poisoned ? 1 : 0;
+  s->last_stamp = nd->last_stamp;
+  return LIO_OK;
+}
+
+extern "C" int lio_node_handles(lio_node *nd, lio_pp **pp, lio_po **po, lio_est **est, lio_pm **pm) {
+  if (!nd) return LIO_ERR_INVALID;
+  if (pp) *pp = nd->pp;
+  if (po) *po = nd->po;
+  if (est) *est = nd->est;
+  if (pm) *pm = nd->pm;
+  return LIO_OK;
+}

@@ -816,20 +816,17 @@ extern "C" int lio_pp_process_host(lio_pp *pp, const float *xyzi, int n) {
   return pp_sync_counts(pp);
 }
 
-// SetInputCloud(PointIR) + PointToRing (ring-field variant, PointProcessor.cc:428-536) + ExtractFeaturePoints; host buffers.
-extern "C" int lio_pp_process_host_ring(lio_pp *pp, const float *xyzi, const uint16_t *rings, int n) {
-  if (!pp || ((!xyzi || !rings) && n > 0) || n < 0) return LIO_ERR_INVALID;
+// PointToRing (ring-field variant, PointProcessor.cc:428-536) + ExtractFeaturePoints on device buffers; stream-ordered, no wait.
+extern "C" int lio_pp_process_dev_ring(lio_pp *pp, const float *xyzi_dev, const uint16_t *rings_dev, int n) {
+  if (!pp || ((!xyzi_dev || !rings_dev) && n > 0) || n < 0) return LIO_ERR_INVALID;
   if (n > pp->max_points) return LIO_ERR_CAPACITY;
   LIO_CUDA_OK(cudaSetDevice(pp->device));
-  if (!pp->d_rings_in) LIO_CUDA_OK(dalloc(&pp->d_rings_in, (size_t)pp->max_points));
   if (!pp->d_end_bits) LIO_CUDA_OK(dalloc(&pp->d_end_bits, 1));
   cudaStream_t st = pp->stream;
   const PPParams &P = pp->P;
   const int R = P.num_rings;
-  if (n > 0) {
-    LIO_CUDA_OK(cudaMemcpyAsync(pp->d_in, xyzi, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, st));
-    LIO_CUDA_OK(cudaMemcpyAsync(pp->d_rings_in, rings, (size_t)n * sizeof(uint16_t), cudaMemcpyHostToDevice, st));
-  }
+  const float4 *in = reinterpret_cast<const float4 *>(xyzi_dev);
+  const unsigned short *rings = reinterpret_cast<const unsigned short *>(rings_dev);
   pp->launches = 0;
   pp->last_n = n;
   pp->counts_valid = false;
@@ -837,10 +834,10 @@ extern "C" int lio_pp_process_host_ring(lio_pp *pp, const float *xyzi, const uin
   if (nb < 1) nb = 1;
   LIO_CUDA_OK(cudaMemsetAsync(pp->d_first_valid, 0x7f, sizeof(int), st));
   LIO_CUDA_OK(cudaMemsetAsync(pp->d_end_bits, 0, sizeof(int), st));   // end_ori_ = 0
-  a_classify_ring<<<nb, kClsThreads, 0, st>>>(pp->d_in, pp->d_rings_in, n, P, pp->d_ring_id, pp->d_azi, pp->d_first_valid, pp->d_hist);
+  a_classify_ring<<<nb, kClsThreads, 0, st>>>(in, rings, n, P, pp->d_ring_id, pp->d_azi, pp->d_first_valid, pp->d_hist);
   a_scan<<<1, kMaxRings, 0, st>>>(pp->d_hist, nb, R, pp->d_offsets, pp->d_ring_start);
   a_endori<<<std::min(nb, 132), 256, 0, st>>>(pp->d_azi, pp->d_ring_id, n, pp->d_first_valid, pp->d_end_bits);
-  a_scatter_ring<<<nb, kClsThreads, 0, st>>>(pp->d_in, n, P, pp->d_ring_id, pp->d_azi, pp->d_first_valid, pp->d_end_bits, pp->d_offsets,
+  a_scatter_ring<<<nb, kClsThreads, 0, st>>>(in, n, P, pp->d_ring_id, pp->d_azi, pp->d_first_valid, pp->d_end_bits, pp->d_offsets,
                                              pp->d_laser, pp->d_full, pp->d_orig, pp->d_start_ori);
   a_ring<<<R, kRingThreads, pp->ring_smem, st>>>(pp->d_laser, pp->d_ring_start, P, pp->d_start_ori, pp->d_mask, pp->d_label,
                                                  pp->d_pick_less, pp->d_n_less, pp->d_pick_flat, pp->d_n_flat, pp->d_lf_ring,
@@ -852,6 +849,21 @@ extern "C" int lio_pp_process_host_ring(lio_pp *pp, const float *xyzi, const uin
   LIO_CUDA_OK(cudaGetLastError());
   LIO_CUDA_OK(cudaMemcpyAsync(pp->h_counts, pp->d_counts, 5 * sizeof(int), cudaMemcpyDeviceToHost, st));
   LIO_CUDA_OK(cudaMemcpyAsync(pp->h_counts + 8, pp->d_err, sizeof(int), cudaMemcpyDeviceToHost, st));
+  return LIO_OK;
+}
+
+// SetInputCloud(PointIR) + the device entry above; host buffers, synchronous.
+extern "C" int lio_pp_process_host_ring(lio_pp *pp, const float *xyzi, const uint16_t *rings, int n) {
+  if (!pp || ((!xyzi || !rings) && n > 0) || n < 0) return LIO_ERR_INVALID;
+  if (n > pp->max_points) return LIO_ERR_CAPACITY;
+  LIO_CUDA_OK(cudaSetDevice(pp->device));
+  if (!pp->d_rings_in) LIO_CUDA_OK(dalloc(&pp->d_rings_in, (size_t)pp->max_points));
+  if (n > 0) {
+    LIO_CUDA_OK(cudaMemcpyAsync(pp->d_in, xyzi, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, pp->stream));
+    LIO_CUDA_OK(cudaMemcpyAsync(pp->d_rings_in, rings, (size_t)n * sizeof(uint16_t), cudaMemcpyHostToDevice, pp->stream));
+  }
+  int rc = lio_pp_process_dev_ring(pp, reinterpret_cast<const float *>(pp->d_in), reinterpret_cast<const uint16_t *>(pp->d_rings_in), n);
+  if (rc != LIO_OK) return rc;
   return pp_sync_counts(pp);
 }
 

@@ -1,0 +1,242 @@
+"""The reference's launch/test_*.launch graph - lio_processor_node + lio_estimator_node (src/processor_node.cc, src/estimator_node.cc) - as
+one device-resident handle over the C-ABI (lio_node_*): raw sweeps and IMU messages in; stage A, the odometry, MeasurementManager's pairing,
+the estimator's start-up and window solve, and its PointMapping inside the library.
+
+SHIPPED holds the three shipped configurations: config/indoor_test_config.yaml, config/outdoor_test_config.yaml and
+config/outdoor_test_config_64.yaml (the values below cite file:line), with the processor_node parameters of the launch file that starts
+each of them.  LioNode.shipped(name, ...) builds a node from one; the capacities and anything else can be given as keyword arguments."""
+from __future__ import annotations
+
+import ctypes as C
+
+import numpy as np
+
+from . import _lib, synth
+from .estimator import Estimator
+from .point_mapping import PointMapping
+from .point_odometry import PointOdometry
+from .point_processor import PointProcessor
+
+_I3 = [[1.0, 0.0, 0.0], [0.0, 1.0, 0.0], [0.0, 0.0, 1.0]]
+
+# Lines are the same in the two 70-line files (indoor_test_config.yaml, outdoor_test_config.yaml); outdoor_test_config_64.yaml has one line
+# more ("# KITTI 00", :23), so its lines from extrinsic_rotation on are one later.  min_plane_dis :3, min_match_sq_dis :5,
+# corner_filter_size :7, surf_filter_size :8, map_filter_size :9, window_size :12, opt_window_size :13, init_window_factor :15,
+# estimate_extrinsic :18, opt_extrinsic :21 in all three.
+SHIPPED = {
+    "indoor": dict(
+        yaml="config/indoor_test_config.yaml",
+        launch="launch/test_indoor.launch",       # sensor_type left at 16; launch/test_indoor_rs32.launch:6 runs the same YAML with 320
+        sensor_type=16, no_deskew=False,
+        min_plane_dis=0.2, min_match_sq_dis=1.0, corner_filter_size=0.2, surf_filter_size=0.4, map_filter_size=0.6,
+        window_size=12, opt_window_size=7, init_window_factor=2, estimate_extrinsic=2, opt_extrinsic=1,
+        extrinsic_rotation=_I3,                   # :23-30
+        extrinsic_translation=[0.0, 0.0, -0.081939],   # :32-36
+        imu_factor=1, point_distance_factor=1,    # :46, :47
+        prior_factor=0, marginalization_factor=1,  # :49, :51
+        odom_io=2,                                # :53
+        acc_n=0.2, gyr_n=0.02, acc_w=0.0002, gyr_w=2.0e-5, g_norm=9.805,   # :58-62
+        enable_deskew=1, cutoff_deskew=0,         # :65, :66
+        keep_features=1,                          # :68
+        msg_time_delay=0.05),                     # :70
+    "outdoor": dict(
+        yaml="config/outdoor_test_config.yaml",
+        launch="launch/test_outdoor.launch",      # sensor_type left at 16
+        sensor_type=16, no_deskew=False,
+        min_plane_dis=0.2, min_match_sq_dis=1.0, corner_filter_size=0.2, surf_filter_size=0.4, map_filter_size=0.6,
+        window_size=7, opt_window_size=5, init_window_factor=1, estimate_extrinsic=1, opt_extrinsic=1,
+        extrinsic_rotation=_I3,                   # :23-30
+        extrinsic_translation=[-2.4, 0.0, 0.7],   # :32-36
+        imu_factor=1, point_distance_factor=1,    # :46, :47
+        prior_factor=0, marginalization_factor=1,  # :49, :51
+        odom_io=3,                                # :53
+        acc_n=0.2, gyr_n=0.02, acc_w=0.0002, gyr_w=2.0e-5, g_norm=9.80,    # :58-62
+        enable_deskew=1, cutoff_deskew=0,         # :65, :66
+        keep_features=0,                          # :68
+        msg_time_delay=0.05),                     # :70
+    "outdoor_64": dict(
+        yaml="config/outdoor_test_config_64.yaml",
+        launch="launch/test_outdoor_64.launch",   # sensor_type 64 (:6); no_deskew true (:11), a parameter estimator_node.cc never reads
+        sensor_type=64, no_deskew=True,
+        min_plane_dis=0.2, min_match_sq_dis=1.0, corner_filter_size=0.2, surf_filter_size=0.4, map_filter_size=0.6,
+        window_size=7, opt_window_size=5, init_window_factor=1, estimate_extrinsic=1, opt_extrinsic=1,
+        extrinsic_rotation=[[9.999976e-01, 7.553071e-04, -2.035826e-03],     # :24-31 (KITTI 00)
+                            [-7.854027e-04, 9.998898e-01, -1.482298e-02],
+                            [2.024406e-03, 1.482454e-02, 9.998881e-01]],
+        extrinsic_translation=[-8.086759e-01, 3.195559e-01, -7.997231e-01],  # :33-37
+        imu_factor=1, point_distance_factor=1,    # :47, :48
+        prior_factor=1, marginalization_factor=1,  # :50, :52
+        odom_io=3,                                # :54
+        acc_n=0.2, gyr_n=0.02, acc_w=0.0002, gyr_w=2.0e-5, g_norm=9.80,    # :59-63
+        enable_deskew=1, cutoff_deskew=1,         # :66, :67
+        keep_features=0,                          # :69
+        msg_time_delay=0.0),                      # :71
+}
+
+_EST_KEYS = ("min_plane_dis", "min_match_sq_dis", "surf_filter_size", "window_size", "opt_window_size", "init_window_factor",
+             "estimate_extrinsic", "opt_extrinsic", "imu_factor", "point_distance_factor", "prior_factor", "marginalization_factor",
+             "acc_n", "gyr_n", "acc_w", "gyr_w", "g_norm", "enable_deskew", "cutoff_deskew", "keep_features")
+
+
+def shipped_tf_lb7(name):
+    """transform_lb_ of a shipped configuration as estimator_node.cc:90-97 builds it (Quaternionf of the float rotation), tf7."""
+    s = SHIPPED[name]
+    q = synth.rot_to_quat(np.array(s["extrinsic_rotation"], np.float32).astype(np.float64))
+    return np.array([*q, *s["extrinsic_translation"]], np.float32)
+
+
+class _Borrowed:
+    """A wrapper object over an inner handle of a node: its getters work, closing it does nothing (the node owns the handle)."""
+
+    def close(self):
+        pass
+
+
+class _EstimatorView(_Borrowed, Estimator):
+    def __init__(self, h, c):
+        self.h, self.c, self.W, self._cb = h, c, c.window_size, None
+        self.cfg = {name: getattr(c, name) for name, _ in c._fields_}
+
+
+class _MappingView(_Borrowed, PointMapping):
+    def __init__(self, h):
+        self.h = h
+
+
+class _OdometryView(_Borrowed, PointOdometry):
+    def __init__(self, h):
+        self.h = h
+
+
+class _ProcessorView(_Borrowed, PointProcessor):
+    def __init__(self, h, cfg):
+        self._h, self.cfg, self._cloud = h, cfg, None
+
+
+class LioNode:
+    """lio_node: push_imu / push_imu_batch and push_sweep (host arrays) / push_sweep_dev (device pointers) in any order the sensors deliver
+    them; every message that MeasurementManager's pairing releases is processed at once.  status() reports the counters; estimator,
+    mapping, odometry and processor are read-only views of the inner handles (their getters only: the node owns the handles)."""
+
+    def __init__(self, sensor_type=16, odom_io=2, msg_time_delay=0.0, tf_lb7=None, corner_filter_size=0.2, surf_filter_size=0.4,
+                 map_filter_size=0.6, max_points=1 << 18, max_feature_points=1 << 16, max_pending=16, pp=None, device=0, stream=0, **est):
+        L = _lib.lib()
+        _lib.require_device()
+        c = _lib.NodeConfig()
+        L.lio_node_default_config(C.byref(c))
+        c.sensor_type, c.odom_io, c.msg_time_delay = int(sensor_type), int(odom_io), float(msg_time_delay)
+        c.corner_filter_size, c.surf_filter_size, c.map_filter_size = corner_filter_size, surf_filter_size, map_filter_size
+        c.est.surf_filter_size = surf_filter_size   # one YAML key for the Estimator and the PointMapping it is
+        c.max_points, c.max_feature_points, c.max_pending = int(max_points), int(max_feature_points), int(max_pending)
+        if tf_lb7 is not None:
+            c.tf_lb7[:] = [float(v) for v in np.asarray(tf_lb7, np.float32)]
+        for k, v in (pp or {}).items():
+            if not hasattr(c.pp, k):
+                raise AttributeError(f"PointProcessorConfig has no field {k}")
+            setattr(c.pp, k, v)
+        for k, v in est.items():
+            if not hasattr(c.est, k):
+                raise AttributeError(f"EstimatorConfig has no field {k}")
+            setattr(c.est, k, v)
+        self.cfg = c
+        self.h = C.c_void_p()
+        _lib.check(L.lio_node_create(C.byref(c), device, C.c_void_p(stream), C.byref(self.h)), "lio_node_create")
+        pp_h, po_h, est_h, pm_h = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_void_p()
+        _lib.check(L.lio_node_handles(self.h, C.byref(pp_h), C.byref(po_h), C.byref(est_h), C.byref(pm_h)), "lio_node_handles")
+        self.estimator = _EstimatorView(est_h, c.est)
+        self.mapping = _MappingView(pm_h)
+        self.odometry = _OdometryView(po_h)
+        self.processor = _ProcessorView(pp_h, c.pp)
+
+    @classmethod
+    def shipped(cls, name, **overrides):
+        """A node with the values of SHIPPED[name]; keyword arguments (capacities, tf_lb7, any config field) take precedence."""
+        s = SHIPPED[name]
+        kw = dict(sensor_type=s["sensor_type"], odom_io=s["odom_io"], msg_time_delay=s["msg_time_delay"], tf_lb7=shipped_tf_lb7(name),
+                  corner_filter_size=s["corner_filter_size"], surf_filter_size=s["surf_filter_size"], map_filter_size=s["map_filter_size"])
+        kw.update({k: s[k] for k in _EST_KEYS if k != "surf_filter_size"})
+        kw.update(overrides)
+        return cls(**kw)
+
+    def close(self):
+        if getattr(self, "h", None):
+            _lib.lib().lio_node_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def push_imu(self, stamp, acc, gyr):
+        _lib.check(_lib.lib().lio_node_push_imu(self.h, float(stamp), np.ascontiguousarray(acc, np.float64),
+                                                np.ascontiguousarray(gyr, np.float64)), "lio_node_push_imu")
+
+    def push_imu_batch(self, stamps, acc, gyr):
+        """n IMU messages: stamps (n,), acc / gyr (n, 3)."""
+        t = np.ascontiguousarray(stamps, np.float64).reshape(-1)
+        a = np.ascontiguousarray(acc, np.float64).reshape(-1, 3)
+        g = np.ascontiguousarray(gyr, np.float64).reshape(-1, 3)
+        if a.shape[0] != t.shape[0] or g.shape[0] != t.shape[0]:
+            raise ValueError("one acc and one gyr row per stamp")
+        _lib.check(_lib.lib().lio_node_push_imu_batch(self.h, t.shape[0], t, a if t.shape[0] else np.zeros((1, 3)),
+                                                      g if t.shape[0] else np.zeros((1, 3))), "lio_node_push_imu_batch")
+
+    def push_sweep(self, xyzi, stamp, rings=None):
+        """One raw sweep from host arrays: (n, 4) float32 x y z intensity, optional (n,) ring ids (sensor_type 320 only)."""
+        x = np.ascontiguousarray(xyzi, np.float32).reshape(-1, 4)
+        r = None if rings is None else np.ascontiguousarray(rings, np.uint16).reshape(-1)
+        if r is not None and r.shape[0] != x.shape[0]:
+            raise ValueError("one ring index per point")
+        _lib.check(_lib.lib().lio_node_push_sweep_host(self.h, x if x.shape[0] else np.zeros((1, 4), np.float32),
+                                                       None if r is None else r.ctypes.data_as(C.c_void_p), x.shape[0], float(stamp)),
+                   "lio_node_push_sweep_host")
+
+    def push_sweep_dev(self, xyzi_ptr: int, n: int, stamp, rings_ptr: int | None = None):
+        """One raw sweep already in HBM (float4 array, optional uint16 ring array); stream-ordered on the node's stream."""
+        _lib.check(_lib.lib().lio_node_push_sweep_dev(self.h, C.c_void_p(xyzi_ptr), None if rings_ptr is None else C.c_void_p(rings_ptr),
+                                                      int(n), float(stamp)), "lio_node_push_sweep_dev")
+
+    def status(self):
+        s = _lib.NodeInfo()
+        _lib.check(_lib.lib().lio_node_status(self.h, C.byref(s)), "lio_node_status")
+        out = {name: getattr(s, name) for name, _ in s._fields_}
+        for k in ("odom_enabled", "inited", "poisoned"):
+            out[k] = bool(out[k])
+        return out
+
+    # ---- read-only views of the estimator
+    def states(self):
+        return self.estimator.states()
+
+    def map_poses(self):
+        return self.estimator.map_poses()
+
+    def imu_init_status(self):
+        return self.estimator.imu_init_status()
+
+    def extrinsic_calib_status(self):
+        return self.estimator.extrinsic_calib_status()
+
+    def extrinsic(self):
+        return self.estimator.extrinsic()
+
+
+def measure_replay(msg_time_delay, arrivals):
+    """The node's pairing on a replayed arrival sequence (lio_measure_replay; no device needed).  arrivals: list of ("imu", stamp, acc3,
+    gyr3) or ("msg", stamp).  Returns (calls (m, 8) float64 {dt, acc xyz, gyr xyz, stamp}, events [(arrival index, processed, first call)],
+    out-of-order IMU messages dropped)."""
+    n = len(arrivals)
+    kind = np.array([0 if a[0] == "imu" else 1 for a in arrivals] or [0], np.int32)
+    stamp = np.array([a[1] for a in arrivals] or [0.0], np.float64)
+    acc = np.zeros((max(n, 1), 3)); gyr = np.zeros((max(n, 1), 3))
+    for i, a in enumerate(arrivals):
+        if a[0] == "imu":
+            acc[i], gyr[i] = a[2], a[3]
+    cap = 2 * n + 2
+    calls = np.zeros((cap, 8)); ev = np.zeros((cap, 3), np.int32)
+    nc, ne, nd = C.c_int(), C.c_int(), C.c_int()
+    _lib.check(_lib.lib().lio_measure_replay(float(msg_time_delay), n, kind, stamp, acc, gyr, calls, cap, C.byref(nc), ev, cap,
+                                             C.byref(ne), C.byref(nd)), "lio_measure_replay")
+    return calls[:nc.value].copy(), [tuple(int(v) for v in e) for e in ev[:ne.value]], nd.value
