@@ -146,6 +146,21 @@ int lio_transform_to_end_host(float *cloud, int n, const float *tf7_es, float ti
 int lio_laser_odom_host(const float *map, int K, const float *surf, int M, float *tf7, float min_match_sq_dis,
                         float min_plane_dis, int keep_features, int max_iter, float *pts4, float *coef4, int32_t *src,
                         int *n_out, int *iters, int device);
+/* Test seam of the reductions under the 6-DoF Gauss-Newton step: the A^T A (36, row-major) / A^T b (6) that one production
+ * kernel stores for n features (pts4, coef4: n float4) at the transform tf7.  kernel 0..2 = k_odom_reduce in mode 0
+ * (CalculateLaserOdom), 1 (scan-to-map) or 2 (MapBuilder's rotation information matrix) on `blocks` CTAs (1..1024; 0 = the
+ * callers' grid max(1, min(SMs, ceil(n / 256)))); kernel 3 = the fused single-CTA k_odom_round (blocks 0 or 1) with no k-NN
+ * tiles to clear.  Synchronous. */
+int lio_odom_normal_equations_host(const float *pts4, const float *coef4, int n, const float *tf7, int kernel, int blocks,
+                                   double *AtA, double *AtB, int device);
+/* Test seam of the step itself (odom_solve_step): `rounds` steps of one chain from a cleared OdomState and the pose tf7
+ * (in/out).  Round r stores AtA[36 r..] / AtB[6 r..] and the match count n_feat[r], then one thread takes the step of
+ * variant 0 CalculateLaserOdom (first executed round analyses degeneracy, threshold 100, no match minimum), 1 PointMapping
+ * (loop index r, rounds under 50 matches skipped, threshold 100), 2 MapBuilder (as 1, left update) or 3 PointOdometry (loop
+ * index r, minimum 10, threshold 10); a finished chain (done) skips its rounds, as the callers' kernels do.  Optional outputs:
+ * tf_per_round (7 per round), state_out {degenerate, done, iter}, matP (36, row-major).  Synchronous. */
+int lio_odom_step_host(int rounds, const double *AtA, const double *AtB, const int *n_feat, int variant, double delta_r_abort,
+                       double delta_t_abort, float *tf7, float *tf_per_round, int *state_out, float *matP, int device);
 
 /* ---- lio::PointMapping with its rolling cube map resident in HBM (src/point_processor/PointMapping.cc) -------------------
  * The 21 x 21 x 11 cubes of 50 m (:77-82, :121-122) hold their corner / surf clouds as HBM segments; the cube directory

@@ -149,6 +149,8 @@ def lib():
     L.lio_transform_to_end_host.argtypes = [f32p, ip, f32p, C.c_float, ip]
     L.lio_laser_odom_host.argtypes = [f32p, ip, f32p, ip, f32p, C.c_float, C.c_float, ip, ip, f32p, f32p, i32p,
                                       C.POINTER(ip), C.POINTER(ip), ip]
+    L.lio_odom_normal_equations_host.argtypes = [f32p, f32p, ip, f32p, ip, ip, f64p, f64p, ip]
+    L.lio_odom_step_host.argtypes = [ip, f64p, f64p, i32p, ip, C.c_double, C.c_double, f32p, f32p, i32p, f32p, ip]
     L.lio_pp_cloud_count_dev.argtypes = [vp, ip, C.POINTER(vp)]
     L.lio_ppp_evaluate.argtypes = [f64p, f64p, f64p, f64p, f64p, f64p, f64p, f64p, f64p]
     L.lio_ppp_evaluate_batch_host.argtypes = [f32p, f32p, ip, f64p, f64p, f64p, f64p, f64p, ip]

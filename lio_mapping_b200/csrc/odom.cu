@@ -251,7 +251,7 @@ int scan_to_map_run(ScanToMapWork &W, const float4 *d_cmap, int Kc, const float4
                                   &W.d_odom->done, W.w, st, nullptr, 2, W.d_z);
     if (rc != LIO_OK) break;
     k_odom_reduce<<<nb, kOdomThreads, 0, st>>>(W.fo.pts, W.fo.coef, W.fo.count, W.d_tf, W.d_odom, W.d_partial, variant == 1 ? 2 : 1);
-    k_odom_solve<<<1, 32, 0, st>>>(W.d_odom, W.d_tf, delta_r_abort, delta_t_abort, it, W.fo.count, 50, variant == 1 ? 1 : 0);
+    k_odom_solve<<<1, 32, 0, st>>>(W.d_odom, W.d_tf, delta_r_abort, delta_t_abort, it, W.fo.count, kScanToMapMinFeatures, variant == 1 ? 1 : 0);
   }
   if (rc != LIO_OK) return rc;
   int m = 0;
@@ -360,4 +360,77 @@ extern "C" int lio_laser_odom_host(const float *map, int K, const float *surf, i
   h.destroy();
   w.destroy();
   return rc;
+}
+
+// ---- C-ABI: test seams of the 6-DoF Gauss-Newton step --------------------------------------------------------------
+// The normal equations of n explicit features as one of the production reductions leaves them in OdomState.
+extern "C" int lio_odom_normal_equations_host(const float *pts4, const float *coef4, int n, const float *tf7, int kernel, int blocks,
+                                              double *AtA, double *AtB, int device) {
+  constexpr int kMaxBlocks = 1024;
+  if ((n > 0 && (!pts4 || !coef4)) || !tf7 || !AtA || !AtB || n < 0 || kernel < 0 || kernel > 3 || blocks < 0 || blocks > kMaxBlocks ||
+      (kernel == 3 && blocks > 1))
+    return LIO_ERR_INVALID;
+  if (lio_device_count() <= 0) return LIO_ERR_NO_DEVICE;
+  LIO_CUDA_OK(cudaSetDevice(device));
+  int sm = 132;
+  cudaDeviceGetAttribute(&sm, cudaDevAttrMultiProcessorCount, device);
+  DevBufs d;
+  float4 *d_pts = nullptr, *d_coef = nullptr;
+  int *d_n = nullptr;
+  TransformF *d_tf = nullptr;
+  OdomState *d_odom = nullptr;
+  double *d_partial = nullptr;
+  unsigned long long *d_status = nullptr;
+  if (!d.alloc(&d_pts, n) || !d.alloc(&d_coef, n) || !d.alloc(&d_n, 2) || !d.alloc(&d_tf, 1) || !d.alloc(&d_odom, 1) ||
+      !d.alloc(&d_partial, 32 * kMaxBlocks) || !d.alloc(&d_status, 1) || !d.up(d_pts, (const float4 *)pts4, n) ||
+      !d.up(d_coef, (const float4 *)coef4, n) || !d.up(d_n, &n, 1) || !d.up(d_tf, (const TransformF *)tf7, 1) ||
+      !d.ok(cudaMemset(d_odom, 0, sizeof(OdomState))))
+    return LIO_ERR_CUDA;
+  if (kernel < 3) {
+    const int nb = blocks ? blocks : std::max(1, std::min(sm, (n + kOdomThreads - 1) / kOdomThreads));
+    k_odom_reduce<<<nb, kOdomThreads>>>(d_pts, d_coef, d_n, d_tf, d_odom, d_partial, kernel);
+  } else {
+    k_odom_round<<<1, kOdomRoundThreads>>>(d_pts, d_coef, d_n, d_tf, d_odom, 0.05, 0.05, d_status, 0, d_n + 1);
+  }
+  OdomState hs;
+  if (!d.ok(cudaGetLastError()) || !d.down(&hs, d_odom, 1)) return LIO_ERR_CUDA;
+  for (int k = 0; k < 36; ++k) AtA[k] = hs.AtA[k];
+  for (int k = 0; k < 6; ++k) AtB[k] = hs.AtB[k];
+  return LIO_OK;
+}
+
+// variant 0 CalculateLaserOdom, 1 PointMapping, 2 MapBuilder (left update), 3 PointOdometry, with the parameters of their loops
+__global__ void k_odom_step_variant(OdomState *__restrict__ st, TransformF *__restrict__ tf_dev, double delta_r_abort, double delta_t_abort,
+                                    int variant, int round, const int *__restrict__ n_dev) {
+  if (threadIdx.x != 0 || st->done) return;
+  if (variant == 0) odom_solve_step(st, tf_dev, delta_r_abort, delta_t_abort);
+  else if (variant == 1) odom_solve_step(st, tf_dev, delta_r_abort, delta_t_abort, round, n_dev, kScanToMapMinFeatures, 0);
+  else if (variant == 2) odom_solve_step(st, tf_dev, delta_r_abort, delta_t_abort, round, n_dev, kScanToMapMinFeatures, 1);
+  else odom_solve_step(st, tf_dev, delta_r_abort, delta_t_abort, round, n_dev, kPoMinFeatures, 0, kPoEigThre);
+}
+
+// `rounds` steps of one chain from a cleared OdomState: round r stores AtA[36 r..], AtB[6 r..] and n_feat[r] and takes the step.
+extern "C" int lio_odom_step_host(int rounds, const double *AtA, const double *AtB, const int *n_feat, int variant, double delta_r_abort,
+                                  double delta_t_abort, float *tf7, float *tf_per_round, int *state_out, float *matP, int device) {
+  if (rounds < 0 || (rounds > 0 && (!AtA || !AtB || !n_feat)) || !tf7 || variant < 0 || variant > 3) return LIO_ERR_INVALID;
+  if (lio_device_count() <= 0) return LIO_ERR_NO_DEVICE;
+  LIO_CUDA_OK(cudaSetDevice(device));
+  DevBufs d;
+  TransformF *d_tf = nullptr;
+  OdomState *d_odom = nullptr;
+  int *d_n = nullptr;
+  if (!d.alloc(&d_tf, 1) || !d.alloc(&d_odom, 1) || !d.alloc(&d_n, 1) || !d.up(d_tf, (const TransformF *)tf7, 1) ||
+      !d.ok(cudaMemset(d_odom, 0, sizeof(OdomState))))
+    return LIO_ERR_CUDA;
+  for (int r = 0; r < rounds; ++r) {
+    if (!d.up(d_odom->AtA, AtA + 36 * r, 36) || !d.up(d_odom->AtB, AtB + 6 * r, 6) || !d.up(d_n, n_feat + r, 1)) return LIO_ERR_CUDA;
+    k_odom_step_variant<<<1, 1>>>(d_odom, d_tf, delta_r_abort, delta_t_abort, variant, r, d_n);
+    if (!d.ok(cudaGetLastError())) return LIO_ERR_CUDA;
+    if (tf_per_round && !d.down((TransformF *)(tf_per_round + 7 * r), d_tf, 1)) return LIO_ERR_CUDA;
+  }
+  OdomState hs;
+  if (!d.down(&hs, d_odom, 1) || !d.down((TransformF *)tf7, d_tf, 1)) return LIO_ERR_CUDA;
+  if (state_out) { state_out[0] = hs.degenerate; state_out[1] = hs.done; state_out[2] = hs.iter; }
+  if (matP) for (int k = 0; k < 36; ++k) matP[k] = hs.matP[k];
+  return LIO_OK;
 }

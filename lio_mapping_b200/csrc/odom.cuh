@@ -139,12 +139,21 @@ __device__ __forceinline__ void sym_eigen6(const float *Ain, float *evals, float
   }
 }
 
+// Parameters of the loops that share odom_solve_step: the eigenvalue below which a leading direction of the first round's
+// A^T A is degenerate (Estimator.cc:1320, PointMapping.cc:662, MapBuilder.cc:942; PointOdometry.cc:596) and the match count
+// below which a round is skipped (PointMapping.cc:610, MapBuilder.cc:874; PointOdometry.cc:535).  CalculateLaserOdom has no
+// match minimum.
+constexpr float kOdomEigThre = 100.f;
+constexpr int kScanToMapMinFeatures = 50;
+constexpr float kPoEigThre = 10.f;
+constexpr int kPoMinFeatures = 10;
+
 // round < 0: CalculateLaserOdom (the first executed round carries the degeneracy analysis);  round >= 0: scan-to-map loop
 // index of PointMapping::OptimizeTransformTobeMapped, where a round with fewer than min_features matches is skipped
 // entirely (`continue`, PointMapping.cc:609-611) and the degeneracy analysis belongs to loop index 0 only.
 __device__ inline void odom_solve_step(OdomState *__restrict__ st, TransformF *__restrict__ tf_dev, double delta_r_abort, double delta_t_abort,
                                 int round = -1, const int *__restrict__ n_dev = nullptr, int min_features = 0, int left_update = 0,
-                                float eig_thre = 100.f) {
+                                float eig_thre = kOdomEigThre) {
   if (n_dev && *n_dev < min_features) { st->iter += 1; return; }
   const bool first_round = round < 0 ? (st->iter == 0) : (round == 0);
   float A[6][6], B[6], X[6], AtA[36];

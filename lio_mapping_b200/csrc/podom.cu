@@ -292,7 +292,7 @@ po_round(const float4 *__restrict__ sharp, int ns, const float4 *__restrict__ fl
       for (int c = a; c < 6; ++c) { st->AtA[a * 6 + c] = s_red[0][k]; st->AtA[c * 6 + a] = s_red[0][k]; ++k; }
     for (int a = 0; a < 6; ++a) st->AtB[a] = s_red[0][21 + a];
     *nsel_out = (int)s_red[0][27];
-    odom_solve_step(st, tf_dev, 0.1, 0.1, iter, nsel_out, 10, 0, 10.f);   // num_point_sel < 10 -> continue; abort 0.1 deg / 0.1 cm
+    odom_solve_step(st, tf_dev, 0.1, 0.1, iter, nsel_out, kPoMinFeatures, 0, kPoEigThre);   // abort 0.1 deg / 0.1 cm
   }
 }
 

@@ -132,7 +132,8 @@ __device__ __forceinline__ void colpiv_qr_solve(float (&a)[R][C], float (&b)[R],
       float s = b[i];
 #pragma unroll
       for (int j = i + 1; j < size; ++j) if (j < nonzero_pivots) s -= a[i][j] * b[j];
-      b[i] = s / a[i][i];
+      // Eigen's triangular solve divides only a nonzero right-hand side: a zero pivot under a zero rhs leaves 0, not 0 / 0
+      b[i] = (s != 0.f) ? s / a[i][i] : s;
     }
   }
 #pragma unroll

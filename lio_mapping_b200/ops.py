@@ -178,3 +178,34 @@ def scan_to_map(corner_map, surf_map, corner, surf, tf7, min_match_sq_dis=1.0, m
                                                tf, min_match_sq_dis, min_plane_dis, max_iter, delta_r_abort, delta_t_abort, variant, pts, coef, src,
                                                C.byref(n), C.byref(it), device), "lio_scan_to_map_host")
     return tf, pts[:n.value].copy(), coef[:n.value].copy(), src[:n.value].copy(), it.value
+
+
+def odom_normal_equations(pts, coef, tf7, kernel: int, blocks: int = 0, device: int = 0):
+    """A^T A (6 x 6) and A^T b (6) of the features as one production reduction stores them (lio_odom_normal_equations_host):
+    kernel 0..2 = k_odom_reduce mode 0..2 on `blocks` CTAs (0 = the callers' grid), 3 = the fused single-CTA k_odom_round."""
+    _lib.require_device()
+    p = np.ascontiguousarray(pts, np.float32).reshape(-1, 4)
+    c = np.ascontiguousarray(coef, np.float32).reshape(-1, 4)
+    pad = [x if x.shape[0] else np.zeros((1, 4), np.float32) for x in (p, c)]
+    AtA, AtB = np.zeros(36), np.zeros(6)
+    _lib.check(_lib.lib().lio_odom_normal_equations_host(pad[0], pad[1], p.shape[0], np.ascontiguousarray(tf7, np.float32), kernel, blocks,
+                                                         AtA, AtB, device), "lio_odom_normal_equations_host")
+    return AtA.reshape(6, 6), AtB
+
+
+def odom_step(AtA, AtB, n_feat, tf7, variant: int, delta_r_abort=0.05, delta_t_abort=0.05, device: int = 0):
+    """One chain of odom_solve_step rounds on given normal equations (lio_odom_step_host; variant 0 CalculateLaserOdom,
+    1 PointMapping, 2 MapBuilder, 3 PointOdometry).  Returns (tf7, tf7 after each round, {degenerate, done, iter}, matP)."""
+    _lib.require_device()
+    A = np.ascontiguousarray(AtA, np.float64).reshape(-1, 36)
+    rounds = A.shape[0]
+    b = np.ascontiguousarray(AtB, np.float64).reshape(rounds, 6)
+    n = np.ascontiguousarray(n_feat, np.int32).reshape(rounds)
+    tf = np.ascontiguousarray(tf7, np.float32).copy()
+    per = np.zeros((max(rounds, 1), 7), np.float32)
+    st = np.zeros(3, np.int32)
+    matP = np.zeros(36, np.float32)
+    pad = [x if rounds else np.zeros(k, x.dtype) for x, k in ((A, 36), (b, 6), (n, 1))]
+    _lib.check(_lib.lib().lio_odom_step_host(rounds, pad[0], pad[1], pad[2], variant, delta_r_abort, delta_t_abort, tf, per, st, matP, device),
+               "lio_odom_step_host")
+    return tf, per[:rounds].copy(), dict(degenerate=int(st[0]), done=int(st[1]), iter=int(st[2])), matP.reshape(6, 6)

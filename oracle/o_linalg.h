@@ -430,7 +430,7 @@ inline void colpiv_householder_qr_solve(T a[R][C], T b[R], T x[C]) {
   for (int i = nonzero_pivots - 1; i >= 0; --i) {
     T s = b[i];
     for (int j = i + 1; j < nonzero_pivots; ++j) s -= a[i][j] * b[j];
-    b[i] = s / a[i][i];
+    b[i] = (s != T(0)) ? s / a[i][i] : s;  // Eigen divides only a nonzero rhs (triangular_solve_vector)
   }
   for (int k = 0; k < C; ++k) x[k] = 0;
   for (int i = 0; i < nonzero_pivots; ++i) x[perm[i]] = b[i];
