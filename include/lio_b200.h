@@ -932,6 +932,52 @@ int lio_node_status(lio_node *node, lio_node_info *status);
  * ...).  Their process, set-up, attach and destroy entries must not be called: the node owns them.  Any pointer may be NULL. */
 int lio_node_handles(lio_node *node, lio_pp **pp, lio_po **po, lio_est **est, lio_pm **pm);
 
+/* ---- map_4D.launch / map_4D_indoor.launch beside the node: map_builder_node (src/map_builder_node.cc) on the estimator's /local
+ * clouds, and save_bag_to_pcd (src/save_bag_to_pcd.cc) on a /cloud_registered topic.
+ *   lio_node_enable_map_builder     creates an lio_mb handle (lio_mb_create with cfg; lio_mb_default_config holds the values of both
+ *                                   launch files: compact_data false, enable_4d true, map_filter_size 0.2 from map_builder_node.cc) on the
+ *                                   node's device and stream, sized from lio_est_local_clouds_dev's capacities: max_points = max(corner,
+ *                                   surf), max_full_points = full.  Only once and only before the first sweep; otherwise LIO_ERR_INVALID
+ *                                   and nothing changes.  A refusal of lio_mb_create is returned as its status.
+ *   which messages                  map_builder_node runs ProcessMap when HasNewData() (PointMapping.cc:291-297) sees its four topics new
+ *                                   with stamps within 5 ms.  The three clouds are published by SolveOptimization (Estimator.cc:2355-2375,
+ *                                   stamp Headers_[pivot+1]); /local_laser_odom only in the INITED branch of ProcessLaserOdom (:725-742,
+ *                                   the same stamp: SlideWindow does not move Headers_, :441 / :2650).  The start-up solve (:575 with
+ *                                   imu_factor = 1, :505-517 with imu_factor = 0) publishes clouds without /local_laser_odom, and the next
+ *                                   message's clouds replace them.  So the map builder runs once for every message that reaches the
+ *                                   estimator already INITED: after that message's successful estimator call, lio_est_local_clouds_dev and
+ *                                   lio_est_local_laser_odom go to lio_mb_process_map_dev on the node's stream; then its pose row is kept.
+ *                                   The reference's map builder is a separate process whose subscriber queues hold 2 messages, so under
+ *                                   load it can skip sets, depending on thread timing; the node processes every set, in order, on its
+ *                                   one stream.  The call adds the map builder's own host waits (lio_mb_process_map_dev) to the message.
+ *                                   A map builder failure poisons the node as an estimator failure does; note that lio_mb_process_map_dev
+ *                                   can return LIO_ERR_CAPACITY after it has advanced the handle's pose.
+ *   lio_node_map_builder            the lio_mb handle, for lio_pm_map_centre, the cube accessors, lio_mb_surround_* and lio_mb_full_*.
+ *                                   Its process and destroy entries must not be called (as for lio_node_handles).  LIO_ERR_INVALID
+ *                                   without a map builder.
+ *   lio_node_map_builder_poses      the drive's 4-D trajectory, one row per map builder call in call order: stamp = the set's header stamp
+ *                                   (Headers_[pivot+1]: the message pushed O - 1 pushes before the newest), tobe7 = transform_tobe_mapped_,
+ *                                   aft7 = transform_aft_mapped_ (/aft_mapped_to_init of PublishMapBuilderResults, MapBuilder.cc:186-200),
+ *                                   info6 as lio_mb_process_map_*.  Kept on the host.  *n = the number of rows; LIO_ERR_CAPACITY and
+ *                                   nothing copied when it exceeds cap.  Any array may be NULL.  LIO_ERR_INVALID without a map builder.
+ *   lio_node_attach_registered_map  every cloud that source publishes is inserted into rm with lio_rm_insert_dev, stream-ordered (no host
+ *                                   wait), in publication order.  LIO_NODE_MAP_ESTIMATOR: the estimator's PointMapping /cloud_registered,
+ *                                   save_bag_to_pcd's default topic (:66).  It publishes once per processed message: PointMapping::Process
+ *                                   publishes on the messages that arrive NOT INITED (the start-up message included: Process runs before
+ *                                   SetInitFlag, :544, and the start-up solve runs no PublishResults), PublishResults (:721) on the messages
+ *                                   that arrive INITED (Process skips it there, PointMapping.cc:1033, or is not run, :810-812).
+ *                                   LIO_NODE_MAP_BUILDER: the map builder's cloud_registered (MapBuilder.cc:113, :178-185), once per map
+ *                                   builder call; it needs lio_node_enable_map_builder first.  rm must be on the node's device and stream,
+ *                                   attached once, and must outlive the node (there is no detach).  A full map sets rm's sticky overflow
+ *                                   flag and does not fail the node.  Refusals (an unknown source, the map builder's source without a map
+ *                                   builder, another device or stream, an rm attached already, a poisoned node) return LIO_ERR_INVALID and
+ *                                   change nothing. */
+enum { LIO_NODE_MAP_ESTIMATOR = 0, LIO_NODE_MAP_BUILDER = 1 };
+int lio_node_enable_map_builder(lio_node *node, const lio_mb_config *cfg);
+int lio_node_map_builder(lio_node *node, lio_pm **mb);
+int lio_node_map_builder_poses(lio_node *node, double *stamp, float *tobe7, float *aft7, int *info6, int cap, int *n);
+int lio_node_attach_registered_map(lio_node *node, lio_rm *rm, int source);
+
 /* ------------------------------------------------------------------------------------------
  * Dense fp64 kernels of the host shell (host only; test seams).
  * ---------------------------------------------------------------------------------------- */

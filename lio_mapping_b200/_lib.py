@@ -259,6 +259,10 @@ def lib():
     L.lio_node_push_sweep_host.argtypes = [vp, f32p, vp, ip, C.c_double]
     L.lio_node_status.argtypes = [vp, C.POINTER(NodeInfo)]
     L.lio_node_handles.argtypes = [vp, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]
+    L.lio_node_enable_map_builder.argtypes = [vp, C.POINTER(MBConfig)]
+    L.lio_node_map_builder.argtypes = [vp, C.POINTER(vp)]
+    L.lio_node_map_builder_poses.argtypes = [vp, f64p, f32p, f32p, i32p, ip, C.POINTER(ip)]
+    L.lio_node_attach_registered_map.argtypes = [vp, vp, ip]
     _LIB = L
     return L
 

@@ -3,13 +3,18 @@
 // one stream.  Stage A, the odometry, the estimator and its attached PointMapping are the existing handles; this unit only restates
 // the glue between them: the /compact_data queue (the odometry's published clouds copied into HBM slots), MeasurementManager's
 // pairing and ProcessEstimation's IMU loop (measure.cc), and the /enable_odom call.  No kernel of its own: the slot copies are the
-// count-guarded copy_cloud of the estimator.
+// count-guarded copy_cloud of the estimator.  Optionally it also runs map_4D*.launch's map_builder_node on the estimator's /local/*
+// clouds (lio_node_enable_map_builder) and feeds drive maps (lio_node_attach_registered_map): the map builder's kernels and
+// lio_rm_insert_dev, enqueued on the same stream.
+#include <algorithm>
 #include <cmath>
 #include <cstring>
+#include <deque>
 #include <new>
 #include <vector>
 #include "estimator.cuh"
 #include "measure.h"
+#include "regmap.cuh"
 
 namespace {
 
@@ -19,6 +24,17 @@ struct Slot {                 // one published /compact_data message waiting for
   int n[3] = {};              // the same counts as the host knows them (the bounds handed on)
   float sum7[7] = {};         // transform_sum_
   double stamp = 0;           // header.stamp
+};
+
+struct MbRow {                // one map builder call: the set's stamp, transform_tobe_mapped_, transform_aft_mapped_, info6
+  double stamp;
+  float tobe7[7], aft7[7];
+  int info6[6];
+};
+
+struct DriveMap {             // an attached lio_rm and the /cloud_registered it takes
+  lio_rm *rm;
+  int source;
 };
 
 }  // namespace
@@ -43,6 +59,10 @@ struct lio_node {
   long long sweeps = 0, published = 0, processed = 0, dropped = 0;
   bool odom_on = true, inited = false, poisoned = false;
   double last_stamp = -1;
+  std::deque<double> headers;          // Headers_ (Estimator.cc:441): the stamps of the last W + 1 pushed messages
+  lio_pm *mb = nullptr;                // lio_node_enable_map_builder
+  std::vector<MbRow> mb_rows;
+  std::vector<DriveMap> maps;          // lio_node_attach_registered_map, in attach order
 };
 
 static bool ring_sensor(const lio_node *nd) { return nd->cfg.sensor_type == 320; }
@@ -57,6 +77,7 @@ static int check_rings(const lio_node *nd, bool has_rings, int n) {
 static void node_free(lio_node *nd) {
   if (!nd) return;
   cudaSetDevice(nd->device);
+  if (nd->mb) lio_pm_destroy(nd->mb);
   if (nd->est) lio_est_destroy(nd->est);   // releases the attached map first
   if (nd->pm) lio_pm_destroy(nd->pm);
   if (nd->po) lio_po_destroy(nd->po);
@@ -148,12 +169,45 @@ extern "C" int lio_node_destroy(lio_node *nd) {
   return LIO_OK;
 }
 
+// map_builder_node on the set the estimator has just published (INITED messages only, see lio_node_enable_map_builder): its /local/*
+// clouds and /local_laser_odom as they lie in HBM, on the node's stream; then the pose row.
+static int map_builder_step(lio_node *nd) {
+  const float *ptr[3];
+  const int *n_dev = nullptr;
+  int n_host[3];
+  MbRow row{};
+  int rc = lio_est_local_clouds_dev(nd->est, ptr, &n_dev, n_host);
+  float sum7[7];
+  if (rc == LIO_OK) rc = lio_est_local_laser_odom(nd->est, sum7);
+  if (rc == LIO_OK) rc = lio_mb_process_map_dev(nd->mb, ptr[0], ptr[1], ptr[2], n_dev, n_host, sum7, row.tobe7, row.aft7, row.info6);
+  if (rc != LIO_OK) return rc;
+  // Headers_[pivot_idx + 1] (Estimator.cc:727, :2364), the stamp of both the clouds and /local_laser_odom: Headers_ is full (W + 1)
+  // once INITED, so this is the message pushed O - 1 pushes before the newest
+  row.stamp = nd->headers[nd->headers.size() - nd->cfg.est.opt_window_size];
+  nd->mb_rows.push_back(row);
+  return LIO_OK;
+}
+
+// save_bag_to_pcd on the attached maps: the registered cloud of every publication of their source, stream-ordered, no host wait.
+static int insert_registered(lio_node *nd, int source) {
+  const float *p = nullptr;
+  int n = 0, rc = LIO_OK;
+  for (const DriveMap &d : nd->maps) {
+    if (d.source != source) continue;
+    if (!p && (rc = lio_mb_full_dev(source == LIO_NODE_MAP_ESTIMATOR ? nd->pm : nd->mb, &p, &n)) != LIO_OK) return rc;
+    if ((rc = lio_rm_insert_dev(d.rm, p, n)) != LIO_OK) return rc;
+  }
+  return LIO_OK;
+}
+
 // One released message: ProcessEstimation's ProcessImu calls, then ProcessCompactData on its slot (Estimator.cc:2682-2736), then the
-// /enable_odom call of the RunInitialization success path (:542-560).  Any failure poisons the node.
+// /enable_odom call of the RunInitialization success path (:542-560); with a map builder, its call when the message arrived INITED;
+// then the drive-map inserts.  Any failure poisons the node.
 static int process_message(lio_node *nd, const Slot &s) {
   nd->calls.clear();
   nd->pairing.integrate(s.stamp, nd->list, &nd->calls);
   int rc = LIO_OK;
+  const bool was_inited = nd->inited;
   for (const lio::ImuCall &c : nd->calls)
     if ((rc = lio_est_process_imu(nd->est, c.dt, c.acc, c.gyr, c.stamp)) != LIO_OK) break;
   if (rc == LIO_OK) rc = lio_est_process_compact_stamped_dev(nd->est, (const float *)s.cloud[0], (const float *)s.cloud[1], (const float *)s.cloud[2],
@@ -163,6 +217,10 @@ static int process_message(lio_node *nd, const Slot &s) {
   if (rc != LIO_OK) { nd->poisoned = true; return rc; }
   ++nd->processed;
   nd->last_stamp = s.stamp;
+  if (info[2]) {   // the message passed the init_window_factor gate (:436-439) and was pushed: Headers_.push(header) (:441)
+    nd->headers.push_back(s.stamp);
+    if ((int)nd->headers.size() > nd->cfg.est.window_size + 1) nd->headers.pop_front();
+  }
   const bool now_inited = info[0] != 0;
   const lio_est_config &ec = nd->cfg.est;
   if (ec.imu_factor && !nd->inited && now_inited && (ec.enable_deskew || ec.cutoff_deskew)) {
@@ -170,6 +228,10 @@ static int process_message(lio_node *nd, const Slot &s) {
     nd->odom_on = false;
   }
   nd->inited = now_inited;
+  if (nd->mb && was_inited && (rc = map_builder_step(nd)) != LIO_OK) { nd->poisoned = true; return rc; }
+  // the estimator's PointMapping publishes /cloud_registered once per processed message (see lio_node_attach_registered_map)
+  if ((rc = insert_registered(nd, LIO_NODE_MAP_ESTIMATOR)) != LIO_OK) { nd->poisoned = true; return rc; }
+  if (nd->mb && was_inited && (rc = insert_registered(nd, LIO_NODE_MAP_BUILDER)) != LIO_OK) { nd->poisoned = true; return rc; }
   return LIO_OK;
 }
 
@@ -189,7 +251,7 @@ static int drain(lio_node *nd) {
 
 static int refuse_poisoned(lio_node *nd) {
   if (!nd->poisoned) return LIO_OK;
-  lio_set_last_error(__FILE__, __LINE__, "lio_node: an earlier estimator failure poisoned the node; destroy and re-create it");
+  lio_set_last_error(__FILE__, __LINE__, "lio_node: an earlier estimator or map builder failure poisoned the node; destroy and re-create it");
   return LIO_ERR_INVALID;
 }
 
@@ -302,5 +364,61 @@ extern "C" int lio_node_handles(lio_node *nd, lio_pp **pp, lio_po **po, lio_est 
   if (po) *po = nd->po;
   if (est) *est = nd->est;
   if (pm) *pm = nd->pm;
+  return LIO_OK;
+}
+
+extern "C" int lio_node_enable_map_builder(lio_node *nd, const lio_mb_config *cfg) {
+  if (!nd || !cfg) return LIO_ERR_INVALID;
+  if (nd->mb || nd->sweeps > 0 || nd->poisoned) {
+    lio_set_last_error(__FILE__, __LINE__, "lio_node_enable_map_builder: once, before the first sweep");
+    return LIO_ERR_INVALID;
+  }
+  const float *ptr[3];
+  const int *n_dev = nullptr;
+  int n_host[3];
+  int rc = lio_est_local_clouds_dev(nd->est, ptr, &n_dev, n_host);
+  if (rc != LIO_OK) return rc;
+  LIO_CUDA_OK(cudaSetDevice(nd->device));
+  return lio_mb_create(cfg, std::max(n_host[0], n_host[1]), n_host[2], nd->device, nd->stream, &nd->mb);
+}
+
+extern "C" int lio_node_map_builder(lio_node *nd, lio_pm **mb) {
+  if (!nd || !mb) return LIO_ERR_INVALID;
+  *mb = nd->mb;
+  if (nd->mb) return LIO_OK;
+  lio_set_last_error(__FILE__, __LINE__, "lio_node_map_builder: no map builder (lio_node_enable_map_builder)");
+  return LIO_ERR_INVALID;
+}
+
+extern "C" int lio_node_map_builder_poses(lio_node *nd, double *stamp, float *tobe7, float *aft7, int *info6, int cap, int *n) {
+  if (!nd || !n || cap < 0) return LIO_ERR_INVALID;
+  if (!nd->mb) {
+    lio_set_last_error(__FILE__, __LINE__, "lio_node_map_builder_poses: no map builder (lio_node_enable_map_builder)");
+    return LIO_ERR_INVALID;
+  }
+  const int rows = (int)nd->mb_rows.size();
+  *n = rows;
+  if (rows > cap) return LIO_ERR_CAPACITY;
+  for (int r = 0; r < rows; ++r) {
+    const MbRow &row = nd->mb_rows[r];
+    if (stamp) stamp[r] = row.stamp;
+    if (tobe7) std::memcpy(tobe7 + 7 * r, row.tobe7, sizeof(row.tobe7));
+    if (aft7) std::memcpy(aft7 + 7 * r, row.aft7, sizeof(row.aft7));
+    if (info6) std::memcpy(info6 + 6 * r, row.info6, sizeof(row.info6));
+  }
+  return LIO_OK;
+}
+
+extern "C" int lio_node_attach_registered_map(lio_node *nd, lio_rm *rm, int source) {
+  if (!nd || !rm) return LIO_ERR_INVALID;
+  const char *why = nullptr;
+  if (source != LIO_NODE_MAP_ESTIMATOR && source != LIO_NODE_MAP_BUILDER) why = "lio_node_attach_registered_map: unknown source";
+  else if (source == LIO_NODE_MAP_BUILDER && !nd->mb) why = "lio_node_attach_registered_map: the map builder's source needs lio_node_enable_map_builder first";
+  else if (rm_device(rm) != nd->device || rm_stream(rm) != nd->stream) why = "lio_node_attach_registered_map: the map must be on the node's device and stream";
+  else if (nd->poisoned) why = "lio_node_attach_registered_map: the node is poisoned";
+  for (const DriveMap &d : nd->maps)
+    if (!why && d.rm == rm) why = "lio_node_attach_registered_map: the map is attached already";
+  if (why) { lio_set_last_error(__FILE__, __LINE__, why); return LIO_ERR_INVALID; }
+  nd->maps.push_back(DriveMap{rm, source});
   return LIO_OK;
 }

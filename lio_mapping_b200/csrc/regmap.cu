@@ -22,6 +22,7 @@
 #include <cstring>
 #include <vector>
 #include "primitives.cuh"
+#include "regmap.cuh"
 
 namespace lio {
 
@@ -346,6 +347,9 @@ static int rm_insert(lio_rm *m, const float4 *src, const float *host_src, int n)
   m->last_launches = launches;
   return LIO_OK;
 }
+
+int rm_device(const lio_rm *m) { return m->device; }
+cudaStream_t rm_stream(const lio_rm *m) { return m->stream; }
 
 extern "C" int lio_rm_insert_dev(lio_rm *m, const float *xyzi_dev, int n) {
   if (!m || n < 0 || (n > 0 && !xyzi_dev)) return LIO_ERR_INVALID;

@@ -4,7 +4,12 @@ the estimator's start-up and window solve, and its PointMapping inside the libra
 
 SHIPPED holds the three shipped configurations: config/indoor_test_config.yaml, config/outdoor_test_config.yaml and
 config/outdoor_test_config_64.yaml (the values below cite file:line), with the processor_node parameters of the launch file that starts
-each of them.  LioNode.shipped(name, ...) builds a node from one; the capacities and anything else can be given as keyword arguments."""
+each of them.  LioNode.shipped(name, ...) builds a node from one; the capacities and anything else can be given as keyword arguments.
+
+The second line of the reference's example, launch/map_4D*.launch (map_builder_node on the estimator's /local/* clouds), runs inside the
+node after enable_map_builder() (or shipped(name, map_4d=True)): one MapBuilder::ProcessMap per message that reaches the estimator
+INITED, on the node's stream.  map_builder_poses() is the drive's 4-D trajectory; attach_registered_map() feeds a RegisteredMap (the
+save_bag_to_pcd tool) from the estimator's or the map builder's /cloud_registered."""
 from __future__ import annotations
 
 import ctypes as C
@@ -13,6 +18,7 @@ import numpy as np
 
 from . import _lib, synth
 from .estimator import Estimator
+from .map_builder import MapBuilder
 from .point_mapping import PointMapping
 from .point_odometry import PointOdometry
 from .point_processor import PointProcessor
@@ -103,6 +109,16 @@ class _MappingView(_Borrowed, PointMapping):
         self.h = h
 
 
+class _MapBuilderView(_Borrowed, MapBuilder):
+    def __init__(self, h, config):
+        self.h, self.config = h, config   # transform_aft_mapped: see LioNode.map_builder_poses()
+
+    def ProcessMap(self, *args):
+        raise TypeError("the node runs its map builder; ProcessMap is not available on the view")
+
+    ProcessMapDev = ProcessMap
+
+
 class _OdometryView(_Borrowed, PointOdometry):
     def __init__(self, h):
         self.h = h
@@ -147,16 +163,64 @@ class LioNode:
         self.mapping = _MappingView(pm_h)
         self.odometry = _OdometryView(po_h)
         self.processor = _ProcessorView(pp_h, c.pp)
+        self.map_builder = None
+        self._maps = []   # attached RegisteredMaps: the node inserts into them, so it keeps them alive
 
     @classmethod
-    def shipped(cls, name, **overrides):
-        """A node with the values of SHIPPED[name]; keyword arguments (capacities, tf_lb7, any config field) take precedence."""
+    def shipped(cls, name, map_4d=False, **overrides):
+        """A node with the values of SHIPPED[name]; keyword arguments (capacities, tf_lb7, any config field) take precedence.  map_4d=True
+        also runs map_4D*.launch's map builder with its defaults (enable_map_builder())."""
         s = SHIPPED[name]
         kw = dict(sensor_type=s["sensor_type"], odom_io=s["odom_io"], msg_time_delay=s["msg_time_delay"], tf_lb7=shipped_tf_lb7(name),
                   corner_filter_size=s["corner_filter_size"], surf_filter_size=s["surf_filter_size"], map_filter_size=s["map_filter_size"])
         kw.update({k: s[k] for k in _EST_KEYS if k != "surf_filter_size"})
         kw.update(overrides)
-        return cls(**kw)
+        node = cls(**kw)
+        if map_4d:
+            node.enable_map_builder()
+        return node
+
+    def enable_map_builder(self, **cfg):
+        """map_builder_node inside the node (lio_node_enable_map_builder): MBConfig fields as keyword arguments over the defaults of
+        map_4D.launch / map_4D_indoor.launch (map_builder.default_config()).  Once, before the first sweep.  Afterwards map_builder is a
+        read-only MapBuilder view of it."""
+        c = _lib.MBConfig()
+        _lib.lib().lio_mb_default_config(C.byref(c))
+        for k, v in cfg.items():
+            if not hasattr(c, k):
+                raise AttributeError(f"MapBuilderConfig has no field {k}")
+            setattr(c, k, v)
+        _lib.check(_lib.lib().lio_node_enable_map_builder(self.h, C.byref(c)), "lio_node_enable_map_builder")
+        mb = C.c_void_p()
+        _lib.check(_lib.lib().lio_node_map_builder(self.h, C.byref(mb)), "lio_node_map_builder")
+        self.map_builder = _MapBuilderView(mb, {name: getattr(c, name) for name, _ in c._fields_})
+
+    def map_builder_poses(self):
+        """The map builder's trajectory, one row per call: dict of stamp (n,) float64 (the set's header stamp), tobe and aft (n, 7) float32
+        tf7 (transform_tobe_mapped_, transform_aft_mapped_), and the per-call iterations, optimised, corner_from_map, surf_from_map,
+        surround_published and surround_size as (n,) arrays."""
+        L = _lib.lib()
+        n = C.c_int()
+        one = (np.zeros(1), np.zeros((1, 7), np.float32), np.zeros((1, 7), np.float32), np.zeros((1, 6), np.int32))
+        rc = L.lio_node_map_builder_poses(self.h, *one, 0, C.byref(n))
+        if rc != -3:   # LIO_ERR_CAPACITY: *n rows do not fit in 0, as asked
+            _lib.check(rc, "lio_node_map_builder_poses")
+        cap = max(n.value, 1)
+        stamp, tobe, aft, info = np.zeros(cap), np.zeros((cap, 7), np.float32), np.zeros((cap, 7), np.float32), np.zeros((cap, 6), np.int32)
+        _lib.check(L.lio_node_map_builder_poses(self.h, stamp, tobe, aft, info, cap, C.byref(n)), "lio_node_map_builder_poses")
+        k = n.value
+        out = dict(stamp=stamp[:k], tobe=tobe[:k], aft=aft[:k])
+        for j, name in enumerate(("iterations", "optimised", "corner_from_map", "surf_from_map", "surround_published", "surround_size")):
+            out[name] = info[:k, j].astype(bool) if name in ("optimised", "surround_published") else info[:k, j].copy()
+        return out
+
+    def attach_registered_map(self, rm, source="estimator"):
+        """Insert every /cloud_registered of source ("estimator": the estimator's PointMapping, once per processed message;
+        "map_builder": once per map builder call) into the RegisteredMap rm, stream-ordered.  rm must be on the node's device and stream;
+        the node keeps a reference to it."""
+        code = {"estimator": 0, "map_builder": 1}.get(source, -1)
+        _lib.check(_lib.lib().lio_node_attach_registered_map(self.h, rm.h, code), "lio_node_attach_registered_map")
+        self._maps.append(rm)
 
     def close(self):
         if getattr(self, "h", None):
