@@ -384,6 +384,10 @@ int lio_asm_set_fold_chunks(int chunks);
  * factorisation, trailing update incl. barrier} as seen by the warp that runs the serial chain, then the back substitution. */
 int lio_dev_cholesky_solve_host(const double *A, const double *b, int n, double *x, int *ok, long long *prof, int device);
 
+/* Test seam of the library's resource ownership: the device and pinned host allocations, streams, events, graphs, graph execs
+ * and node sub-handles currently held by every handle of the process.  Creation, enable / attach calls, a first solve's graph capture and
+ * map regrowth move it; destroying a handle returns it to where it was before the handle's creation. */
+long long lio_live_resources(void);
 /* Test seam of the sort under every device VoxelGrid and the cube-map insert: the stable LSD radix sort of (key, value) pairs
  * by the low key_bits (1..32) bits, rounded up to whole 8-bit passes, on n host pairs; the result is read from whichever
  * buffer pair the last pass wrote.  Synchronous. */

@@ -85,6 +85,7 @@ def lib():
     L.lio_last_error.restype = C.c_char_p
     L.lio_version.restype = C.c_int
     L.lio_device_count.restype = C.c_int
+    L.lio_live_resources.restype = C.c_longlong
     vp, ip = C.c_void_p, C.c_int
     L.lio_pp_default_config.argtypes = [C.POINTER(PPConfig)]
     L.lio_pp_create.argtypes = [C.POINTER(PPConfig), ip, ip, vp, C.POINTER(vp)]

@@ -279,17 +279,9 @@ asm_ppp(const AsmParams P, const double *__restrict__ Rt, double *__restrict__ p
 
 int AsmWork::init(int max_features_total) {
   ntiles_max = max_features_total / kAsmThreads + 2 * kMaxOpt + 16;
-  if (cudaMalloc(&partial, sizeof(double) * (size_t)ntiles_max * kAsmStride) != cudaSuccess) return -1;
-  if (cudaMalloc(&out, sizeof(double) * kMaxOpt * kAsmStride) != cudaSuccess) return -1;
-  if (cudaMalloc(&counter, sizeof(unsigned)) != cudaSuccess) return -1;
+  if (!alloc(partial, (size_t)ntiles_max * kAsmStride) || !alloc(out, kMaxOpt * kAsmStride) || !alloc(counter, 1)) return -1;
   cudaMemset(counter, 0, sizeof(unsigned));
   return 0;
-}
-void AsmWork::destroy() {
-  if (partial) cudaFree(partial);
-  if (out) cudaFree(out);
-  if (counter) cudaFree(counter);
-  partial = out = nullptr; counter = nullptr;
 }
 
 static int g_fold_chunks = kAsmFold / kAsmPerThread;

@@ -36,12 +36,11 @@ struct AsmParams {
 };
 
 struct AsmWork {
-  double *partial = nullptr;  // [ntiles_max][kAsmStride]
-  double *out = nullptr;      // [kMaxOpt][kAsmStride] device
-  unsigned *counter = nullptr;
+  DevMem<double> partial;     // [ntiles_max][kAsmStride]
+  DevMem<double> out;         // [kMaxOpt][kAsmStride] device
+  DevMem<unsigned> counter;
   int ntiles_max = 0;
   int init(int max_features_total);
-  void destroy();
 };
 
 // Test seam: stages between folds of the running (1 + r^2) product (default 1024 = 2048 features per thread).

@@ -1,8 +1,9 @@
-// lio_mapping_b200 — library-wide C-ABI helpers (error text, device probe).
+// lio_mapping_b200 — library-wide C-ABI helpers (error text, device probe, live-resource count).
 #include "common.cuh"
 #include <cstring>
 
 static thread_local char g_err[512] = "";
+std::atomic<long long> lio::g_live_resources{0};
 
 void lio_set_last_error(const char *file, int line, const char *msg) {
   snprintf(g_err, sizeof(g_err), "%s:%d: %s", file, line, msg ? msg : "");
@@ -10,6 +11,7 @@ void lio_set_last_error(const char *file, int line, const char *msg) {
 
 extern "C" const char *lio_last_error(void) { return g_err; }
 extern "C" int lio_version(void) { return 100; }
+extern "C" long long lio_live_resources(void) { return lio::g_live_resources.load(); }
 extern "C" int lio_device_count(void) {
   int n = 0;
   cudaError_t e = cudaGetDeviceCount(&n);

@@ -5,6 +5,7 @@
 #include <cstdio>
 #include <vector>
 #include "../../include/lio_b200.h"
+#include "own.cuh"
 
 #define LIO_CUDA_OK(expr)                                                                   \
   do {                                                                                      \
@@ -22,24 +23,23 @@ namespace lio {
 // Device buffers of a host-array entry, freed when the entry returns.  alloc / up / down / ok set lio_last_error and return
 // false on failure, so an entry stops at the first failed allocation, copy or CUDA call.
 struct DevBufs {
-  std::vector<void *> p;
-  DevBufs() = default;
-  DevBufs(const DevBufs &) = delete;
-  DevBufs &operator=(const DevBufs &) = delete;
-  ~DevBufs() { for (void *q : p) cudaFree(q); }
+  std::vector<DevMem<void>> p;
   template <class T> bool alloc(T **out, size_t n) {
-    void *q = nullptr;
-    if (cudaMalloc(&q, sizeof(T) * (n ? n : 1)) != cudaSuccess) { lio_set_last_error(__FILE__, __LINE__, "cudaMalloc failed"); return false; }
-    p.push_back(q); *out = (T *)q;
+    DevMem<T> q;
+    if (!lio::alloc(q, n)) return false;
+    *out = q;
+    p.push_back(std::move(q));
     return true;
   }
-  // n elements of T; n == 0 copies nothing and leaves the pointers untouched
-  template <class T> static bool up(T *dst, const T *src, size_t n) {
+  // n elements of T; n == 0 copies nothing and leaves the pointers untouched.  T comes from the host side, so the device side
+  // may be an owner.
+  template <class T> struct Dev { using type = T; };
+  template <class T> static bool up(typename Dev<T>::type *dst, const T *src, size_t n) {
     if (n == 0 || cudaMemcpy(dst, src, sizeof(T) * n, cudaMemcpyHostToDevice) == cudaSuccess) return true;
     lio_set_last_error(__FILE__, __LINE__, "upload failed");
     return false;
   }
-  template <class T> static bool down(T *dst, const T *src, size_t n) {
+  template <class T> static bool down(T *dst, const typename Dev<T>::type *src, size_t n) {
     return n == 0 || ok(cudaMemcpy(dst, src, sizeof(T) * n, cudaMemcpyDeviceToHost));
   }
   static bool ok(cudaError_t e) {

@@ -26,6 +26,7 @@
 #include <cmath>
 #include <cstdio>
 #include <cstring>
+#include <memory>
 #include <new>
 #include <vector>
 #include "odom.cuh"
@@ -157,7 +158,7 @@ k_gather_segments(const Segment *__restrict__ seg, int nseg, float4 *__restrict_
 using namespace lio;
 
 struct lio_pm {
-  struct Cube { float4 *p = nullptr; int n = 0, cap = 0; };
+  struct Cube { DevMem<float4> p; int n = 0, cap = 0; };
   int device = 0;
   cudaStream_t stream = nullptr;
   int sm = 132;
@@ -170,13 +171,13 @@ struct lio_pm {
   double delta_r_abort = 0.05, delta_t_abort = 0.05;
   TwistF sum, bef, aft, tobe;          // transform_sum_, transform_bef_mapped_, transform_aft_mapped_, transform_tobe_mapped_
   // device scratch
-  float4 *d_in[2] = {nullptr, nullptr}, *d_stack[2] = {nullptr, nullptr}, *d_ds[2] = {nullptr, nullptr}, *d_mapped = nullptr;
-  float4 *d_map[2] = {nullptr, nullptr};
+  DevMem<float4> d_in[2], d_stack[2], d_ds[2], d_mapped;
+  DevMem<float4> d_map[2];
   int map_cap[2] = {0, 0};
-  int *d_cnt = nullptr;                // [0,1] input sizes, [2,3] down-sampled sizes, [4] full cloud, [5,6] surround map in / out,
+  DevMem<int> d_cnt;                   // [0,1] input sizes, [2,3] down-sampled sizes, [4] full cloud, [5,6] surround map in / out,
                                        // [7] input count over its bound, [8..10] counts uploaded by the host entries
   int h_cnt[8] = {};                   // read-back of d_cnt[0..7] after the down-sampling
-  Segment *d_seg = nullptr;
+  DevMem<Segment> d_seg;
   VoxelGrid vg;
   ScanToMapWork stm;
   int stm_cap[3] = {0, 0, 0};
@@ -184,24 +185,26 @@ struct lio_pm {
   std::vector<size_t> last_valid, last_surround;   // laser_cloud_valid_idx_ / laser_cloud_surround_idx_ of the last process call
   // UpdateMapDatabase (pm_update).  Insert: sort buffers for ins_cap (initially 2 * max_points) keys, per-key slot / first position, the run list
   // (pinned, written by the device), the touched cubes' table (pinned and its device copy).
-  unsigned *d_ins_k[2] = {nullptr, nullptr}, *d_ins_v[2] = {nullptr, nullptr};
+  DevMem<unsigned> d_ins_k[2], d_ins_v[2];
   RadixSortTemp ins_rs;
   int ins_cap = 0;
-  int *d_ins_n = nullptr;              // [0] points, [1] runs
-  int *d_slot_of = nullptr, *d_start_of = nullptr;
-  InsRun *h_runs = nullptr, *h_runs_dev = nullptr;
-  int *h_nruns = nullptr;              // read-back of d_ins_n: [0] points inserted, [1] runs
-  CubeEnd *h_tab = nullptr, *d_tab = nullptr;
-  cudaEvent_t ev_ins = nullptr;
+  DevMem<int> d_ins_n;                 // [0] points, [1] runs
+  DevMem<int> d_slot_of, d_start_of;
+  HostMem<InsRun> h_runs;              // mapped: h_runs_dev is its device address
+  InsRun *h_runs_dev = nullptr;
+  HostMem<int> h_nruns;                // read-back of d_ins_n: [0] points inserted, [1] runs
+  HostMem<CubeEnd> h_tab;
+  DevMem<CubeEnd> d_tab;
+  Event ev_ins;
   // Re-filter: one segmented VoxelGrid over the jobs; their output counts arrive in h_jn (pinned) behind ev_counts and are applied
   // to the directory by pm_counts before anything reads it.
   SegVoxelGrid svg;
-  VgJob *h_jobs = nullptr;
-  int *h_jn = nullptr;
+  HostMem<VgJob> h_jobs;
+  HostMem<int> h_jn;
   std::vector<std::pair<int, size_t>> pend_jobs;   // (cloud, cube) of every job whose count is in flight
   bool counts_pending = false;
   bool counts_broken = false;          // a job exceeded the 2^24-voxel bound: its cubes are wrong, every later reader fails
-  cudaEvent_t ev_counts = nullptr;
+  Event ev_counts;
   int upd_stats[4] = {0, 0, 0, 0};     // last UpdateMapDatabase: cube jobs, kernel launches, host waits (the later wait for the
                                        // re-filtered counts included), points inserted
   bool started = false;               // a process call has run (lio_pm_enable_publish must come before it)
@@ -214,9 +217,10 @@ struct lio_pm {
   int map_frame_count = 4;             // num_map_frames_ - 1 (PointMapping.cc:104): the first frame publishes
   float map_leaf = 0.2f;               // down_size_filter_map_ (PointMapping.cc:123 0.6, map_builder_node 0.2)
   int max_full = 0, n_full = 0, n_surround = 0, sur_cap = 0;
-  float4 *d_full_in = nullptr, *d_full_out = nullptr, *d_sur = nullptr, *d_sur_ds = nullptr;
-  Segment *d_sur_seg = nullptr, *h_sur_seg = nullptr;   // h_sur_seg / h_sur_n: pinned, so their uploads need no sync
-  int *h_sur_n = nullptr;
+  DevMem<float4> d_full_in, d_full_out, d_sur, d_sur_ds;
+  DevMem<Segment> d_sur_seg;
+  HostMem<Segment> h_sur_seg;          // h_sur_seg / h_sur_n: pinned, so their uploads need no sync
+  HostMem<int> h_sur_n;
   VoxelGrid vg_sur;                    // down_size_filter_map_, sized for the surround map
 };
 
@@ -230,24 +234,7 @@ static int cube_of_host(float v, int cen) {
 extern "C" int lio_pm_destroy(lio_pm *m) {
   if (!m) return LIO_OK;
   if (m->attached) { lio_set_last_error(__FILE__, __LINE__, "lio_pm_destroy: the map is attached to an estimator (lio_est_destroy releases it)"); return LIO_ERR_INVALID; }
-  cudaSetDevice(m->device);
-  for (int w = 0; w < 2; ++w) {
-    for (lio_pm::Cube &c : m->cube[w]) if (c.p) cudaFree(c.p);
-    void *fr[] = {m->d_in[w], m->d_stack[w], m->d_ds[w], m->d_map[w]};
-    for (void *q : fr) if (q) cudaFree(q);
-  }
-  void *fr[] = {m->d_mapped, m->d_cnt, m->d_seg, m->d_full_in, m->d_full_out, m->d_sur, m->d_sur_ds, m->d_sur_seg, m->d_ins_k[0],
-                m->d_ins_k[1], m->d_ins_v[0], m->d_ins_v[1], m->d_ins_n, m->d_slot_of, m->d_start_of, m->d_tab};
-  for (void *q : fr) if (q) cudaFree(q);
-  void *frh[] = {m->h_sur_seg, m->h_sur_n, m->h_runs, m->h_nruns, m->h_tab, m->h_jobs, m->h_jn};
-  for (void *q : frh) if (q) cudaFreeHost(q);
-  if (m->ev_ins) cudaEventDestroy(m->ev_ins);
-  if (m->ev_counts) cudaEventDestroy(m->ev_counts);
-  m->vg.destroy();
-  m->vg_sur.destroy();
-  m->svg.destroy();
-  m->ins_rs.destroy();
-  m->stm.destroy();
+  cudaSetDevice(m->device);   // the buffers belong to the handle's device, whichever is current
   delete m;
   return LIO_OK;
 }
@@ -257,45 +244,26 @@ extern "C" int lio_pm_create(int max_points, float corner_filter_size, float sur
   if (!out || max_points < 16 || !(corner_filter_size > 0) || !(surf_filter_size > 0) || max_iterations < 0) return LIO_ERR_INVALID;
   if (lio_device_count() <= 0) return LIO_ERR_NO_DEVICE;
   LIO_CUDA_OK(cudaSetDevice(device));
-  lio_pm *m = new (std::nothrow) lio_pm();
+  std::unique_ptr<lio_pm> m(new (std::nothrow) lio_pm());
   if (!m) return LIO_ERR_INVALID;
   m->device = device; m->stream = (cudaStream_t)cuda_stream; m->max_points = max_points;
   m->leaf[0] = corner_filter_size; m->leaf[1] = surf_filter_size;
   m->min_match_sq_dis = min_match_sq_dis; m->min_plane_dis = min_plane_dis; m->max_iter = max_iterations;
   cudaDeviceGetAttribute(&m->sm, cudaDevAttrMultiProcessorCount, device);
-  m->cube[0].assign(kCubes, lio_pm::Cube());
-  m->cube[1].assign(kCubes, lio_pm::Cube());
-  bool ok = true;
-  for (int w = 0; w < 2 && ok; ++w) {
-    ok = ok && cudaMalloc(&m->d_in[w], sizeof(float4) * max_points) == cudaSuccess;
-    ok = ok && cudaMalloc(&m->d_stack[w], sizeof(float4) * max_points) == cudaSuccess;
-    ok = ok && cudaMalloc(&m->d_ds[w], sizeof(float4) * max_points) == cudaSuccess;
-  }
-  m->ins_cap = 2 * max_points;
-  ok = ok && cudaMalloc(&m->d_mapped, sizeof(float4) * 2 * max_points) == cudaSuccess;
-  ok = ok && cudaMalloc(&m->d_cnt, sizeof(int) * 12) == cudaSuccess;
-  ok = ok && cudaMalloc(&m->d_seg, sizeof(Segment) * 256) == cudaSuccess;
-  ok = ok && m->vg.init(max_points) == 0;
-  for (int b = 0; b < 2 && ok; ++b) {
-    ok = ok && cudaMalloc(&m->d_ins_k[b], sizeof(unsigned) * 2 * max_points) == cudaSuccess;
-    ok = ok && cudaMalloc(&m->d_ins_v[b], sizeof(unsigned) * 2 * max_points) == cudaSuccess;
-  }
-  ok = ok && m->ins_rs.init(2 * max_points) == 0;
-  ok = ok && cudaMalloc(&m->d_ins_n, sizeof(int) * 2) == cudaSuccess;
-  ok = ok && cudaMalloc(&m->d_slot_of, sizeof(int) * kInsOutside) == cudaSuccess;
-  ok = ok && cudaMalloc(&m->d_start_of, sizeof(int) * kInsOutside) == cudaSuccess;
-  ok = ok && cudaMalloc(&m->d_tab, sizeof(CubeEnd) * kInsOutside) == cudaSuccess;
-  ok = ok && cudaHostAlloc(&m->h_runs, sizeof(InsRun) * kInsOutside, cudaHostAllocMapped) == cudaSuccess;
-  ok = ok && cudaHostGetDevicePointer(&m->h_runs_dev, m->h_runs, 0) == cudaSuccess;
-  ok = ok && cudaMallocHost(&m->h_nruns, sizeof(int) * 2) == cudaSuccess;
-  ok = ok && cudaMallocHost(&m->h_tab, sizeof(CubeEnd) * kInsOutside) == cudaSuccess;
-  ok = ok && m->svg.init() == 0;
-  ok = ok && cudaMallocHost(&m->h_jobs, sizeof(VgJob) * kVgMaxJobs) == cudaSuccess;
-  ok = ok && cudaMallocHost(&m->h_jn, sizeof(int) * (kVgMaxJobs + 1)) == cudaSuccess;
-  ok = ok && cudaEventCreateWithFlags(&m->ev_ins, cudaEventDisableTiming) == cudaSuccess;
-  ok = ok && cudaEventCreateWithFlags(&m->ev_counts, cudaEventDisableTiming) == cudaSuccess;
-  if (!ok) { lio_set_last_error(__FILE__, __LINE__, "lio_pm_create: device allocation failed"); lio_pm_destroy(m); return LIO_ERR_CUDA; }
-  *out = m;
+  m->cube[0].resize(kCubes);
+  m->cube[1].resize(kCubes);
+  const int n = max_points;
+  m->ins_cap = 2 * n;
+  const bool ok = alloc(m->d_in[0], n) && alloc(m->d_stack[0], n) && alloc(m->d_ds[0], n) && alloc(m->d_in[1], n) && alloc(m->d_stack[1], n) &&
+                  alloc(m->d_ds[1], n) && alloc(m->d_mapped, 2 * n) && alloc(m->d_cnt, 12) && alloc(m->d_seg, 256) && m->vg.init(n) == 0 &&
+                  alloc(m->d_ins_k[0], 2 * n) && alloc(m->d_ins_v[0], 2 * n) && alloc(m->d_ins_k[1], 2 * n) && alloc(m->d_ins_v[1], 2 * n) &&
+                  m->ins_rs.init(2 * n) == 0 && alloc(m->d_ins_n, 2) && alloc(m->d_slot_of, kInsOutside) && alloc(m->d_start_of, kInsOutside) &&
+                  alloc(m->d_tab, kInsOutside) && alloc_host(m->h_runs, kInsOutside, cudaHostAllocMapped) &&
+                  cudaHostGetDevicePointer(&m->h_runs_dev, m->h_runs, 0) == cudaSuccess && alloc_host(m->h_nruns, 2) &&
+                  alloc_host(m->h_tab, kInsOutside) && m->svg.init() == 0 && alloc_host(m->h_jobs, kVgMaxJobs) && alloc_host(m->h_jn, kVgMaxJobs + 1) &&
+                  create(m->ev_ins) && create(m->ev_counts);
+  if (!ok) { lio_set_last_error(__FILE__, __LINE__, "lio_pm_create: device allocation failed"); return LIO_ERR_CUDA; }
+  *out = m.release();
   return LIO_OK;
 }
 
@@ -367,11 +335,12 @@ static int pm_grow(lio_pm *m, lio_pm::Cube &c, int need) {
   if (need <= c.cap) return LIO_OK;
   int cap = std::max(1024, c.cap);
   while (cap < need) cap *= 2;
-  float4 *p = nullptr;
-  LIO_CUDA_OK(cudaMalloc(&p, sizeof(float4) * cap));
+  // allocate new, copy, synchronise, then drop the old segment
+  DevMem<float4> p;
+  if (!alloc(p, cap)) return LIO_ERR_CUDA;
   if (c.p && c.n > 0) LIO_CUDA_OK(cudaMemcpyAsync(p, c.p, sizeof(float4) * c.n, cudaMemcpyDeviceToDevice, m->stream));
-  if (c.p) { LIO_CUDA_OK(cudaStreamSynchronize(m->stream)); cudaFree(c.p); }
-  c.p = p; c.cap = cap;
+  if (c.p) LIO_CUDA_OK(cudaStreamSynchronize(m->stream));
+  c.p = std::move(p); c.cap = cap;
   return LIO_OK;
 }
 
@@ -383,10 +352,12 @@ static int pm_from_map(lio_pm *m, const std::vector<size_t> &valid, int w, int &
     const lio_pm::Cube &c = m->cube[w][v];
     if (c.n > 0) { seg.push_back(Segment{c.p, c.n, total}); total += c.n; }
   }
-  if (total > m->map_cap[w]) {
-    if (m->d_map[w]) cudaFree(m->d_map[w]);
-    m->map_cap[w] = std::max(2 * total, 1 << 16);
-    LIO_CUDA_OK(cudaMalloc(&m->d_map[w], sizeof(float4) * m->map_cap[w]));
+  if (total > m->map_cap[w]) {   // the old map is rebuilt below: it goes first
+    m->d_map[w] = {};
+    m->map_cap[w] = 0;
+    const int cap = std::max(2 * total, 1 << 16);
+    if (!alloc(m->d_map[w], cap)) return LIO_ERR_CUDA;
+    m->map_cap[w] = cap;
   }
   if (seg.empty()) return LIO_OK;
   if (seg.size() > 256) return LIO_ERR_CAPACITY;
@@ -561,7 +532,7 @@ static int pm_optimise(lio_pm *m, const int K[2], const int n_ds[2], int variant
   m->last_iters = 0;
   if (m->max_iter <= 0) return LIO_OK;
   if (K[0] > m->stm_cap[0] || K[1] > m->stm_cap[1] || n_ds[0] + n_ds[1] > m->stm_cap[2]) {
-    m->stm.destroy();
+    m->stm = ScanToMapWork{};
     m->stm_cap[0] = std::max(2 * K[0], 1 << 15); m->stm_cap[1] = std::max(2 * K[1], 1 << 16); m->stm_cap[2] = std::max(2 * (n_ds[0] + n_ds[1]), 1 << 15);
     if (m->stm.init(m->stm_cap[0], m->stm_cap[1], m->stm_cap[2]) != 0) { lio_set_last_error(__FILE__, __LINE__, "scan-to-map workspace allocation failed"); return LIO_ERR_CUDA; }
   }
@@ -736,15 +707,13 @@ static int mb_surround(lio_pm *m, const std::vector<size_t> &surround) {
       if (c.n > 0) { m->h_sur_seg[nseg++] = Segment{c.p, c.n, total}; total += c.n; }
     }
   if (total == 0) { LIO_CUDA_OK(cudaMemsetAsync(m->d_cnt + 6, 0, sizeof(int), st)); return LIO_OK; }
-  if (total > m->sur_cap) {
-    if (m->d_sur) cudaFree(m->d_sur);
-    if (m->d_sur_ds) cudaFree(m->d_sur_ds);
-    m->d_sur = m->d_sur_ds = nullptr;
-    m->vg_sur.destroy();
+  if (total > m->sur_cap) {   // the old surround map is rebuilt below: it goes first
+    m->d_sur = {};
+    m->d_sur_ds = {};
+    m->vg_sur = VoxelGrid{};
     m->sur_cap = 0;
     const int cap = std::max(2 * total, 1 << 16);
-    LIO_CUDA_OK(cudaMalloc(&m->d_sur, sizeof(float4) * cap));
-    LIO_CUDA_OK(cudaMalloc(&m->d_sur_ds, sizeof(float4) * cap));
+    if (!alloc(m->d_sur, cap) || !alloc(m->d_sur_ds, cap)) return LIO_ERR_CUDA;
     if (m->vg_sur.init(cap) != 0) { lio_set_last_error(__FILE__, __LINE__, "surround VoxelGrid allocation failed"); return LIO_ERR_CUDA; }
     m->sur_cap = cap;
   }
@@ -758,21 +727,17 @@ static int mb_surround(lio_pm *m, const std::vector<size_t> &surround) {
 // Buffers of the published clouds (full cloud in / registered, surround segments); the surround map itself grows on demand.
 // On failure nothing stays allocated and the handle does not publish.
 static bool pm_alloc_publish(lio_pm *m, int max_full_points) {
+  DevMem<float4> full_in, full_out;
+  DevMem<Segment> sur_seg;
+  HostMem<Segment> h_sur_seg;
+  HostMem<int> h_sur_n;
+  if (!alloc(full_in, max_full_points) || !alloc(full_out, max_full_points) || !alloc(sur_seg, 2 * 125) || !alloc_host(h_sur_seg, 2 * 125) ||
+      !alloc_host(h_sur_n, 1))
+    return false;
+  m->d_full_in = std::move(full_in); m->d_full_out = std::move(full_out); m->d_sur_seg = std::move(sur_seg);
+  m->h_sur_seg = std::move(h_sur_seg); m->h_sur_n = std::move(h_sur_n);
   m->max_full = max_full_points;
-  bool ok = cudaMalloc(&m->d_full_in, sizeof(float4) * max_full_points) == cudaSuccess;
-  ok = ok && cudaMalloc(&m->d_full_out, sizeof(float4) * max_full_points) == cudaSuccess;
-  ok = ok && cudaMalloc(&m->d_sur_seg, sizeof(Segment) * 2 * 125) == cudaSuccess;
-  ok = ok && cudaMallocHost(&m->h_sur_seg, sizeof(Segment) * 2 * 125) == cudaSuccess;
-  ok = ok && cudaMallocHost(&m->h_sur_n, sizeof(int)) == cudaSuccess;
-  if (!ok) {
-    void *fr[] = {m->d_full_in, m->d_full_out, m->d_sur_seg};
-    for (void *q : fr) if (q) cudaFree(q);
-    if (m->h_sur_seg) cudaFreeHost(m->h_sur_seg);
-    if (m->h_sur_n) cudaFreeHost(m->h_sur_n);
-    m->d_full_in = m->d_full_out = nullptr; m->d_sur_seg = m->h_sur_seg = nullptr; m->h_sur_n = nullptr;
-    m->max_full = 0;
-  }
-  return ok;
+  return true;
 }
 
 extern "C" void lio_mb_default_config(lio_mb_config *cfg) {
@@ -879,13 +844,13 @@ extern "C" int lio_mb_process_map_dev(lio_pm *m, const float *corner_dev, const 
 
 extern "C" int lio_mb_surround_dev(lio_pm *m, const float **ptr, int *n) {
   if (!m || !(m->mb || m->publish) || !ptr || !n) return LIO_ERR_INVALID;
-  *ptr = (const float *)m->d_sur_ds; *n = m->n_surround;
+  *ptr = (const float *)m->d_sur_ds.get(); *n = m->n_surround;
   return LIO_OK;
 }
 
 extern "C" int lio_mb_full_dev(lio_pm *m, const float **ptr, int *n) {
   if (!m || !(m->mb || m->publish) || !ptr || !n) return LIO_ERR_INVALID;
-  *ptr = (const float *)m->d_full_out; *n = m->n_full;
+  *ptr = (const float *)m->d_full_out.get(); *n = m->n_full;
   return LIO_OK;
 }
 
@@ -968,28 +933,17 @@ int pm_attach(lio_pm *m, int device, float corner_leaf, float surf_leaf, int ins
   if (rc != LIO_OK) return rc;
   if (ins_bound > m->ins_cap) {   // an accumulated surf slot exceeds 2 * max_points: new insert buffers, swapped in on success
     LIO_CUDA_OK(cudaStreamSynchronize(m->stream));
-    float4 *mapped = nullptr;
-    unsigned *k[2] = {nullptr, nullptr}, *v[2] = {nullptr, nullptr};
+    DevMem<float4> mapped;
+    DevMem<unsigned> k[2], v[2];
     RadixSortTemp rs;
-    bool ok = cudaMalloc(&mapped, sizeof(float4) * ins_bound) == cudaSuccess;
-    for (int b = 0; b < 2 && ok; ++b) {
-      ok = ok && cudaMalloc(&k[b], sizeof(unsigned) * ins_bound) == cudaSuccess;
-      ok = ok && cudaMalloc(&v[b], sizeof(unsigned) * ins_bound) == cudaSuccess;
-    }
-    ok = ok && rs.init(ins_bound) == 0;
-    if (!ok) {
-      void *fr[] = {mapped, k[0], k[1], v[0], v[1]};
-      for (void *q : fr) if (q) cudaFree(q);
-      rs.destroy();
+    if (!alloc(mapped, ins_bound) || !alloc(k[0], ins_bound) || !alloc(v[0], ins_bound) || !alloc(k[1], ins_bound) || !alloc(v[1], ins_bound) ||
+        rs.init(ins_bound) != 0) {
       lio_set_last_error(__FILE__, __LINE__, "lio_est_attach_map: insert buffer allocation failed");
       return LIO_ERR_CUDA;
     }
-    void *fr[] = {m->d_mapped, m->d_ins_k[0], m->d_ins_k[1], m->d_ins_v[0], m->d_ins_v[1]};
-    for (void *q : fr) cudaFree(q);
-    m->ins_rs.destroy();
-    m->d_mapped = mapped;
-    for (int b = 0; b < 2; ++b) { m->d_ins_k[b] = k[b]; m->d_ins_v[b] = v[b]; }
-    m->ins_rs = rs;
+    m->d_mapped = std::move(mapped);
+    for (int b = 0; b < 2; ++b) { m->d_ins_k[b] = std::move(k[b]); m->d_ins_v[b] = std::move(v[b]); }
+    m->ins_rs = std::move(rs);
     m->ins_cap = ins_bound;
   }
   m->attached = true;

@@ -23,23 +23,6 @@ k_local_gather(const LocalGather G, int *__restrict__ n_out) {
 }  // namespace lio
 
 // ---- /local/* clouds (Estimator.cc:474-482, :628-693, :2355-2375, :2416) ------------------------------------------------
-void LocalClouds::release() {
-  if (stream) cudaStreamSynchronize(stream);
-  for (int w = 0; w < 2; ++w) {
-    for (float4 *p : slot[w]) if (p) cudaFree(p);
-    if (d_stage[w]) cudaFree(d_stage[w]);
-  }
-  for (int w = 0; w < 3; ++w) if (d_pub[w]) cudaFree(d_pub[w]);
-  if (d_slot_n) cudaFree(d_slot_n);
-  if (d_stage_n) cudaFree(d_stage_n);
-  if (d_pub_n) cudaFree(d_pub_n);
-  vg.destroy();
-  if (stream) cudaStreamDestroy(stream);
-  if (ev_fork) cudaEventDestroy(ev_fork);
-  if (ev_join) cudaEventDestroy(ev_join);
-  *this = LocalClouds();
-}
-
 extern "C" int lio_est_enable_local_clouds(lio_est *e, float corner_filter_size, int max_corner_points, int max_full_points) {
   if (!e || !(corner_filter_size > 0) || max_corner_points < 1 || max_full_points < 1) return LIO_ERR_INVALID;
   if (e->lc.on || e->frames_started) {
@@ -52,33 +35,28 @@ extern "C" int lio_est_enable_local_clouds(lio_est *e, float corner_filter_size,
   }
   LIO_CUDA_OK(cudaSetDevice(e->device));
   const int W = e->W;
-  e->lc.corner_leaf = corner_filter_size;
-  e->lc.cap[0] = max_corner_points; e->lc.cap[1] = max_full_points;
-  e->lc.pub_cap[0] = max_corner_points; e->lc.pub_cap[1] = e->cfg.max_frame_points; e->lc.pub_cap[2] = max_full_points;
+  LocalClouds lc;
+  lc.corner_leaf = corner_filter_size;
+  lc.cap[0] = max_corner_points; lc.cap[1] = max_full_points;
+  lc.pub_cap[0] = max_corner_points; lc.pub_cap[1] = e->cfg.max_frame_points; lc.pub_cap[2] = max_full_points;
   bool ok = true;
   for (int w = 0; w < 2; ++w) {
-    e->lc.slot[w].assign(W + 1, nullptr);
-    for (int k = 0; k <= W; ++k) ok = ok && cudaMalloc(&e->lc.slot[w][k], sizeof(float4) * e->lc.cap[w]) == cudaSuccess;
-    ok = ok && cudaMalloc(&e->lc.d_stage[w], sizeof(float4) * e->lc.cap[w]) == cudaSuccess;
+    lc.slot[w].resize(W + 1);
+    for (int k = 0; k <= W; ++k) ok = ok && alloc(lc.slot[w][k], lc.cap[w]);
+    ok = ok && alloc(lc.d_stage[w], lc.cap[w]);
   }
-  for (int w = 0; w < 3; ++w) ok = ok && cudaMalloc(&e->lc.d_pub[w], sizeof(float4) * e->lc.pub_cap[w]) == cudaSuccess;
-  ok = ok && cudaMalloc(&e->lc.d_slot_n, sizeof(int) * 2 * (W + 1)) == cudaSuccess;
-  ok = ok && cudaMalloc(&e->lc.d_stage_n, sizeof(int) * 2) == cudaSuccess;
-  ok = ok && cudaMalloc(&e->lc.d_pub_n, sizeof(int) * 3) == cudaSuccess;
-  ok = ok && cudaMemset(e->lc.d_slot_n, 0, sizeof(int) * 2 * (W + 1)) == cudaSuccess;
-  ok = ok && cudaMemset(e->lc.d_stage_n, 0, sizeof(int) * 2) == cudaSuccess;
-  ok = ok && cudaMemset(e->lc.d_pub_n, 0, sizeof(int) * 3) == cudaSuccess;
-  ok = ok && e->lc.vg.init(max_corner_points) == 0;
-  ok = ok && cudaStreamCreateWithFlags(&e->lc.stream, cudaStreamNonBlocking) == cudaSuccess;
-  ok = ok && cudaEventCreateWithFlags(&e->lc.ev_fork, cudaEventDisableTiming) == cudaSuccess;
-  ok = ok && cudaEventCreateWithFlags(&e->lc.ev_join, cudaEventDisableTiming) == cudaSuccess;
-  ok = ok && cudaDeviceSynchronize() == cudaSuccess;   // the memsets above ran on the legacy stream
-  if (!ok) {
+  for (int w = 0; w < 3; ++w) ok = ok && alloc(lc.d_pub[w], lc.pub_cap[w]);
+  ok = ok && alloc(lc.d_slot_n, 2 * (W + 1)) && alloc(lc.d_stage_n, 2) && alloc(lc.d_pub_n, 3) &&
+       cudaMemset(lc.d_slot_n, 0, sizeof(int) * 2 * (W + 1)) == cudaSuccess && cudaMemset(lc.d_stage_n, 0, sizeof(int) * 2) == cudaSuccess &&
+       cudaMemset(lc.d_pub_n, 0, sizeof(int) * 3) == cudaSuccess && lc.vg.init(max_corner_points) == 0 && create(lc.stream) &&
+       create(lc.ev_fork) && create(lc.ev_join) &&
+       cudaDeviceSynchronize() == cudaSuccess;   // the memsets above ran on the legacy stream
+  if (!ok) {   // lc goes: the handle stays usable with local clouds off
     lio_set_last_error(__FILE__, __LINE__, "lio_est_enable_local_clouds: device allocation failed");
-    e->lc.release();   // the handle stays usable with local clouds off
     return LIO_ERR_CUDA;
   }
-  e->lc.on = true;
+  lc.on = true;
+  e->lc = std::move(lc);
   return LIO_OK;
 }
 
@@ -178,7 +156,7 @@ extern "C" int lio_est_local_clouds_dev(lio_est *e, const float *ptr[3], const i
   if (!e) return LIO_ERR_INVALID;
   if (!e->lc.on) { lio_set_last_error(__FILE__, __LINE__, "local clouds are off"); return LIO_ERR_INVALID; }
   for (int w = 0; w < 3; ++w) {
-    if (ptr) ptr[w] = reinterpret_cast<const float *>(e->lc.d_pub[w]);
+    if (ptr) ptr[w] = reinterpret_cast<const float *>(e->lc.d_pub[w].get());
     if (n_host) n_host[w] = e->lc.pub_cap[w];
   }
   if (n_dev) *n_dev = e->lc.d_pub_n;
@@ -278,39 +256,28 @@ int map_step(lio_est *e) {
   return LIO_OK;
 }
 
-void AttachedMap::release() {
-  if (pm) {   // the pending insert reads the estimator's slots: wait for it, then release the map
-    if (pending) cudaEventSynchronize(ev_done);
-    pm_detach(pm);
-  }
-  for (int w = 0; w < 2; ++w) if (d_keep[w]) cudaFree(d_keep[w]);
-  if (d_keep_n) cudaFree(d_keep_n);
-  if (ev_in) cudaEventDestroy(ev_in);
-  if (ev_done) cudaEventDestroy(ev_done);
-  *this = AttachedMap();
+void AttachedMap::detach() {
+  if (!pm) return;
+  if (pending) cudaEventSynchronize(ev_done);   // the pending insert reads the estimator's slots
+  pm_detach(pm);
+  pm = nullptr;
+  pending = false;
 }
 
 // The estimator's side of both attaches: the map-step events, the W == O de-skew copies, and the handle's own checks (pm_attach).
 static int attach_common(lio_est *e, lio_pm *pm, bool fresh) {
   LIO_CUDA_OK(cudaSetDevice(e->device));
   const bool keep = e->W == e->O && map_deskew(e);
-  bool ok = cudaEventCreateWithFlags(&e->map.ev_in, cudaEventDisableTiming) == cudaSuccess;
-  ok = ok && cudaEventCreateWithFlags(&e->map.ev_done, cudaEventDisableTiming) == cudaSuccess;
-  if (keep) {
-    ok = ok && cudaMalloc(&e->map.d_keep[0], sizeof(float4) * e->lc.cap[0]) == cudaSuccess;
-    ok = ok && cudaMalloc(&e->map.d_keep[1], sizeof(float4) * e->slot_cap) == cudaSuccess;
-    ok = ok && cudaMalloc(&e->map.d_keep_n, sizeof(int) * 2) == cudaSuccess;
-  }
+  AttachedMap map;
+  bool ok = create(map.ev_in) && create(map.ev_done);
+  if (keep) ok = ok && alloc(map.d_keep[0], e->lc.cap[0]) && alloc(map.d_keep[1], e->slot_cap) && alloc(map.d_keep_n, 2);
   int rc = ok ? LIO_OK : LIO_ERR_CUDA;
   if (!ok) lio_set_last_error(__FILE__, __LINE__, "lio_est_attach_map: device allocation failed");
   // an accumulated surf slot holds up to max_frame_points * (W - O + 1) points: the map's insert buffers grow to it
   if (ok) rc = pm_attach(pm, e->device, e->lc.corner_leaf, e->cfg.surf_filter_size, e->lc.cap[0] + e->slot_cap, e->lc.cap[1], fresh);
-  if (rc != LIO_OK) {   // nothing changed: the buffers go, the handle stays usable without a map
-    e->map.release();
-    return rc;
-  }
-  e->map.pm = pm;
-  e->map.scans = 0;
+  if (rc != LIO_OK) return rc;   // nothing changed: map goes, the handle stays usable without a map
+  map.pm = pm;
+  e->map = std::move(map);
   return LIO_OK;
 }
 

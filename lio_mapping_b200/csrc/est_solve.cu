@@ -1042,18 +1042,18 @@ int solve_dev(lio_est *e, int max_it, bool assemble_only) {
       const int l0 = e->launches;
       LIO_CUDA_OK(cudaStreamBeginCapture(gs, cudaStreamCaptureModeThreadLocal));
       rc = enqueue(gs, true);
-      cudaGraph_t g = nullptr;
-      const cudaError_t ce = cudaStreamEndCapture(gs, &g);
-      if (rc != LIO_OK) { if (g) cudaGraphDestroy(g); return rc; }
+      Graph g;
+      const cudaError_t ce = end_capture(gs, g);
+      if (rc != LIO_OK) return rc;
       if (ce != cudaSuccess || !g) { lio_set_last_error(__FILE__, __LINE__, cudaGetErrorString(ce)); return LIO_ERR_CUDA; }
-      e->sgraph = g;
+      e->sgraph = std::move(g);
       e->graph_launches = e->launches - l0;
       e->launches = l0;
-      LIO_CUDA_OK(cudaGraphInstantiate(&e->sexec, g, 0));
+      if (!instantiate(e->sexec, e->sgraph)) return LIO_ERR_CUDA;
       size_t nn = 0;
-      LIO_CUDA_OK(cudaGraphGetNodes(g, nullptr, &nn));
+      LIO_CUDA_OK(cudaGraphGetNodes(e->sgraph, nullptr, &nn));
       std::vector<cudaGraphNode_t> nodes(nn);
-      LIO_CUDA_OK(cudaGraphGetNodes(g, nodes.data(), &nn));
+      LIO_CUDA_OK(cudaGraphGetNodes(e->sgraph, nodes.data(), &nn));
       e->asm_nodes.clear();
       for (cudaGraphNode_t nd : nodes) if (asm_is_graph_node(nd)) e->asm_nodes.push_back(nd);
       if ((int)e->asm_nodes.size() != nevals) { lio_set_last_error(__FILE__, __LINE__, "solver graph: unexpected node count"); return LIO_ERR_CUDA; }

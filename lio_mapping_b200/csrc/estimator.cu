@@ -90,44 +90,9 @@ extern "C" void lio_est_default_config(lio_est_config *c) {
   c->init_window_factor = 1;
 }
 
-void PeerExchange::release() {
-  if (xbuf) cudaFree(xbuf);
-  if (fslab) cudaFree(fslab);
-  *this = PeerExchange();
-}
-
 extern "C" int lio_est_destroy(lio_est *e) {
   if (!e) return LIO_OK;
-  if (e->mjob.running) { e->worker.wait(); e->mjob.running = false; }
-  cudaSetDevice(e->device);
-  e->map.release();
-  for (float4 *p : e->slot_ptr) if (p) cudaFree(p);
-  for (FeatureOut &f : e->feats) if (f.src) cudaFree(f.src);
-  void *ptrs[] = {e->d_slot_n, e->d_own_n, e->d_scan, e->d_local, e->d_map, e->d_tmp, e->d_counts, e->d_tf, e->d_odom, e->d_odom_partial};
-  for (void *p : ptrs) if (p) cudaFree(p);
-  for (int k = 0; k < 48; ++k) if (e->evp[k]) cudaEventDestroy(e->evp[k]);
-  e->ds.destroy();
-  if (e->sexec) cudaGraphExecDestroy(e->sexec);
-  if (e->sgraph) cudaGraphDestroy(e->sgraph);
-  if (e->gstream) cudaStreamDestroy(e->gstream);
-  if (e->ev_gin) cudaEventDestroy(e->ev_gin);
-  if (e->ev_gout) cudaEventDestroy(e->ev_gout);
-  if (e->ev0) cudaEventDestroy(e->ev0);
-  if (e->ev1) cudaEventDestroy(e->ev1);
-  if (e->evk0) cudaEventDestroy(e->evk0);
-  if (e->evk1) cudaEventDestroy(e->evk1);
-  e->px.release();
-  if (e->h_tf) cudaFreeHost(e->h_tf);
-  if (e->h_S) cudaFreeHost(e->h_S);
-  if (e->h_Rt) cudaFreeHost(e->h_Rt);
-  if (e->d_Rt) cudaFree(e->d_Rt);
-  if (e->h_counts) cudaFreeHost(e->h_counts);
-  e->vg.destroy(); e->hash.destroy(); e->knn.destroy(); e->knn2.destroy(); e->asmw.destroy();
-  if (e->ostream) cudaStreamDestroy(e->ostream);
-  if (e->ev_map) cudaEventDestroy(e->ev_map);
-  if (e->ev_odom) cudaEventDestroy(e->ev_odom);
-  e->lc.release();
-  e->mapping.release();
+  cudaSetDevice(e->device);   // the resources belong to the context's device, whichever is current
   delete e;
   return LIO_OK;
 }
@@ -142,7 +107,7 @@ extern "C" int lio_est_create(const lio_est_config *cfg, int device, void *cuda_
   }
   if (lio_device_count() <= 0) return LIO_ERR_NO_DEVICE;
   LIO_CUDA_OK(cudaSetDevice(device));
-  lio_est *e = new (std::nothrow) lio_est();
+  std::unique_ptr<lio_est> e(new (std::nothrow) lio_est());
   if (!e) return LIO_ERR_INVALID;
   e->cfg = *cfg; e->W = W; e->O = O; e->device = device; e->stream = (cudaStream_t)cuda_stream;
   cudaDeviceGetAttribute(&e->sm_count, cudaDevAttrMultiProcessorCount, device);
@@ -160,39 +125,27 @@ extern "C" int lio_est_create(const lio_est_config *cfg, int device, void *cuda_
   e->local_tf.assign(W + 1, TransformF{0, 0, 0, 1, 0, 0, 0});
   const int pivot = W - O;
   e->slot_cap = cfg->max_frame_points * (pivot + 1);
-  e->slot_ptr.assign(W + 1, nullptr);
+  e->slot_ptr.resize(W + 1);
   e->slot_of.resize(W + 1);
   bool ok = true;
   for (int k = 0; k <= W; ++k) {
     e->slot_of[k] = k;
-    ok = ok && cudaMalloc(&e->slot_ptr[k], sizeof(float4) * e->slot_cap) == cudaSuccess;
+    ok = ok && alloc(e->slot_ptr[k], e->slot_cap);
   }
   e->local_cap = e->slot_cap + cfg->max_frame_points * (O > 1 ? O - 1 : 1);
-  ok = ok && cudaMalloc(&e->d_slot_n, sizeof(int) * (W + 1)) == cudaSuccess;
-  ok = ok && cudaMalloc(&e->d_own_n, sizeof(int) * (W + 1)) == cudaSuccess;
-  ok = ok && cudaMalloc(&e->d_scan, sizeof(float4) * cfg->max_scan_points) == cudaSuccess;
-  ok = ok && cudaMalloc(&e->d_local, sizeof(float4) * e->local_cap) == cudaSuccess;
-  ok = ok && cudaMalloc(&e->d_map, sizeof(float4) * e->local_cap) == cudaSuccess;
-  ok = ok && cudaMalloc(&e->d_tmp, sizeof(float4) * e->slot_cap) == cudaSuccess;
-  ok = ok && cudaMalloc(&e->d_counts, sizeof(int) * 8) == cudaSuccess;
-  ok = ok && cudaMalloc(&e->d_tf, sizeof(TransformF) * (W + 1)) == cudaSuccess;
-  ok = ok && cudaMalloc(&e->d_odom, sizeof(OdomState)) == cudaSuccess;
-  ok = ok && cudaMalloc(&e->d_odom_partial, sizeof(double) * 32 * 1024) == cudaSuccess;
-  ok = ok && cudaMallocHost((void **)&e->h_tf, sizeof(TransformF) * (W + 1)) == cudaSuccess;
-  ok = ok && cudaMallocHost((void **)&e->h_S, sizeof(double) * kMaxOpt * kAsmStride) == cudaSuccess;
-  ok = ok && cudaMallocHost((void **)&e->h_Rt, sizeof(double) * kMaxOpt * kAsmRtStride) == cudaSuccess;
-  ok = ok && cudaMalloc(&e->d_Rt, sizeof(double) * kMaxOpt * kAsmRtStride) == cudaSuccess;
-  ok = ok && cudaMallocHost((void **)&e->h_counts, sizeof(int) * (W + 16)) == cudaSuccess;
+  ok = ok && alloc(e->d_slot_n, W + 1) && alloc(e->d_own_n, W + 1) && alloc(e->d_scan, cfg->max_scan_points) && alloc(e->d_local, e->local_cap) &&
+       alloc(e->d_map, e->local_cap) && alloc(e->d_tmp, e->slot_cap) && alloc(e->d_counts, 8) && alloc(e->d_tf, W + 1) && alloc(e->d_odom, 1) &&
+       alloc(e->d_odom_partial, 32 * 1024) && alloc_host(e->h_tf, W + 1) && alloc_host(e->h_S, kMaxOpt * kAsmStride) &&
+       alloc_host(e->h_Rt, kMaxOpt * kAsmRtStride) && alloc(e->d_Rt, kMaxOpt * kAsmRtStride) && alloc_host(e->h_counts, W + 16);
   if (ok) { std::memset(e->h_counts, 0, sizeof(int) * (W + 16)); e->h_xerr = e->h_counts + W + 10; }
   int vg_cap = std::max(e->local_cap, cfg->max_scan_points);
   ok = ok && e->vg.init(vg_cap) == 0;
   ok = ok && e->hash.init(e->local_cap) == 0;
   ok = ok && e->knn.init(cfg->max_frame_points * (O + 1)) == 0;
   ok = ok && e->knn2.init(cfg->max_frame_points) == 0;
-  ok = ok && cudaStreamCreateWithFlags(&e->ostream, cudaStreamNonBlocking) == cudaSuccess;
-  ok = ok && cudaEventCreateWithFlags(&e->ev_map, cudaEventDisableTiming) == cudaSuccess;
-  ok = ok && cudaEventCreateWithFlags(&e->ev_odom, cudaEventDisableTiming) == cudaSuccess;
+  ok = ok && create(e->ostream) && create(e->ev_map) && create(e->ev_odom);
   e->feats.assign(W + 1, FeatureOut());
+  e->feat_src.resize(W + 1);
   long long total_feat = 0;
   {
     e->px.foff_pts.assign(W + 1, 0); e->px.foff_coef.assign(W + 1, 0);
@@ -208,33 +161,27 @@ extern "C" int lio_est_create(const lio_est_config *cfg, int device, void *cuda_
     e->px.fpar_stride = off;
     e->px.foff_flags = 2 * off;
     e->px.fslab_bytes = 2 * off + 256;   // epoch flags (one per source rank) + error word behind the two parities
-    ok = ok && cudaMalloc(&e->px.fslab, e->px.fslab_bytes) == cudaSuccess && cudaMemset(e->px.fslab, 0, e->px.fslab_bytes) == cudaSuccess;
-    for (int k = pivot + 1; k <= W && ok; ++k) ok = ok && cudaMalloc(&e->feats[k].src, sizeof(int) * e->feats[k].cap) == cudaSuccess;
-    if (ok) set_feature_parity(e, 0);
+    ok = ok && alloc(e->px.fslab, e->px.fslab_bytes) && cudaMemset(e->px.fslab, 0, e->px.fslab_bytes) == cudaSuccess;
+    for (int k = pivot + 1; k <= W && ok; ++k) {
+      ok = alloc(e->feat_src[k], e->feats[k].cap);
+      e->feats[k].src = e->feat_src[k];
+    }
+    if (ok) set_feature_parity(e.get(), 0);
   }
-  ok = ok && e->asmw.init((int)std::min<long long>(total_feat, 1ll << 30)) == 0;
-  if (ok) {
-    ok = ok && cudaMemset(e->d_slot_n, 0, sizeof(int) * (W + 1)) == cudaSuccess;
-    ok = ok && cudaMemset(e->d_own_n, 0, sizeof(int) * (W + 1)) == cudaSuccess;
-    ok = ok && cudaMemset(e->d_counts, 0, sizeof(int) * 8) == cudaSuccess;
-  }
-  ok = ok && cudaEventCreate(&e->ev0) == cudaSuccess && cudaEventCreate(&e->ev1) == cudaSuccess;
-  ok = ok && cudaEventCreate(&e->evk0) == cudaSuccess && cudaEventCreate(&e->evk1) == cudaSuccess;
-  ok = ok && cudaMalloc(&e->px.xbuf, kXBytes) == cudaSuccess && cudaMemset(e->px.xbuf, 0, kXBytes) == cudaSuccess;
-  for (int k = 0; k < 48 && ok; ++k) ok = ok && cudaEventCreate(&e->evp[k]) == cudaSuccess;
+  ok = ok && e->asmw.init((int)std::min<long long>(total_feat, 1ll << 30)) == 0 && cudaMemset(e->d_slot_n, 0, sizeof(int) * (W + 1)) == cudaSuccess &&
+       cudaMemset(e->d_own_n, 0, sizeof(int) * (W + 1)) == cudaSuccess && cudaMemset(e->d_counts, 0, sizeof(int) * 8) == cudaSuccess;
+  ok = ok && create(e->ev0, cudaEventDefault) && create(e->ev1, cudaEventDefault) && create(e->evk0, cudaEventDefault) &&
+       create(e->evk1, cudaEventDefault);
+  ok = ok && alloc(e->px.xbuf, kXBytes) && cudaMemset(e->px.xbuf, 0, kXBytes) == cudaSuccess;
+  for (int k = 0; k < 48 && ok; ++k) ok = create(e->evp[k], cudaEventDefault);
   e->use_dev_solver = cfg->device_solver != 0 && e->ds.supports(O) && cfg->max_num_iterations <= 22;
   if (e->use_dev_solver) ok = ok && e->ds.init(O) == 0;
-  if (e->use_dev_solver && cfg->solver_graph) {
-    ok = ok && cudaStreamCreateWithFlags(&e->gstream, cudaStreamNonBlocking) == cudaSuccess;
-    ok = ok && cudaEventCreateWithFlags(&e->ev_gin, cudaEventDisableTiming) == cudaSuccess;
-    ok = ok && cudaEventCreateWithFlags(&e->ev_gout, cudaEventDisableTiming) == cudaSuccess;
-  }
+  if (e->use_dev_solver && cfg->solver_graph) ok = ok && create(e->gstream) && create(e->ev_gin) && create(e->ev_gout);
   if (!ok) {
     lio_set_last_error(__FILE__, __LINE__, "lio_est_create: device allocation failed");
-    lio_est_destroy(e);
     return LIO_ERR_CUDA;
   }
-  *out = e;
+  *out = e.release();
   return LIO_OK;
 }
 
@@ -828,7 +775,7 @@ extern "C" int lio_est_solver_trace(lio_est *e, long long *out, int cap) {
   if (!e || !out || cap < 24 * 16 + 4 * 28 + 4) return LIO_ERR_INVALID;
   if (!e->use_dev_solver) { std::memset(out, 0, sizeof(long long) * (24 * 16 + 4 * 28 + 4)); return LIO_OK; }
   LIO_CUDA_OK(cudaSetDevice(e->device));
-  LIO_CUDA_OK(cudaMemcpy(out, reinterpret_cast<const char *>(e->ds.st) + offsetof(DevSolveState, dbg), sizeof(long long) * (24 * 16 + 4 * 28 + 4), cudaMemcpyDeviceToHost));
+  LIO_CUDA_OK(cudaMemcpy(out, reinterpret_cast<const char *>(e->ds.st.get()) + offsetof(DevSolveState, dbg), sizeof(long long) * (24 * 16 + 4 * 28 + 4), cudaMemcpyDeviceToHost));
   return LIO_OK;
 }
 

@@ -133,8 +133,8 @@ struct Worker {
   }
 };
 
-// ---- the optional parts of a context: each is off until its enable / attach call succeeds, and release() returns it to that state
-// (lio_est_destroy, and the enable / attach call that failed half-way)
+// ---- the optional parts of a context: each is off until its enable / attach call succeeds.  The call builds the part in a local and
+// moves it in on success, so a call that fails half-way leaves the context as it was.
 
 // /local/* publication (lio_est_enable_local_clouds): corner_stack_ / full_stack_ beside the surf slots.  The per-frame work runs on
 // `stream`, forked from the scan's stream after the surf push and joined before SlideWindow.
@@ -142,17 +142,16 @@ struct LocalClouds {
   bool on = false, staged = false, pending = false;
   float corner_leaf = 0.2f;
   int cap[2] = {0, 0};             // corner, full points per slot (and per staged cloud)
-  std::vector<float4 *> slot[2];   // physical slots [corner / full][slot], rotated through slot_of with the surf slots
-  int *d_slot_n = nullptr;         // [0, W] corner counts per physical slot, [W + 1, 2W + 1] full counts
-  float4 *d_stage[2] = {nullptr, nullptr};   // staged corner / full cloud of the next push
-  int *d_stage_n = nullptr;        // [2]
-  float4 *d_pub[3] = {nullptr, nullptr, nullptr};   // published corner / surf / full of frame W - O (lio_mb_* argument order)
-  int *d_pub_n = nullptr;          // [3]
+  std::vector<DevMem<float4>> slot[2];   // physical slots [corner / full][slot], rotated through slot_of with the surf slots
+  DevMem<int> d_slot_n;            // [0, W] corner counts per physical slot, [W + 1, 2W + 1] full counts
+  DevMem<float4> d_stage[2];       // staged corner / full cloud of the next push
+  DevMem<int> d_stage_n;           // [2]
+  DevMem<float4> d_pub[3];         // published corner / surf / full of frame W - O (lio_mb_* argument order)
+  DevMem<int> d_pub_n;             // [3]
   int pub_cap[3] = {0, 0, 0};
   VoxelGrid vg;                    // down_size_filter_corner_ (its own workspace: it runs beside the surf filter)
-  cudaStream_t stream = nullptr;
-  cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
-  void release();
+  Stream stream;
+  Event ev_fork, ev_join;
 };
 
 // The global cube map after initialisation (lio_est_attach_map / lio_est_attach_mapping): the PointMapping the reference's Estimator
@@ -161,12 +160,12 @@ struct AttachedMap {
   lio_pm *pm = nullptr;
   int scans = 0;                   // INITED scans since the attach: opt_point_coeff_mask_.first() is false from scan O on
   bool pending = false;
-  float4 *d_keep[2] = {nullptr, nullptr};   // W == O with de-skew: the previous frame's corner / surf cloud, kept until its insert
-  int *d_keep_n = nullptr;         // [2]
-  cudaEvent_t ev_in = nullptr, ev_done = nullptr;
+  DevMem<float4> d_keep[2];        // W == O with de-skew: the previous frame's corner / surf cloud, kept until its insert
+  DevMem<int> d_keep_n;            // [2]
+  Event ev_in, ev_done;
   lio::TwistF insert;              // opt_transforms_.first() of the last insert
   int info[4] = {0, 0, 0, 0};      // inserted, points inserted, surround published, last surround size
-  void release();                  // waits for the pending map work, then detaches the handle
+  void detach();                   // waits for the pending map work, then detaches the handle (the map is not owned)
 };
 
 // imu_factor = 0 from the odometry's clouds (lio_est_attach_mapping): the estimator's own PointMapping::Process on every message,
@@ -187,7 +186,6 @@ struct Mapping {
   bool attempted = false;             // the last message ran an attempt
   M3 R_WI = M3::I();                  // R_WI_
   std::vector<double> attempt_states; // (W+1) x 16 (lio_est_get_states layout) as the last attempt left them, before any solve
-  void release() { *this = Mapping(); }
 };
 
 // estimate_extrinsic = 2 on an IMU mapping (lio_est_enable_extrinsic_calibration): EstimateExtrinsicRotation before RunInitialization
@@ -210,18 +208,17 @@ constexpr size_t kXErrOff = kXFlagOff + sizeof(unsigned) * kMaxPeers;
 constexpr size_t kXBytes = kXErrOff + 64;
 
 struct PeerExchange {
-  char *xbuf = nullptr;
+  DevMem<char> xbuf;
   char *peer_base[kMaxPeers] = {};
   int npeers = 0;
   unsigned xepoch = 0;
-  char *fslab = nullptr;
+  DevMem<char> fslab;
   size_t fslab_bytes = 0, fpar_stride = 0, foff_cnt = 0, foff_flags = 0;
   std::vector<size_t> foff_pts, foff_coef;
   bool fpeers = false;
   char *fpeer_base[kMaxPeers] = {};
   unsigned fepoch = 0;
   int fparity = 0;
-  void release();
 };
 
 struct lio_est {
@@ -258,33 +255,34 @@ struct lio_est {
   bool ex_constant = false;
   ExtrinsicCalib calib;
   // ---- device
-  std::vector<float4 *> slot_ptr;    // physical slots
+  std::vector<DevMem<float4>> slot_ptr;   // physical slots
   std::vector<int> slot_of;          // logical frame -> physical slot
-  int *d_slot_n = nullptr;           // counts per physical slot
+  DevMem<int> d_slot_n;              // counts per physical slot
   std::vector<int> size_surf_stack;  // host mirror of each frame's own size (logical)
-  int *d_own_n = nullptr;            // device: own size per physical slot (for SlideWindow's skip)
+  DevMem<int> d_own_n;               // device: own size per physical slot (for SlideWindow's skip)
   int slot_cap = 0;
-  float4 *d_scan = nullptr, *d_local = nullptr, *d_map = nullptr, *d_tmp = nullptr;
+  DevMem<float4> d_scan, d_local, d_map, d_tmp;
   int local_cap = 0;
-  int *d_counts = nullptr;  // [0] scan n [1] local n [2] map n [3] tmp n
+  DevMem<int> d_counts;     // [0] scan n [1] local n [2] map n [3] tmp n
   VoxelGrid vg;
   CellHash hash;
   KnnWork knn;
   KnnWork knn2;                     // launch state of the LaserOdom chain, which runs beside the frame-batched k-NN launch
-  cudaStream_t ostream = nullptr;   // stream of that chain
-  cudaEvent_t ev_map = nullptr, ev_odom = nullptr;
-  std::vector<FeatureOut> feats;  // logical frame index
+  Stream ostream;                   // stream of that chain
+  Event ev_map, ev_odom;
+  std::vector<FeatureOut> feats;  // logical frame index: pts / coef / count in the feature slab, src in feat_src
+  std::vector<DevMem<int>> feat_src;
   int *d_feat_counts = nullptr;   // W+1 (inside the feature slab, current parity)
-  TransformF *d_tf = nullptr;     // W+1
-  TransformF *h_tf = nullptr;     // pinned
+  DevMem<TransformF> d_tf;        // W+1
+  HostMem<TransformF> h_tf;       // pinned
   AsmWork asmw;
-  double *h_Rt = nullptr;   // pinned kMaxOpt*kAsmRtStride
-  double *d_Rt = nullptr;
-  double *h_S = nullptr;    // pinned kMaxOpt*kAsmStride
-  int *h_counts = nullptr;  // pinned
+  HostMem<double> h_Rt;     // pinned kMaxOpt*kAsmRtStride
+  DevMem<double> d_Rt;
+  HostMem<double> h_S;      // pinned kMaxOpt*kAsmStride
+  HostMem<int> h_counts;    // pinned
   int *h_xerr = nullptr;    // h_counts + W + 10: the rows exchange's bounded-wait error word (the feature exchange's is W + 9)
-  OdomState *d_odom = nullptr;
-  double *d_odom_partial = nullptr;
+  DevMem<OdomState> d_odom;
+  DevMem<double> d_odom_partial;
   // ---- sharding
   int rank = 0, world = 1;
   lio_allreduce_fn allreduce = nullptr;
@@ -310,20 +308,20 @@ struct lio_est {
   DevSolver ds;
   bool use_dev_solver = false;
   // the device solver's launches of one solve, captured once and replayed (single-GPU contexts)
-  cudaStream_t gstream = nullptr;
-  cudaGraph_t sgraph = nullptr;
-  cudaGraphExec_t sexec = nullptr;
-  std::vector<cudaGraphNode_t> asm_nodes;
-  cudaEvent_t ev_gin = nullptr, ev_gout = nullptr;
+  Stream gstream;
+  Graph sgraph;
+  GraphExec sexec;                    // declared after sgraph, so destroyed before it
+  std::vector<cudaGraphNode_t> asm_nodes;   // nodes of sgraph, re-parameterised on sexec every scan
+  Event ev_gin, ev_gout;
   int graph_launches = 0;
   bool prior_uploaded = false;
   bool ds_prepared = false, ds_prepared_asm = false;   // solve_dev_prepare ran for the current parameters
   int ds_prepared_it = 0;
-  cudaEvent_t evp[2 * 24] = {};
+  Event evp[2 * 24];
   // cached lidar reduction for the current parameter values
   bool S_valid = false;
   // CUDA-event timing of the fused kernel (on the launching stream)
-  cudaEvent_t ev0 = nullptr, ev1 = nullptr, evk0 = nullptr, evk1 = nullptr;
+  Event ev0, ev1, evk0, evk1;
   double knn_ms_sum = 0;
   long long knn_launch_count = 0, knn_query_sum = 0;
   bool knn_timed = false;
@@ -335,6 +333,14 @@ struct lio_est {
   LocalClouds lc;
   AttachedMap map;
   Mapping mapping;
+  // The members go in reverse declaration order once these waits are done.  The running marginalisation job is joined first.  The
+  // attached map's pending insert reads the estimator's slots and the map is not owned: it is waited for and the map detached before
+  // any slot is freed.  The local clouds' stream is drained before its buffers and the slots it reads go.
+  ~lio_est() {
+    if (mjob.running) worker.wait();
+    map.detach();
+    if (lc.stream) cudaStreamSynchronize(lc.stream);
+  }
 };
 
 

@@ -103,20 +103,10 @@ int CellHash::init(int cap) {
   while (table_size < 2 * cap) table_size <<= 1;
   eff_size = table_size;
   int ntiles = table_size / (kHashThreads * kScanPer) + 1;
-  if (cudaMalloc(&keys, sizeof(unsigned long long) * table_size) != cudaSuccess) return -1;
-  if (cudaMalloc(&count, sizeof(int) * table_size) != cudaSuccess) return -1;
-  if (cudaMalloc(&start, sizeof(int) * table_size) != cudaSuccess) return -1;
-  if (cudaMalloc(&slot_of, sizeof(int) * cap) != cudaSuccess) return -1;
-  if (cudaMalloc(&rank_of, sizeof(int) * cap) != cudaSuccess) return -1;
-  if (cudaMalloc(&cellpts, sizeof(float4) * cap) != cudaSuccess) return -1;
-  if (cudaMalloc(&status, sizeof(unsigned long long) * ntiles) != cudaSuccess) return -1;
-  if (cudaMalloc(&ticket, sizeof(int)) != cudaSuccess) return -1;
-  return 0;
-}
-void CellHash::destroy() {
-  void *p[] = {keys, count, start, slot_of, rank_of, cellpts, status, ticket};
-  for (void *q : p) if (q) cudaFree(q);
-  keys = nullptr; count = start = slot_of = rank_of = ticket = nullptr; cellpts = nullptr; status = nullptr;
+  return alloc(keys, table_size) && alloc(count, table_size) && alloc(start, table_size) && alloc(slot_of, cap) && alloc(rank_of, cap) &&
+                 alloc(cellpts, cap) && alloc(status, ntiles) && alloc(ticket, 1)
+             ? 0
+             : -1;
 }
 
 int CellHash::build(const float4 *map, const int *n_dev, int n_max, float cell_size, cudaStream_t st, int *launches) {
@@ -493,14 +483,7 @@ knn_plane(const KnnBatch B, const unsigned long long *__restrict__ hkeys, const 
 
 int KnnWork::init(int max_queries_total) {
   ntiles_max = (max_queries_total + kQueriesPerBlock - 1) / kQueriesPerBlock + kMaxKnnFrames + 1;
-  if (cudaMalloc(&status, sizeof(unsigned long long) * ntiles_max) != cudaSuccess) return -1;
-  if (cudaMalloc(&ticket, sizeof(int)) != cudaSuccess) return -1;
-  return 0;
-}
-void KnnWork::destroy() {
-  if (status) cudaFree(status);
-  if (ticket) cudaFree(ticket);
-  status = nullptr; ticket = nullptr;
+  return alloc(status, ntiles_max) && alloc(ticket, 1) ? 0 : -1;
 }
 
 void knn_plan(KnnBatch &b) {
@@ -607,8 +590,6 @@ static int features_batch_host(const float *map, int K, float cell_size, float m
     rc = LIO_ERR_CUDA;
   if (rc == LIO_OK)
     for (int k = 0; k < nframes; ++k) count_per_frame[k] = hn[3 + 2 * k];
-  h.destroy();
-  w.destroy();
   return rc;
 }
 
@@ -670,7 +651,6 @@ extern "C" int lio_cell_hash_build_host(const float *map, int n, int n_max, int 
         !d.down((float4 *)cellpts, h.cellpts, n))
       rc = LIO_ERR_CUDA;
   }
-  h.destroy();
   return rc;
 }
 

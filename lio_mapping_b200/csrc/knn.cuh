@@ -13,15 +13,14 @@ struct CellHash {
   int eff_size = 0;    // slots in use by the current build: the power of two >= 2 x its point bound (<= table_size)
   int cap_points = 0;
   float cell = 1.0f, inv_cell = 1.0f;
-  unsigned long long *keys = nullptr;  // [table_size], ~0 = empty
-  int *count = nullptr;                // [table_size]
-  int *start = nullptr;                // [table_size]
-  int *slot_of = nullptr, *rank_of = nullptr;  // [cap_points]
-  float4 *cellpts = nullptr;           // [cap_points] xyz + bitcast(map index)
-  unsigned long long *status = nullptr;
-  int *ticket = nullptr;
+  DevMem<unsigned long long> keys;     // [table_size], ~0 = empty
+  DevMem<int> count;                   // [table_size]
+  DevMem<int> start;                   // [table_size]
+  DevMem<int> slot_of, rank_of;        // [cap_points]
+  DevMem<float4> cellpts;              // [cap_points] xyz + bitcast(map index)
+  DevMem<unsigned long long> status;
+  DevMem<int> ticket;
   int init(int cap_points);
-  void destroy();
   // Builds the hash over map[0..*n_dev): cells of edge `cell` (>= search radius).  n_max bounds *n_dev; the table, its
   // memsets and the scan are sized from n_max, so a tight bound (the caller usually knows one) keeps the build cheap.
   int build(const float4 *map, const int *n_dev, int n_max, float cell_size, cudaStream_t st, int *launches);
@@ -57,11 +56,10 @@ struct KnnBatch {
 };
 
 struct KnnWork {
-  unsigned long long *status = nullptr;
-  int *ticket = nullptr;
+  DevMem<unsigned long long> status;
+  DevMem<int> ticket;
   int ntiles_max = 0;
   int init(int max_queries_total);
-  void destroy();
 };
 
 // CalculateFeatures for several frames against the same map in ONE launch (tiles are dealt frame-major so each

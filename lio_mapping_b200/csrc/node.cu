@@ -19,8 +19,8 @@
 namespace {
 
 struct Slot {                 // one published /compact_data message waiting for its IMU
-  float4 *cloud[3] = {};      // /laser_cloud_corner_last, /laser_cloud_surf_last, the full cloud
-  int *d_n = nullptr;         // their device counts
+  lio::DevMem<float4> cloud[3];   // /laser_cloud_corner_last, /laser_cloud_surf_last, the full cloud
+  lio::DevMem<int> d_n;       // their device counts
   int n[3] = {};              // the same counts as the host knows them (the bounds handed on)
   float sum7[7] = {};         // transform_sum_
   double stamp = 0;           // header.stamp
@@ -37,6 +37,18 @@ struct DriveMap {             // an attached lio_rm and the /cloud_registered it
   int source;
 };
 
+// The sub-handles a node creates, destroyed through their own entries (each counts as one live resource)
+template <class T, int (*Destroy)(T *)> struct DestroyHandle { void operator()(T *h) const { Destroy(h); } };
+template <class T, int (*Destroy)(T *)> using SubHandle = lio::Own<T *, DestroyHandle<T, Destroy>>;
+
+// create(&h) of one sub-handle; the node owns it from here
+template <class T, class D, class F> int make(lio::Own<T *, D> &h, F create) {
+  T *p = nullptr;
+  const int rc = create(&p);
+  if (rc == LIO_OK) h.take(cudaSuccess, p, nullptr);
+  return rc;
+}
+
 }  // namespace
 
 struct lio_node {
@@ -44,13 +56,16 @@ struct lio_node {
   int device = 0;
   int sm_count = 132;
   cudaStream_t stream = nullptr;
-  lio_pp *pp = nullptr;
-  lio_po *po = nullptr;
-  lio_pm *pm = nullptr;
-  lio_est *est = nullptr;
-  float4 *d_in = nullptr;              // upload target of lio_node_push_sweep_host
-  uint16_t *d_rings = nullptr;
+  lio::DevMem<float4> d_in;            // upload target of lio_node_push_sweep_host
+  lio::DevMem<uint16_t> d_rings;
   std::vector<Slot> slots;
+  // The sub-handles go before the node's own buffers, in the order mb, est, pm, po, pp (reverse declaration order): the estimator
+  // detaches pm, so it goes before pm.
+  SubHandle<lio_pp, lio_pp_destroy> pp;
+  SubHandle<lio_po, lio_po_destroy> po;
+  SubHandle<lio_pm, lio_pm_destroy> pm;
+  SubHandle<lio_est, lio_est_destroy> est;
+  SubHandle<lio_pm, lio_pm_destroy> mb;   // lio_node_enable_map_builder
   std::vector<int> free_slots;
   lio::MeasurementPairing pairing{0};
   std::vector<lio::ImuMsg> list;
@@ -60,7 +75,6 @@ struct lio_node {
   bool odom_on = true, inited = false, poisoned = false;
   double last_stamp = -1;
   std::deque<double> headers;          // Headers_ (Estimator.cc:441): the stamps of the last W + 1 pushed messages
-  lio_pm *mb = nullptr;                // lio_node_enable_map_builder
   std::vector<MbRow> mb_rows;
   std::vector<DriveMap> maps;          // lio_node_attach_registered_map, in attach order
 };
@@ -72,23 +86,6 @@ static int check_rings(const lio_node *nd, bool has_rings, int n) {
   if (ring_sensor(nd) ? (has_rings || n == 0) : !has_rings) return LIO_OK;
   lio_set_last_error(__FILE__, __LINE__, "lio_node: rings are required with sensor_type 320 and refused otherwise");
   return LIO_ERR_INVALID;
-}
-
-static void node_free(lio_node *nd) {
-  if (!nd) return;
-  cudaSetDevice(nd->device);
-  if (nd->mb) lio_pm_destroy(nd->mb);
-  if (nd->est) lio_est_destroy(nd->est);   // releases the attached map first
-  if (nd->pm) lio_pm_destroy(nd->pm);
-  if (nd->po) lio_po_destroy(nd->po);
-  if (nd->pp) lio_pp_destroy(nd->pp);
-  for (Slot &s : nd->slots) {
-    for (float4 *c : s.cloud) if (c) cudaFree(c);
-    if (s.d_n) cudaFree(s.d_n);
-  }
-  if (nd->d_in) cudaFree(nd->d_in);
-  if (nd->d_rings) cudaFree(nd->d_rings);
-  delete nd;
 }
 
 extern "C" void lio_node_default_config(lio_node_config *c) {
@@ -119,14 +116,13 @@ extern "C" int lio_node_create(const lio_node_config *cfg, int device, void *cud
   }
   if (lio_device_count() <= 0) return LIO_ERR_NO_DEVICE;
   LIO_CUDA_OK(cudaSetDevice(device));
-  lio_node *nd = new (std::nothrow) lio_node();
+  std::unique_ptr<lio_node> nd(new (std::nothrow) lio_node());
   if (!nd) return LIO_ERR_INVALID;
   nd->cfg = *cfg;
   nd->device = device;
   nd->stream = (cudaStream_t)cuda_stream;
   cudaDeviceGetAttribute(&nd->sm_count, cudaDevAttrMultiProcessorCount, device);
   nd->pairing = lio::MeasurementPairing(cfg->msg_time_delay);
-  auto fail = [&](int rc) { node_free(nd); return rc; };
   // processor_node.cc:64-74: the sensor presets (320 = RS-32 with the ring field)
   lio_pp_config pc = cfg->pp;
   if (st == 16) { pc.lower_bound = -15.f; pc.upper_bound = 15.f; pc.num_rings = 16; }
@@ -136,36 +132,38 @@ extern "C" int lio_node_create(const lio_node_config *cfg, int device, void *cud
   const int F = cfg->max_feature_points, N = cfg->max_points;
   const lio_est_config &ec = cfg->est;
   int rc;
-  if ((rc = lio_pp_create(&pc, N, device, cuda_stream, &nd->pp)) != LIO_OK) return fail(rc);
+  if ((rc = make(nd->pp, [&](lio_pp **h) { return lio_pp_create(&pc, N, device, cuda_stream, h); })) != LIO_OK) return rc;
   // estimator_node.cc:145-147: PointOdometry(0.1, odom_io) with its default 25 iterations
-  if ((rc = lio_po_create(0.1f, cfg->odom_io, 25, F, N, device, cuda_stream, &nd->po)) != LIO_OK) return fail(rc);
+  if ((rc = make(nd->po, [&](lio_po **h) { return lio_po_create(0.1f, cfg->odom_io, 25, F, N, device, cuda_stream, h); })) != LIO_OK) return rc;
   // the Estimator is a PointMapping (num_max_iterations_ 10, PointMapping.h:171) with the YAML's leaves
-  if ((rc = lio_pm_create(F, cfg->corner_filter_size, cfg->surf_filter_size, ec.min_match_sq_dis, ec.min_plane_dis, 10, device, cuda_stream,
-                          &nd->pm)) != LIO_OK)
-    return fail(rc);
-  if ((rc = lio_pm_enable_publish(nd->pm, cfg->map_filter_size, N)) != LIO_OK) return fail(rc);
-  if ((rc = lio_est_create(&ec, device, cuda_stream, &nd->est)) != LIO_OK) return fail(rc);
-  if ((rc = lio_est_set_extrinsic(nd->est, cfg->tf_lb7)) != LIO_OK) return fail(rc);
-  if ((rc = lio_est_enable_local_clouds(nd->est, cfg->corner_filter_size, F, N)) != LIO_OK) return fail(rc);
-  if (ec.imu_factor && ec.estimate_extrinsic == 2 && (rc = lio_est_enable_extrinsic_calibration(nd->est)) != LIO_OK) return fail(rc);
+  if ((rc = make(nd->pm, [&](lio_pm **h) {
+         return lio_pm_create(F, cfg->corner_filter_size, cfg->surf_filter_size, ec.min_match_sq_dis, ec.min_plane_dis, 10, device, cuda_stream, h);
+       })) != LIO_OK)
+    return rc;
+  if ((rc = lio_pm_enable_publish(nd->pm, cfg->map_filter_size, N)) != LIO_OK) return rc;
+  if ((rc = make(nd->est, [&](lio_est **h) { return lio_est_create(&ec, device, cuda_stream, h); })) != LIO_OK) return rc;
+  if ((rc = lio_est_set_extrinsic(nd->est, cfg->tf_lb7)) != LIO_OK) return rc;
+  if ((rc = lio_est_enable_local_clouds(nd->est, cfg->corner_filter_size, F, N)) != LIO_OK) return rc;
+  if (ec.imu_factor && ec.estimate_extrinsic == 2 && (rc = lio_est_enable_extrinsic_calibration(nd->est)) != LIO_OK) return rc;
   rc = ec.imu_factor ? lio_est_attach_imu_mapping(nd->est, nd->pm) : lio_est_attach_mapping(nd->est, nd->pm);
-  if (rc != LIO_OK) return fail(rc);
+  if (rc != LIO_OK) return rc;
   nd->slots.resize(cfg->max_pending);
   for (int k = cfg->max_pending - 1; k >= 0; --k) {
     Slot &s = nd->slots[k];
-    if (cudaMalloc(&s.cloud[0], sizeof(float4) * F) != cudaSuccess || cudaMalloc(&s.cloud[1], sizeof(float4) * F) != cudaSuccess ||
-        cudaMalloc(&s.cloud[2], sizeof(float4) * N) != cudaSuccess || cudaMalloc(&s.d_n, sizeof(int) * 3) != cudaSuccess) {
+    if (!lio::alloc(s.cloud[0], F) || !lio::alloc(s.cloud[1], F) || !lio::alloc(s.cloud[2], N) || !lio::alloc(s.d_n, 3)) {
       lio_set_last_error(__FILE__, __LINE__, "lio_node_create: cudaMalloc of a queue slot failed");
-      return fail(LIO_ERR_CUDA);
+      return LIO_ERR_CUDA;
     }
     nd->free_slots.push_back(k);
   }
-  *out = nd;
+  *out = nd.release();
   return LIO_OK;
 }
 
 extern "C" int lio_node_destroy(lio_node *nd) {
-  node_free(nd);
+  if (!nd) return LIO_OK;
+  cudaSetDevice(nd->device);   // the buffers belong to the node's device, whichever is current
+  delete nd;
   return LIO_OK;
 }
 
@@ -210,7 +208,7 @@ static int process_message(lio_node *nd, const Slot &s) {
   const bool was_inited = nd->inited;
   for (const lio::ImuCall &c : nd->calls)
     if ((rc = lio_est_process_imu(nd->est, c.dt, c.acc, c.gyr, c.stamp)) != LIO_OK) break;
-  if (rc == LIO_OK) rc = lio_est_process_compact_stamped_dev(nd->est, (const float *)s.cloud[0], (const float *)s.cloud[1], (const float *)s.cloud[2],
+  if (rc == LIO_OK) rc = lio_est_process_compact_stamped_dev(nd->est, (const float *)s.cloud[0].get(), (const float *)s.cloud[1].get(), (const float *)s.cloud[2].get(),
                                                             s.d_n, s.n, s.sum7, s.stamp);
   int info[4] = {};
   if (rc == LIO_OK) rc = lio_est_compact_status(nd->est, info);
@@ -331,13 +329,13 @@ extern "C" int lio_node_push_sweep_host(lio_node *nd, const float *xyzi, const u
   if ((rc = refuse_poisoned(nd)) != LIO_OK) return rc;
   if (n > nd->cfg.max_points) return LIO_ERR_CAPACITY;
   LIO_CUDA_OK(cudaSetDevice(nd->device));
-  if (!nd->d_in) LIO_CUDA_OK(cudaMalloc(&nd->d_in, sizeof(float4) * nd->cfg.max_points));
-  if (rings && !nd->d_rings) LIO_CUDA_OK(cudaMalloc(&nd->d_rings, sizeof(uint16_t) * nd->cfg.max_points));
+  if (!nd->d_in && !lio::alloc(nd->d_in, nd->cfg.max_points)) return LIO_ERR_CUDA;
+  if (rings && !nd->d_rings && !lio::alloc(nd->d_rings, nd->cfg.max_points)) return LIO_ERR_CUDA;
   if (n > 0) {
     LIO_CUDA_OK(cudaMemcpyAsync(nd->d_in, xyzi, sizeof(float4) * n, cudaMemcpyHostToDevice, nd->stream));
     if (rings) LIO_CUDA_OK(cudaMemcpyAsync(nd->d_rings, rings, sizeof(uint16_t) * n, cudaMemcpyHostToDevice, nd->stream));
   }
-  rc = lio_node_push_sweep_dev(nd, (const float *)nd->d_in, rings ? nd->d_rings : nullptr, n, stamp);
+  rc = lio_node_push_sweep_dev(nd, (const float *)nd->d_in.get(), rings ? nd->d_rings.get() : nullptr, n, stamp);
   const cudaError_t e = cudaStreamSynchronize(nd->stream);   // the caller's buffers may be reused on return
   if (rc == LIO_OK && e != cudaSuccess) { lio_set_last_error(__FILE__, __LINE__, cudaGetErrorString(e)); return LIO_ERR_CUDA; }
   return rc;
@@ -379,7 +377,7 @@ extern "C" int lio_node_enable_map_builder(lio_node *nd, const lio_mb_config *cf
   int rc = lio_est_local_clouds_dev(nd->est, ptr, &n_dev, n_host);
   if (rc != LIO_OK) return rc;
   LIO_CUDA_OK(cudaSetDevice(nd->device));
-  return lio_mb_create(cfg, std::max(n_host[0], n_host[1]), n_host[2], nd->device, nd->stream, &nd->mb);
+  return make(nd->mb, [&](lio_pm **h) { return lio_mb_create(cfg, std::max(n_host[0], n_host[1]), n_host[2], nd->device, nd->stream, h); });
 }
 
 extern "C" int lio_node_map_builder(lio_node *nd, lio_pm **mb) {

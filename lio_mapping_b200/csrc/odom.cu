@@ -198,21 +198,13 @@ int odom_rounds(const CellHash &h, const float4 *surf, const int *n_dev, int n_b
 int ScanToMapWork::init(int cap_corner_map, int cap_surf_map, int cap_queries) {
   cap_feat = cap_queries > 0 ? cap_queries : 1;
   if (hc.init(cap_corner_map > 0 ? cap_corner_map : 1) != 0 || hs.init(cap_surf_map > 0 ? cap_surf_map : 1) != 0 || w.init(cap_feat + 1) != 0) return -1;
-  auto alloc = [](void **p, size_t bytes) { return cudaMalloc(p, bytes ? bytes : 16) == cudaSuccess; };
-  if (!(alloc((void **)&fo.pts, sizeof(float4) * cap_feat) && alloc((void **)&fo.coef, sizeof(float4) * cap_feat) &&
-        alloc((void **)&fo.src, sizeof(int) * cap_feat) && alloc((void **)&d_n, sizeof(int) * 8) && alloc((void **)&d_tf, sizeof(TransformF)) &&
-        alloc((void **)&d_odom, sizeof(OdomState)) && alloc((void **)&d_partial, sizeof(double) * 32 * 1024) && alloc((void **)&d_z, sizeof(float) * 4)))
+  if (!(alloc(d_fpts, cap_feat) && alloc(d_fcoef, cap_feat) && alloc(d_fsrc, cap_feat) && alloc(d_n, 8) && alloc(d_tf, 1) && alloc(d_odom, 1) &&
+        alloc(d_partial, 32 * 1024) && alloc(d_z, 4)))
     return -1;
+  fo.pts = d_fpts; fo.coef = d_fcoef; fo.src = d_fsrc;
   fo.cap = cap_feat;
   fo.count = d_n + 4;
   return 0;
-}
-
-void ScanToMapWork::destroy() {
-  void *fr[] = {fo.pts, fo.coef, fo.src, d_n, d_tf, d_odom, d_partial, d_z};
-  for (void *q : fr) if (q) cudaFree(q);
-  hc.destroy(); hs.destroy(); w.destroy();
-  fo = FeatureOut(); d_n = nullptr; d_tf = nullptr; d_odom = nullptr; d_partial = nullptr; d_z = nullptr;
 }
 
 // Maps and stacks are device arrays; Kc / Ks are known on the host (the caller assembled the maps), the stack sizes are
@@ -304,7 +296,6 @@ extern "C" int lio_scan_to_map_host(const float *corner_map, int Kc, const float
     if ((pts4 && !d.down((float4 *)pts4, W.fo.pts, m)) || (coef4 && !d.down((float4 *)coef4, W.fo.coef, m)) || (src && !d.down(src, W.fo.src, m)))
       rc = LIO_ERR_CUDA;
   }
-  W.destroy();
   return rc;
 }
 
@@ -357,8 +348,6 @@ extern "C" int lio_laser_odom_host(const float *map, int K, const float *surf, i
     if ((pts4 && !d.down((float4 *)pts4, fo.pts, m)) || (coef4 && !d.down((float4 *)coef4, fo.coef, m)) || (src && !d.down(src, fo.src, m)))
       rc = LIO_ERR_CUDA;
   }
-  h.destroy();
-  w.destroy();
   return rc;
 }
 

@@ -22,15 +22,16 @@ struct OdomState {
 struct ScanToMapWork {
   CellHash hc, hs;
   KnnWork w;
-  FeatureOut fo;
-  int *d_n = nullptr;          // [0] Kc [1] Ks [4] feature count
-  TransformF *d_tf = nullptr;
-  OdomState *d_odom = nullptr;
-  double *d_partial = nullptr;
-  float *d_z = nullptr;
+  DevMem<float4> d_fpts, d_fcoef;
+  DevMem<int> d_fsrc;
+  FeatureOut fo;               // view of d_fpts / d_fcoef / d_fsrc and the count d_n[4]
+  DevMem<int> d_n;             // [0] Kc [1] Ks [4] feature count
+  DevMem<TransformF> d_tf;
+  DevMem<OdomState> d_odom;
+  DevMem<double> d_partial;
+  DevMem<float> d_z;
   int cap_feat = 0;
   int init(int cap_corner_map, int cap_surf_map, int cap_queries);
-  void destroy();
 };
 int scan_to_map_run(ScanToMapWork &W, const float4 *d_cmap, int Kc, const float4 *d_smap, int Ks, const float4 *d_corner, const int *d_nc,
                     int Mc_max, const float4 *d_surf, const int *d_ns, int Ms_max, float *tf7, float min_match_sq_dis, float min_plane_dis,

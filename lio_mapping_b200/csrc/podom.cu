@@ -23,6 +23,7 @@
 #include <cmath>
 #include <cstdio>
 #include <cstring>
+#include <memory>
 #include <new>
 #include "odom.cuh"
 #include "twistf.h"
@@ -343,15 +344,14 @@ struct lio_po {
   int cap_feat = 0, cap_full = 0;
   bool system_inited = false, enable_odom = true;
   long frame_count = 0;
-  float4 *d_sharp = nullptr, *d_flat = nullptr, *d_less_sharp = nullptr, *d_less_flat = nullptr, *d_last_corner = nullptr, *d_last_surf = nullptr,
-         *d_full = nullptr;
+  DevMem<float4> d_sharp, d_flat, d_less_sharp, d_less_flat, d_last_corner, d_last_surf, d_full;
   int n_sharp = 0, n_flat = 0, n_less_sharp = 0, n_less_flat = 0, n_last_corner = 0, n_last_surf = 0, n_full = 0;
-  int *d_idx_c = nullptr, *d_idx_s = nullptr, *d_nsel = nullptr;
-  int *d_cnt = nullptr;                // lio_po_process_dev: [0..4] clamped input counts, [5] a count over its bound
+  DevMem<int> d_idx_c, d_idx_s, d_nsel;
+  DevMem<int> d_cnt;                   // lio_po_process_dev: [0..4] clamped input counts, [5] a count over its bound
   int h_cnt[6] = {};                   // their read-back
-  int *d_pub_n = nullptr;              // counts of the published clouds {last_corner, last_surf, full} (lio_po_clouds_dev)
-  TransformF *d_tf = nullptr;
-  OdomState *d_odom = nullptr;
+  DevMem<int> d_pub_n;                 // counts of the published clouds {last_corner, last_surf, full} (lio_po_clouds_dev)
+  DevMem<TransformF> d_tf;
+  DevMem<OdomState> d_odom;
   TwistF es, sum;
   int published = 0;
   int launches = 0;
@@ -359,10 +359,7 @@ struct lio_po {
 
 extern "C" int lio_po_destroy(lio_po *p) {
   if (!p) return LIO_OK;
-  cudaSetDevice(p->device);
-  void *fr[] = {p->d_sharp, p->d_flat, p->d_less_sharp, p->d_less_flat, p->d_last_corner, p->d_last_surf, p->d_full, p->d_idx_c, p->d_idx_s,
-                p->d_nsel, p->d_cnt, p->d_pub_n, p->d_tf, p->d_odom};
-  for (void *q : fr) if (q) cudaFree(q);
+  cudaSetDevice(p->device);   // the buffers belong to the handle's device, whichever is current
   delete p;
   return LIO_OK;
 }
@@ -372,26 +369,19 @@ extern "C" int lio_po_create(float scan_period, int io_ratio, int num_max_iterat
   if (!out || !(scan_period > 0) || num_max_iterations < 0 || max_feature_points < 16 || max_full_points < 16) return LIO_ERR_INVALID;
   if (lio_device_count() <= 0) return LIO_ERR_NO_DEVICE;
   LIO_CUDA_OK(cudaSetDevice(device));
-  lio_po *p = new (std::nothrow) lio_po();
+  std::unique_ptr<lio_po> p(new (std::nothrow) lio_po());
   if (!p) return LIO_ERR_INVALID;
   p->device = device; p->stream = (cudaStream_t)cuda_stream;
   cudaDeviceGetAttribute(&p->sm, cudaDevAttrMultiProcessorCount, device);
   p->time_factor = 1 / scan_period; p->io_ratio = io_ratio; p->max_iter = num_max_iterations;
   p->cap_feat = max_feature_points; p->cap_full = max_full_points;
-  bool ok = true;
-  float4 **clouds[] = {&p->d_sharp, &p->d_flat, &p->d_less_sharp, &p->d_less_flat, &p->d_last_corner, &p->d_last_surf};
-  for (float4 **c : clouds) ok = ok && cudaMalloc(c, sizeof(float4) * max_feature_points) == cudaSuccess;
-  ok = ok && cudaMalloc(&p->d_full, sizeof(float4) * max_full_points) == cudaSuccess;
-  ok = ok && cudaMalloc(&p->d_idx_c, sizeof(int) * 2 * max_feature_points) == cudaSuccess;
-  ok = ok && cudaMalloc(&p->d_idx_s, sizeof(int) * 3 * max_feature_points) == cudaSuccess;
-  ok = ok && cudaMalloc(&p->d_nsel, sizeof(int)) == cudaSuccess;
-  ok = ok && cudaMalloc(&p->d_tf, sizeof(TransformF)) == cudaSuccess;
-  ok = ok && cudaMalloc(&p->d_odom, sizeof(OdomState)) == cudaSuccess;
-  ok = ok && cudaMalloc(&p->d_cnt, sizeof(int) * 6) == cudaSuccess;
-  ok = ok && cudaMalloc(&p->d_pub_n, sizeof(int) * 3) == cudaSuccess;
-  ok = ok && cudaMemset(p->d_pub_n, 0, sizeof(int) * 3) == cudaSuccess;
-  if (!ok) { lio_set_last_error(__FILE__, __LINE__, "lio_po_create: device allocation failed"); lio_po_destroy(p); return LIO_ERR_CUDA; }
-  *out = p;
+  const int nf = max_feature_points;
+  const bool ok = alloc(p->d_sharp, nf) && alloc(p->d_flat, nf) && alloc(p->d_less_sharp, nf) && alloc(p->d_less_flat, nf) &&
+                  alloc(p->d_last_corner, nf) && alloc(p->d_last_surf, nf) && alloc(p->d_full, max_full_points) && alloc(p->d_idx_c, 2 * nf) &&
+                  alloc(p->d_idx_s, 3 * nf) && alloc(p->d_nsel, 1) && alloc(p->d_tf, 1) && alloc(p->d_odom, 1) && alloc(p->d_cnt, 6) &&
+                  alloc(p->d_pub_n, 3) && cudaMemset(p->d_pub_n, 0, sizeof(int) * 3) == cudaSuccess;
+  if (!ok) { lio_set_last_error(__FILE__, __LINE__, "lio_po_create: device allocation failed"); return LIO_ERR_CUDA; }
+  *out = p.release();
   return LIO_OK;
 }
 
@@ -527,7 +517,7 @@ extern "C" int lio_po_process_dev(lio_po *p, const float *const clouds_dev[5], c
 
 extern "C" int lio_po_clouds_dev(lio_po *p, const float *ptr[3], const int **n_dev, int n_host[3]) {
   if (!p || !ptr || !n_dev || !n_host) return LIO_ERR_INVALID;
-  ptr[0] = (const float *)p->d_last_corner; ptr[1] = (const float *)p->d_last_surf; ptr[2] = (const float *)p->d_full;
+  ptr[0] = (const float *)p->d_last_corner.get(); ptr[1] = (const float *)p->d_last_surf.get(); ptr[2] = (const float *)p->d_full.get();
   *n_dev = p->d_pub_n;
   n_host[0] = p->n_last_corner; n_host[1] = p->n_last_surf; n_host[2] = p->n_full;
   return LIO_OK;

@@ -63,11 +63,11 @@ constexpr int kRsBits = 8;
 constexpr int kRsBins = 1 << kRsBits;
 
 struct RadixSortTemp {
+  DevMem<unsigned> mem;      // init's allocation; empty when buf points into a caller's own scratch
   unsigned *buf = nullptr;   // digit histograms [4][256] | tickets [8] | look-back status [4][ntiles_max][256]
   size_t words = 0;
   int ntiles_max = 0;
   int init(int max_keys);
-  void destroy();
 };
 
 // Sorts n pairs by the low `key_bits` bits (rounded up to a multiple of 8).  n is read from the

@@ -20,6 +20,7 @@
 #include <cerrno>
 #include <cmath>
 #include <cstring>
+#include <memory>
 #include <vector>
 #include "primitives.cuh"
 #include "regmap.cuh"
@@ -184,18 +185,18 @@ struct lio_rm {
   float leaf = 0.f, inv_leaf = 0.f;
   long long capacity = 0;
   // raw mode: the concatenation, its size and the overflow flag are host state
-  float4 *d_pts = nullptr;
+  DevMem<float4> d_pts;
   long long n_raw = 0, raw_overflow = 0;
   // voxel mode
-  unsigned long long *d_slot_key = nullptr;
-  int *d_slot_id = nullptr;
+  DevMem<unsigned long long> d_slot_key;
+  DevMem<int> d_slot_id;
   long long nslots = 0;
-  double4 *d_sum = nullptr;
-  long long *d_cnt = nullptr;
-  float4 *d_export = nullptr;
-  RmState *d_state = nullptr;
-  RmState *h_state = nullptr;   // pinned
-  // per-insert scratch, grown stream-ordered (cudaMallocAsync) for a larger cloud
+  DevMem<double4> d_sum;
+  DevMem<long long> d_cnt;
+  DevMem<float4> d_export;
+  DevMem<RmState> d_state;
+  HostMem<RmState> h_state;     // pinned
+  // per-insert scratch, grown stream-ordered (cudaMallocAsync) for a larger cloud: the views below point into it
   int batch_cap = 0;
   void *d_batch_mem = nullptr;
   float4 *d_in = nullptr;
@@ -207,6 +208,11 @@ struct lio_rm {
   RadixSortTemp sort_tmp;
   // host counters: insert calls, points offered, host waits of every entry, stream operations of the last insert
   long long inserts = 0, offered = 0, waits = 0, last_launches = 0;
+  // The scratch goes behind the stream's last use of it, and the stream drains before the buffers above are freed.
+  ~lio_rm() {
+    if (d_batch_mem) cudaFreeAsync(d_batch_mem, stream);
+    cudaStreamSynchronize(stream);
+  }
 };
 
 static long long rm_blocks(long long n) { return std::max(1LL, (n + kRmThreads - 1) / kRmThreads); }
@@ -255,16 +261,6 @@ static int rm_clear(lio_rm *m) {
   return LIO_OK;
 }
 
-static void rm_free(lio_rm *m) {
-  if (m->d_batch_mem) cudaFreeAsync(m->d_batch_mem, m->stream);
-  cudaStreamSynchronize(m->stream);
-  for (void *p : {(void *)m->d_pts, (void *)m->d_slot_key, (void *)m->d_slot_id, (void *)m->d_sum, (void *)m->d_cnt,
-                  (void *)m->d_export, (void *)m->d_state})
-    if (p) cudaFree(p);
-  if (m->h_state) cudaFreeHost(m->h_state);
-  delete m;
-}
-
 extern "C" int lio_rm_create(float leaf, long long capacity, int device, void *cuda_stream, lio_rm **out) {
   if (!out || !(leaf >= 0.f) || !std::isfinite(leaf) || capacity < 1 || (leaf > 0.f && capacity > (1LL << 30)) ||
       (leaf > 0.f && !std::isfinite(1.0f / leaf)))
@@ -272,37 +268,31 @@ extern "C" int lio_rm_create(float leaf, long long capacity, int device, void *c
   *out = nullptr;
   if (lio_device_count() <= device || device < 0) return LIO_ERR_NO_DEVICE;
   LIO_CUDA_OK(cudaSetDevice(device));
-  lio_rm *m = new lio_rm;
+  std::unique_ptr<lio_rm> m(new lio_rm);
   m->device = device; m->stream = (cudaStream_t)cuda_stream;
   m->leaf = leaf; m->inv_leaf = leaf > 0.f ? 1.0f / leaf : 0.f;
   m->capacity = capacity;
   bool ok = true;
   if (leaf == 0.f) {
-    ok = cudaMalloc(&m->d_pts, sizeof(float4) * capacity) == cudaSuccess;
+    ok = alloc(m->d_pts, capacity);
   } else {
     m->nslots = 2 * capacity;
-    ok = ok && cudaMalloc(&m->d_slot_key, sizeof(unsigned long long) * m->nslots) == cudaSuccess;
-    ok = ok && cudaMalloc(&m->d_slot_id, sizeof(int) * m->nslots) == cudaSuccess;
-    ok = ok && cudaMalloc(&m->d_sum, sizeof(double4) * capacity) == cudaSuccess;
-    ok = ok && cudaMalloc(&m->d_cnt, sizeof(long long) * capacity) == cudaSuccess;
-    ok = ok && cudaMalloc(&m->d_export, sizeof(float4) * capacity) == cudaSuccess;
-    ok = ok && cudaMalloc(&m->d_state, sizeof(RmState)) == cudaSuccess;
-    ok = ok && cudaMallocHost(&m->h_state, sizeof(RmState)) == cudaSuccess;
+    ok = alloc(m->d_slot_key, m->nslots) && alloc(m->d_slot_id, m->nslots) && alloc(m->d_sum, capacity) && alloc(m->d_cnt, capacity) &&
+         alloc(m->d_export, capacity) && alloc(m->d_state, 1) && alloc_host(m->h_state, 1);
   }
-  if (!ok || rm_clear(m) != LIO_OK || cudaStreamSynchronize(m->stream) != cudaSuccess) {
+  if (!ok || rm_clear(m.get()) != LIO_OK || cudaStreamSynchronize(m->stream) != cudaSuccess) {
     lio_set_last_error(__FILE__, __LINE__, "lio_rm_create: allocation failed");
     cudaGetLastError();
-    rm_free(m);
     return LIO_ERR_CUDA;
   }
-  *out = m;
+  *out = m.release();
   return LIO_OK;
 }
 
 extern "C" int lio_rm_destroy(lio_rm *m) {
   if (!m) return LIO_ERR_INVALID;
-  cudaSetDevice(m->device);
-  rm_free(m);
+  cudaSetDevice(m->device);   // the buffers belong to the handle's device, whichever is current
+  delete m;
   return LIO_OK;
 }
 
@@ -394,10 +384,10 @@ extern "C" int lio_rm_export_dev(lio_rm *m, const float **ptr, long long *n) {
   RmState s;
   int rc = rm_read_state(m, &s);
   if (rc != LIO_OK) return rc;
-  if (m->leaf == 0.f) { *ptr = (const float *)m->d_pts; *n = m->n_raw; return LIO_OK; }
+  if (m->leaf == 0.f) { *ptr = (const float *)m->d_pts.get(); *n = m->n_raw; return LIO_OK; }
   if (s.size > 0) k_rm_export<<<(unsigned)rm_blocks(s.size), kRmThreads, 0, m->stream>>>(m->d_sum, m->d_cnt, s.size, m->d_export);
   LIO_CUDA_OK(cudaGetLastError());
-  *ptr = (const float *)m->d_export; *n = s.size;
+  *ptr = (const float *)m->d_export.get(); *n = s.size;
   return LIO_OK;
 }
 

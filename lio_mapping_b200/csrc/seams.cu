@@ -70,7 +70,6 @@ extern "C" int lio_asm_ppp_host(const float *pts4, const float *coef4, int n, co
     rc = asm_launch(ap, dRt, w, 0, nullptr);
     if (rc == LIO_OK && (!d.ok(cudaDeviceSynchronize()) || !d.down(out32, w.out, kAsmStride))) rc = LIO_ERR_CUDA;
   }
-  w.destroy();
   return rc;
 }
 
@@ -113,7 +112,7 @@ extern "C" int lio_asm_stream_bench(long long n_features, int iters, int device,
   float4 *dp = nullptr, *dc = nullptr;
   double *dRt = nullptr;
   AsmWork w;
-  cudaEvent_t e0 = nullptr, e1 = nullptr;
+  Event e0, e1;
   AsmParams ap;
   std::memset(&ap, 0, sizeof(ap));
   ap.nframes = O;
@@ -129,7 +128,7 @@ extern "C" int lio_asm_stream_bench(long long n_features, int iters, int device,
       const double Rt[kAsmRtStride] = {c, -s, 0, s, c, 0, 0, 0, 1, 0.1 * k, 0.02 * k, 0.0};
       std::memcpy(hRt + k * kAsmRtStride, Rt, sizeof(Rt));
     }
-    if (!d.ok(cudaEventCreate(&e0)) || !d.ok(cudaEventCreate(&e1)) || !d.alloc(&dRt, 8 * kAsmRtStride) || !d.up(dRt, hRt, 8 * kAsmRtStride))
+    if (!create(e0, cudaEventDefault) || !create(e1, cudaEventDefault) || !d.alloc(&dRt, 8 * kAsmRtStride) || !d.up(dRt, hRt, 8 * kAsmRtStride))
       rc = LIO_ERR_CUDA;
   }
   if (rc == LIO_OK) {
@@ -148,8 +147,5 @@ extern "C" int lio_asm_stream_bench(long long n_features, int iters, int device,
     }
     out[0] = sum / iters; out[1] = mn; out[2] = 32.0 * (double)(per * O); out[3] = iters;
   }
-  if (e0) cudaEventDestroy(e0);
-  if (e1) cudaEventDestroy(e1);
-  w.destroy();
   return rc;
 }

@@ -1422,20 +1422,16 @@ int DevSolver::init(int O_) {
   O = O_;
   const int n = 15 * (O + 1) + 6, np = 15 * O + 6;
   smem_bytes = O <= kDsMaxOpt1 ? step_smem_bytes(O) : step_x2_smem_bytes();
-  if (cudaMalloc(&st, sizeof(DevSolveState)) != cudaSuccess) return -1;
-  if (cudaMalloc(&Hs, sizeof(double) * n * n) != cudaSuccess) return -1;
-  if (cudaMalloc(&H0, sizeof(double) * n * n) != cudaSuccess) return -1;
-  if (cudaMalloc(&g0, sizeof(double) * n) != cudaSuccess) return -1;
-  if (cudaMalloc(&Hp, sizeof(double) * np * np) != cudaSuccess) return -1;
-  if (cudaMalloc(&F, sizeof(double) * f_doubles()) != cudaSuccess) return -1;
-  if (cudaMalloc(&Hpart, sizeof(double) * ((size_t)n * n + n + 8)) != cudaSuccess) return -1;
+  if (!alloc(st, 1) || !alloc(Hs, n * n) || !alloc(H0, n * n) || !alloc(g0, n) || !alloc(Hp, np * np) || !alloc(F, f_doubles()) ||
+      !alloc(Hpart, (size_t)n * n + n + 8))
+    return -1;
   if (cudaMemset(Hpart, 0, sizeof(double) * ((size_t)n * n + n + 8)) != cudaSuccess) return -1;
   {
     const size_t NBt = (n + 7) / 8, ntd = NBt * (NBt + 1) / 2 * 64;
-    if (cudaMalloc(&HpartT, sizeof(double) * ntd) != cudaSuccess || cudaMemset(HpartT, 0, sizeof(double) * ntd) != cudaSuccess) return -1;
+    if (!alloc(HpartT, ntd) || cudaMemset(HpartT, 0, sizeof(double) * ntd) != cudaSuccess) return -1;
     if (cudaMemset(Hs, 0, sizeof(double) * n * n) != cudaSuccess) return -1;
   }
-  if (cudaMallocHost((void **)&h_st, sizeof(DevSolveState)) != cudaSuccess) return -1;
+  if (!alloc_host(h_st, 1)) return -1;
   if (cudaMemset(st, 0, sizeof(DevSolveState)) != cudaSuccess) return -1;
   if (cudaMemset(F, 0, sizeof(double) * f_doubles()) != cudaSuccess) return -1;
   if (O <= kDsMaxOpt1) {
@@ -1443,20 +1439,7 @@ int DevSolver::init(int O_) {
   } else if (cudaFuncSetAttribute(k_step_x2, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes) != cudaSuccess) {
     return -1;
   }
-  if (cudaStreamCreateWithFlags(&aux, cudaStreamNonBlocking) != cudaSuccess) return -1;
-  if (cudaEventCreateWithFlags(&ev_fork, cudaEventDisableTiming) != cudaSuccess) return -1;
-  if (cudaEventCreateWithFlags(&ev_join, cudaEventDisableTiming) != cudaSuccess) return -1;
-  return 0;
-}
-
-void DevSolver::destroy() {
-  void *p[] = {st, Hs, H0, g0, Hp, F, Hpart, HpartT};
-  for (void *q : p) if (q) cudaFree(q);
-  if (h_st) cudaFreeHost(h_st);
-  if (aux) cudaStreamDestroy(aux);
-  if (ev_fork) cudaEventDestroy(ev_fork);
-  if (ev_join) cudaEventDestroy(ev_join);
-  st = nullptr; Hs = Hp = H0 = g0 = F = Hpart = HpartT = nullptr; h_st = nullptr; aux = nullptr; ev_fork = ev_join = nullptr;
+  return create(aux) && create(ev_fork) && create(ev_join) ? 0 : -1;
 }
 
 static FPtrs fptrs(const DevSolver &ds) {

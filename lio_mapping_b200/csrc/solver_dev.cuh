@@ -55,23 +55,22 @@ constexpr int kFMStride = 108;     // M_i (6 x 18) of the PivotPointPlane frame 
 constexpr int kFGStride = 344;     // G_i = M_i^T S_gg M_i (18 x 18) | M_i^T S_gr (18) | pad   (written by k_step itself)
 
 struct DevSolver {
-  DevSolveState *st = nullptr;     // device
-  double *Hs = nullptr;            // the Jacobi-scaled normal matrix of the current x as the step kernel's swizzled lower tiles (mu-retry / invalid-step reload)
-  double *HpartT = nullptr;        // evaluations >= 1: scaled lidar-independent share of H in the same tile layout (bulk-copied into shared memory)
+  DevMem<DevSolveState> st;       // device
+  DevMem<double> Hs;               // the Jacobi-scaled normal matrix of the current x as the step kernel's swizzled lower tiles (mu-retry / invalid-step reload)
+  DevMem<double> HpartT;           // evaluations >= 1: scaled lidar-independent share of H in the same tile layout (bulk-copied into shared memory)
                                    // (only re-read when a factorisation has to be repeated with a larger mu)
-  double *Hp = nullptr;            // prior np x np
-  double *H0 = nullptr, *g0 = nullptr;   // first linearisation, unscaled (parity getter)
-  double *F = nullptr;             // factor scratch: imu | M | prior vec | ex prior | G
-  double *Hpart = nullptr;         // n x n row-major, lower triangle: prior + ImuFactor + PriorFactor part of H at the state
+  DevMem<double> Hp;               // prior np x np
+  DevMem<double> H0, g0;           // first linearisation, unscaled (parity getter)
+  DevMem<double> F;                // factor scratch: imu | M | prior vec | ex prior | G
+  DevMem<double> Hpart;            // n x n row-major, lower triangle: prior + ImuFactor + PriorFactor part of H at the state
                                    // being evaluated (unscaled), gathered by k_hpart beside asm_ppp; then n gradient entries
                                    // and 2 words recording the structure flags it was built with
-  DevSolveState *h_st = nullptr;   // pinned staging copy
+  HostMem<DevSolveState> h_st;     // pinned staging copy
   size_t smem_bytes = 0;
   int O = 0;
-  cudaStream_t aux = nullptr;      // k_factors runs beside asm_ppp
-  cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
+  Stream aux;                      // k_factors runs beside asm_ppp
+  Event ev_fork, ev_join;
   int init(int O);
-  void destroy();
   bool supports(int O) const;
   // scratch offsets (doubles)
   size_t off_imu() const { return 0; }

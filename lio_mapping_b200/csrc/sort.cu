@@ -126,11 +126,9 @@ rs_pass(const unsigned *__restrict__ keys, const unsigned *__restrict__ vals, un
 int RadixSortTemp::init(int max_keys) {
   ntiles_max = (max_keys + kRsTile - 1) / kRsTile + 1;
   words = (size_t)4 * kRsBins + 8 + (size_t)4 * ntiles_max * kRsBins;   // digit histograms | tickets | per-pass tile status
-  return cudaMalloc(&buf, sizeof(unsigned) * words) == cudaSuccess ? 0 : -1;
-}
-void RadixSortTemp::destroy() {
-  if (buf) cudaFree(buf);
-  buf = nullptr;
+  if (!alloc(mem, words)) return -1;
+  buf = mem;
+  return 0;
 }
 
 int radix_sort_pairs(unsigned *keys_a, unsigned *vals_a, unsigned *keys_b, unsigned *vals_b, const int *n_dev, int n_max,
@@ -181,6 +179,5 @@ extern "C" int lio_radix_sort_pairs_host(const uint32_t *keys, const uint32_t *v
     else if (!d.ok(cudaDeviceSynchronize()) || !d.down(keys_out, which ? kb : ka, n) || !d.down(vals_out, which ? vb : va, n))
       rc = LIO_ERR_CUDA;
   }
-  tmp.destroy();
   return rc;
 }

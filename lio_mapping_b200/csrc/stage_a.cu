@@ -20,6 +20,7 @@
 //   a_compact  : concatenates per-ring results in the reference's output order
 #include "common.cuh"
 #include <cmath>
+#include <memory>
 #include <new>
 
 namespace lio {
@@ -673,18 +674,18 @@ struct lio_pp {
   int max_points, nb_max;
   size_t ring_smem;
   // device buffers
-  float4 *d_in = nullptr, *d_laser = nullptr, *d_full = nullptr, *d_lf_ring = nullptr;
-  float4 *d_out_sharp = nullptr, *d_out_less = nullptr, *d_out_flat = nullptr, *d_out_lf = nullptr;
-  int16_t *d_ring_id = nullptr;
-  float *d_azi = nullptr, *d_start_ori = nullptr;
-  int *d_first_valid = nullptr, *d_hist = nullptr, *d_offsets = nullptr, *d_ring_start = nullptr, *d_orig = nullptr;
-  unsigned char *d_mask = nullptr;
-  signed char *d_label = nullptr;
-  int *d_pick_less = nullptr, *d_n_less = nullptr, *d_pick_flat = nullptr, *d_n_flat = nullptr, *d_lf_count = nullptr;
-  int *d_idx_sharp = nullptr, *d_idx_less = nullptr, *d_idx_flat = nullptr, *d_counts = nullptr, *d_err = nullptr;
-  unsigned short *d_rings_in = nullptr;  // ring-field variant only (allocated on first use)
-  int *d_end_bits = nullptr;
-  int *h_counts = nullptr;  // pinned: counts[0..4], err
+  DevMem<float4> d_in, d_laser, d_full, d_lf_ring;
+  DevMem<float4> d_out_sharp, d_out_less, d_out_flat, d_out_lf;
+  DevMem<int16_t> d_ring_id;
+  DevMem<float> d_azi, d_start_ori;
+  DevMem<int> d_first_valid, d_hist, d_offsets, d_ring_start, d_orig;
+  DevMem<unsigned char> d_mask;
+  DevMem<signed char> d_label;
+  DevMem<int> d_pick_less, d_n_less, d_pick_flat, d_n_flat, d_lf_count;
+  DevMem<int> d_idx_sharp, d_idx_less, d_idx_flat, d_counts, d_err;
+  DevMem<unsigned short> d_rings_in;  // ring-field variant only (allocated on first use)
+  DevMem<int> d_end_bits;
+  HostMem<int> h_counts;   // pinned: counts[0..4], err
   int launches = 0;
   int last_n = 0;
   bool counts_valid = false;
@@ -695,8 +696,6 @@ extern "C" void lio_pp_default_config(lio_pp_config *c) {
   c->num_scan_subregions = 8; c->num_curvature_regions = 5; c->surf_curv_th = 0.1f;
   c->max_corner_sharp = 2; c->max_corner_less_sharp = 20; c->max_surf_flat = 4; c->less_flat_filter_size = 0.2f;
 }
-
-template <typename T> static cudaError_t dalloc(T **p, size_t n) { return cudaMalloc((void **)p, n * sizeof(T)); }
 
 extern "C" int lio_pp_create(const lio_pp_config *cfg, int max_points, int device, void *cuda_stream, lio_pp **out) {
   if (!cfg || !out || max_points <= 0) return LIO_ERR_INVALID;
@@ -709,7 +708,7 @@ extern "C" int lio_pp_create(const lio_pp_config *cfg, int max_points, int devic
   }
   if (lio_device_count() <= 0) return LIO_ERR_NO_DEVICE;
   LIO_CUDA_OK(cudaSetDevice(device));
-  lio_pp *pp = new (std::nothrow) lio_pp();
+  std::unique_ptr<lio_pp> pp(new (std::nothrow) lio_pp());
   if (!pp) return LIO_ERR_INVALID;
   pp->cfg = *cfg;
   pp->device = device;
@@ -724,40 +723,28 @@ extern "C" int lio_pp_create(const lio_pp_config *cfg, int max_points, int devic
   const int R = P.num_rings, S = P.S;
   pp->nb_max = (max_points + kClsPerBlock - 1) / kClsPerBlock;
   const size_t N = (size_t)max_points;
-  LIO_CUDA_OK(dalloc(&pp->d_in, N)); LIO_CUDA_OK(dalloc(&pp->d_laser, N)); LIO_CUDA_OK(dalloc(&pp->d_full, N));
-  LIO_CUDA_OK(dalloc(&pp->d_lf_ring, N)); LIO_CUDA_OK(dalloc(&pp->d_out_lf, N));
-  LIO_CUDA_OK(dalloc(&pp->d_out_sharp, (size_t)R * S * kMaxLessSharp)); LIO_CUDA_OK(dalloc(&pp->d_out_less, (size_t)R * S * kMaxLessSharp));
-  LIO_CUDA_OK(dalloc(&pp->d_out_flat, (size_t)R * S * kMaxFlat));
-  LIO_CUDA_OK(dalloc(&pp->d_ring_id, N)); LIO_CUDA_OK(dalloc(&pp->d_azi, N)); LIO_CUDA_OK(dalloc(&pp->d_start_ori, 1));
-  LIO_CUDA_OK(dalloc(&pp->d_first_valid, 1)); LIO_CUDA_OK(dalloc(&pp->d_hist, (size_t)pp->nb_max * R));
-  LIO_CUDA_OK(dalloc(&pp->d_offsets, (size_t)pp->nb_max * R)); LIO_CUDA_OK(dalloc(&pp->d_ring_start, R + 1));
-  LIO_CUDA_OK(dalloc(&pp->d_orig, N)); LIO_CUDA_OK(dalloc(&pp->d_mask, N)); LIO_CUDA_OK(dalloc(&pp->d_label, N));
-  LIO_CUDA_OK(dalloc(&pp->d_pick_less, (size_t)R * S * kMaxLessSharp)); LIO_CUDA_OK(dalloc(&pp->d_n_less, (size_t)R * S));
-  LIO_CUDA_OK(dalloc(&pp->d_pick_flat, (size_t)R * S * kMaxFlat)); LIO_CUDA_OK(dalloc(&pp->d_n_flat, (size_t)R * S));
-  LIO_CUDA_OK(dalloc(&pp->d_lf_count, R));
-  LIO_CUDA_OK(dalloc(&pp->d_idx_sharp, (size_t)R * S * kMaxLessSharp)); LIO_CUDA_OK(dalloc(&pp->d_idx_less, (size_t)R * S * kMaxLessSharp));
-  LIO_CUDA_OK(dalloc(&pp->d_idx_flat, (size_t)R * S * kMaxFlat)); LIO_CUDA_OK(dalloc(&pp->d_counts, 8)); LIO_CUDA_OK(dalloc(&pp->d_err, 1));
-  LIO_CUDA_OK(cudaMallocHost((void **)&pp->h_counts, 16 * sizeof(int)));
+  const size_t RS = (size_t)R * S;
+  if (!alloc(pp->d_in, N) || !alloc(pp->d_laser, N) || !alloc(pp->d_full, N) || !alloc(pp->d_lf_ring, N) || !alloc(pp->d_out_lf, N) ||
+      !alloc(pp->d_out_sharp, RS * kMaxLessSharp) || !alloc(pp->d_out_less, RS * kMaxLessSharp) || !alloc(pp->d_out_flat, RS * kMaxFlat) ||
+      !alloc(pp->d_ring_id, N) || !alloc(pp->d_azi, N) || !alloc(pp->d_start_ori, 1) || !alloc(pp->d_first_valid, 1) ||
+      !alloc(pp->d_hist, (size_t)pp->nb_max * R) || !alloc(pp->d_offsets, (size_t)pp->nb_max * R) || !alloc(pp->d_ring_start, R + 1) ||
+      !alloc(pp->d_orig, N) || !alloc(pp->d_mask, N) || !alloc(pp->d_label, N) || !alloc(pp->d_pick_less, RS * kMaxLessSharp) ||
+      !alloc(pp->d_n_less, RS) || !alloc(pp->d_pick_flat, RS * kMaxFlat) || !alloc(pp->d_n_flat, RS) || !alloc(pp->d_lf_count, R) ||
+      !alloc(pp->d_idx_sharp, RS * kMaxLessSharp) || !alloc(pp->d_idx_less, RS * kMaxLessSharp) || !alloc(pp->d_idx_flat, RS * kMaxFlat) ||
+      !alloc(pp->d_counts, 8) || !alloc(pp->d_err, 1) || !alloc_host(pp->h_counts, 16))
+    return LIO_ERR_CUDA;
   LIO_CUDA_OK(cudaMemset(pp->d_err, 0, sizeof(int)));
   // shared memory of the ring kernel: sized for the largest ring we may see
   int maxn = max_points < kMaxRingPoints ? max_points : kMaxRingPoints;
   pp->ring_smem = (size_t)maxn * (8 + 16 + 2) + 64;
   LIO_CUDA_OK(cudaFuncSetAttribute(a_ring, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pp->ring_smem));
-  *out = pp;
+  *out = pp.release();
   return LIO_OK;
 }
 
 extern "C" int lio_pp_destroy(lio_pp *pp) {
   if (!pp) return LIO_OK;
-  cudaSetDevice(pp->device);
-  void *ptrs[] = {pp->d_in, pp->d_laser, pp->d_full, pp->d_lf_ring, pp->d_out_lf, pp->d_out_sharp, pp->d_out_less, pp->d_out_flat,
-                  pp->d_ring_id, pp->d_azi, pp->d_start_ori, pp->d_first_valid, pp->d_hist, pp->d_offsets, pp->d_ring_start,
-                  pp->d_orig, pp->d_mask, pp->d_label, pp->d_pick_less, pp->d_n_less, pp->d_pick_flat, pp->d_n_flat,
-                  pp->d_lf_count, pp->d_idx_sharp, pp->d_idx_less, pp->d_idx_flat, pp->d_counts, pp->d_err};
-  for (void *p : ptrs) if (p) cudaFree(p);
-  if (pp->d_rings_in) cudaFree(pp->d_rings_in);
-  if (pp->d_end_bits) cudaFree(pp->d_end_bits);
-  if (pp->h_counts) cudaFreeHost(pp->h_counts);
+  cudaSetDevice(pp->device);   // the buffers belong to the handle's device, whichever is current
   delete pp;
   return LIO_OK;
 }
@@ -811,7 +798,7 @@ extern "C" int lio_pp_process_host(lio_pp *pp, const float *xyzi, int n) {
   if (n > pp->max_points) return LIO_ERR_CAPACITY;
   LIO_CUDA_OK(cudaSetDevice(pp->device));
   if (n > 0) LIO_CUDA_OK(cudaMemcpyAsync(pp->d_in, xyzi, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, pp->stream));
-  int rc = lio_pp_process_dev(pp, reinterpret_cast<const float *>(pp->d_in), n);
+  int rc = lio_pp_process_dev(pp, reinterpret_cast<const float *>(pp->d_in.get()), n);
   if (rc != LIO_OK) return rc;
   return pp_sync_counts(pp);
 }
@@ -821,7 +808,7 @@ extern "C" int lio_pp_process_dev_ring(lio_pp *pp, const float *xyzi_dev, const 
   if (!pp || ((!xyzi_dev || !rings_dev) && n > 0) || n < 0) return LIO_ERR_INVALID;
   if (n > pp->max_points) return LIO_ERR_CAPACITY;
   LIO_CUDA_OK(cudaSetDevice(pp->device));
-  if (!pp->d_end_bits) LIO_CUDA_OK(dalloc(&pp->d_end_bits, 1));
+  if (!pp->d_end_bits && !alloc(pp->d_end_bits, 1)) return LIO_ERR_CUDA;
   cudaStream_t st = pp->stream;
   const PPParams &P = pp->P;
   const int R = P.num_rings;
@@ -857,12 +844,12 @@ extern "C" int lio_pp_process_host_ring(lio_pp *pp, const float *xyzi, const uin
   if (!pp || ((!xyzi || !rings) && n > 0) || n < 0) return LIO_ERR_INVALID;
   if (n > pp->max_points) return LIO_ERR_CAPACITY;
   LIO_CUDA_OK(cudaSetDevice(pp->device));
-  if (!pp->d_rings_in) LIO_CUDA_OK(dalloc(&pp->d_rings_in, (size_t)pp->max_points));
+  if (!pp->d_rings_in && !alloc(pp->d_rings_in, (size_t)pp->max_points)) return LIO_ERR_CUDA;
   if (n > 0) {
     LIO_CUDA_OK(cudaMemcpyAsync(pp->d_in, xyzi, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, pp->stream));
     LIO_CUDA_OK(cudaMemcpyAsync(pp->d_rings_in, rings, (size_t)n * sizeof(uint16_t), cudaMemcpyHostToDevice, pp->stream));
   }
-  int rc = lio_pp_process_dev_ring(pp, reinterpret_cast<const float *>(pp->d_in), reinterpret_cast<const uint16_t *>(pp->d_rings_in), n);
+  int rc = lio_pp_process_dev_ring(pp, reinterpret_cast<const float *>(pp->d_in.get()), pp->d_rings_in, n);
   if (rc != LIO_OK) return rc;
   return pp_sync_counts(pp);
 }

@@ -141,24 +141,11 @@ vg_emit(const float4 *__restrict__ in, const int *__restrict__ n_dev, const unsi
 
 int VoxelGrid::init(int cap_) {
   cap = cap_;
-  if (cudaMalloc(&keys_a, sizeof(unsigned) * cap) != cudaSuccess) return -1;
-  if (cudaMalloc(&vals_a, sizeof(unsigned) * cap) != cudaSuccess) return -1;
-  if (cudaMalloc(&keys_b, sizeof(unsigned) * cap) != cudaSuccess) return -1;
-  if (cudaMalloc(&vals_b, sizeof(unsigned) * cap) != cudaSuccess) return -1;
-  if (rs.init(cap) != 0) return -1;
   nstatus = (cap + kEmitThreads - 1) / kEmitThreads + 1;
-  if (cudaMalloc(&status, sizeof(unsigned long long) * nstatus) != cudaSuccess) return -1;
-  if (cudaMalloc(&bbox, sizeof(unsigned) * 8) != cudaSuccess) return -1;
-  if (cudaMalloc(&ticket, sizeof(int) * 4) != cudaSuccess) return -1;
-  if (cudaMemset(ticket, 0, sizeof(int) * 4) != cudaSuccess) return -1;
+  if (!alloc(keys_a, cap) || !alloc(vals_a, cap) || !alloc(keys_b, cap) || !alloc(vals_b, cap) || rs.init(cap) != 0 ||
+      !alloc(status, nstatus) || !alloc(bbox, 8) || !alloc(ticket, 4) || cudaMemset(ticket, 0, sizeof(int) * 4) != cudaSuccess)
+    return -1;
   return 0;
-}
-
-void VoxelGrid::destroy() {
-  void *p[] = {keys_a, vals_a, keys_b, vals_b, status, bbox, ticket};
-  for (void *q : p) if (q) cudaFree(q);
-  rs.destroy();
-  keys_a = vals_a = keys_b = vals_b = nullptr; status = nullptr; bbox = nullptr; ticket = nullptr;
 }
 
 int VoxelGrid::run(const float4 *in, const int *n_dev_in, int n_max, float leaf, float4 *out, int out_cap, int *nout_dev,
@@ -300,32 +287,20 @@ vg_seg_scatter(const VgJob *__restrict__ jobs, int njobs, const float4 *__restri
 }
 
 int SegVoxelGrid::init() {
-  if (cudaMalloc(&d_jobs, sizeof(VgJob) * kVgMaxJobs) != cudaSuccess) return -1;
-  if (cudaMalloc(&jbbox, sizeof(unsigned) * 6 * kVgMaxJobs) != cudaSuccess) return -1;
-  if (cudaMalloc(&jstart, sizeof(int) * (kVgMaxJobs + 1)) != cudaSuccess) return -1;
-  if (cudaMalloc(&jn, sizeof(int) * (kVgMaxJobs + 1)) != cudaSuccess) return -1;
-  return 0;
+  return alloc(d_jobs, kVgMaxJobs) && alloc(jbbox, 6 * kVgMaxJobs) && alloc(jstart, kVgMaxJobs + 1) && alloc(jn, kVgMaxJobs + 1) ? 0 : -1;
 }
 
 int SegVoxelGrid::reserve(int total) {
   if (total <= cap) return 0;
-  ws.destroy();
-  if (cat) cudaFree(cat);
-  if (out) cudaFree(out);
-  cat = out = nullptr;
+  // the old workspace goes before the new one is allocated: nothing in it outlives a run
+  ws = VoxelGrid{};
+  cat = {};
+  out = {};
   cap = 0;
   const int c = std::max(2 * total, 1 << 16);
-  if (ws.init(c) != 0 || cudaMalloc(&cat, sizeof(float4) * c) != cudaSuccess || cudaMalloc(&out, sizeof(float4) * c) != cudaSuccess) return -1;
+  if (ws.init(c) != 0 || !alloc(cat, c) || !alloc(out, c)) return -1;
   cap = c;
   return 0;
-}
-
-void SegVoxelGrid::destroy() {
-  ws.destroy();
-  void *p[] = {cat, out, d_jobs, jbbox, jstart, jn};
-  for (void *q : p) if (q) cudaFree(q);
-  cat = out = nullptr; d_jobs = nullptr; jbbox = nullptr; jstart = jn = nullptr;
-  cap = 0;
 }
 
 int SegVoxelGrid::run(const VgJob *h_jobs, int njobs, int total, int *h_jn, cudaStream_t st, int *launches) {
@@ -376,7 +351,6 @@ extern "C" int lio_voxel_grid_host(const float *cloud, int n, float leaf, float 
     if (m > cap) rc = LIO_ERR_CAPACITY;
     else if (!d.down((float4 *)out, d_out, m)) rc = LIO_ERR_CUDA;
   }
-  vg.destroy();
   return rc;
 }
 
@@ -416,6 +390,5 @@ extern "C" int lio_seg_voxel_grid_host(const float *xyzi, const int *n_per_job, 
       rc = LIO_ERR_CUDA;
     }
   }
-  sg.destroy();
   return rc;
 }

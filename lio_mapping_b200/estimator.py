@@ -150,6 +150,11 @@ class Estimator:
         if getattr(self, "h", None):
             _lib.lib().lio_est_destroy(self.h)
             self.h = None
+        # the peer buffers set_peers / set_feature_peers opened from IPC handles: the destroyed context no longer reads them, and
+        # lio_est_destroy left its device current
+        for p in getattr(self, "_peer_open", []) + getattr(self, "_fpeer_open", []):
+            _lib.lib().lio_ipc_close(C.c_void_p(p))
+        self._peer_open, self._fpeer_open = [], []
         self._map = None
 
     def __del__(self):
