@@ -11,6 +11,8 @@
  *   - poses are double[7] {px,py,pz,qx,qy,qz,qw} (para_pose_ layout, Estimator.cc:2445-2452),
  *     float transforms are float[7] {qx,qy,qz,qw,px,py,pz} (Twist<float>);
  *   - every function returns LIO_OK (0) or a negative lio_status; lio_last_error() gives text;
+ *   - an entry that enqueues work on, copies from or waits for a handle's device makes that device current and leaves it
+ *     current, whatever device was current before; an entry that only reads or writes host state leaves it alone;
  *   - "_host" variants take host buffers and copy in/out on the context's stream (synchronous
  *     on return); "_dev" variants take device pointers and are stream-ordered (asynchronous);
  *   - one thread drives a given handle at a time (same rule as the reference objects).

@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 #include <cstdint>
 #include <cstdio>
+#include <type_traits>
 #include <vector>
 #include "../../include/lio_b200.h"
 #include "own.cuh"
@@ -18,7 +19,46 @@
 
 void lio_set_last_error(const char *file, int line, const char *msg);
 
+// Returns the status of expr when it is not LIO_OK.
+#define LIO_TRY(expr)                                                                       \
+  do {                                                                                      \
+    const int _rc = (expr);                                                                 \
+    if (_rc != LIO_OK) return _rc;                                                          \
+  } while (0)
+
+// The first statement of every handle entry.  LIO_ENTER serves the entries that enqueue work on, copy from or wait for the
+// handle's device: it makes that device current and leaves it so.  LIO_ENTER_HOST serves the entries that only touch host
+// state, which leave the current device alone.  Both refuse a null handle with LIO_ERR_INVALID and text naming the entry.
+#define LIO_ENTER(h) LIO_TRY(lio::enter(h, __func__, true))
+#define LIO_ENTER_HOST(h) LIO_TRY(lio::enter(h, __func__, false))
+
 namespace lio {
+
+int refuse_null_handle(const char *entry);
+
+template <class H> int enter(const H *h, const char *entry, bool on_device) {
+  if (!h) return refuse_null_handle(entry);
+  if (on_device) LIO_CUDA_OK(cudaSetDevice(h->device));
+  return LIO_OK;
+}
+
+// The prologue of the create entries and the stateless host-array entries: LIO_ERR_NO_DEVICE without a device, else `device`
+// made current and its SM count in *sms (when given).
+int select_device(int device, int *sms = nullptr);
+
+// Reads the n elements at src back to dst on stream s and waits for the stream.  *count (when given) receives n first; then
+// n > cap returns LIO_ERR_CAPACITY and a null dst with n > 0 LIO_ERR_INVALID, both before anything is copied.
+template <class T>
+int read_back(T *dst, const typename std::common_type<T>::type *src, long long n, long long cap, cudaStream_t s, int *count = nullptr) {
+  if (count) *count = (int)n;
+  if (n > cap) return LIO_ERR_CAPACITY;
+  if (n > 0) {
+    if (!dst) return LIO_ERR_INVALID;
+    LIO_CUDA_OK(cudaMemcpyAsync(dst, src, sizeof(T) * n, cudaMemcpyDeviceToHost, s));
+  }
+  LIO_CUDA_OK(cudaStreamSynchronize(s));
+  return LIO_OK;
+}
 
 // Device buffers of a host-array entry, freed when the entry returns.  alloc / up / down / ok set lio_last_error and return
 // false on failure, so an entry stops at the first failed allocation, copy or CUDA call.

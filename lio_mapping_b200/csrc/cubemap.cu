@@ -242,14 +242,12 @@ extern "C" int lio_pm_destroy(lio_pm *m) {
 extern "C" int lio_pm_create(int max_points, float corner_filter_size, float surf_filter_size, float min_match_sq_dis, float min_plane_dis,
                              int max_iterations, int device, void *cuda_stream, lio_pm **out) {
   if (!out || max_points < 16 || !(corner_filter_size > 0) || !(surf_filter_size > 0) || max_iterations < 0) return LIO_ERR_INVALID;
-  if (lio_device_count() <= 0) return LIO_ERR_NO_DEVICE;
-  LIO_CUDA_OK(cudaSetDevice(device));
   std::unique_ptr<lio_pm> m(new (std::nothrow) lio_pm());
   if (!m) return LIO_ERR_INVALID;
+  LIO_TRY(select_device(device, &m->sm));
   m->device = device; m->stream = (cudaStream_t)cuda_stream; m->max_points = max_points;
   m->leaf[0] = corner_filter_size; m->leaf[1] = surf_filter_size;
   m->min_match_sq_dis = min_match_sq_dis; m->min_plane_dis = min_plane_dis; m->max_iter = max_iterations;
-  cudaDeviceGetAttribute(&m->sm, cudaDevAttrMultiProcessorCount, device);
   m->cube[0].resize(kCubes);
   m->cube[1].resize(kCubes);
   const int n = max_points;
@@ -608,14 +606,13 @@ static int pm_process(lio_pm *m, const float4 *const src[2], const float4 *full,
 // Clouds: HOST arrays of n x 4 floats.
 extern "C" int lio_pm_process_host(lio_pm *m, const float *corner_last, int nc, const float *surf_last, int ns, const float transform_sum7[7],
                                    float transform_tobe_mapped7[7], int info3[3]) {
-  if (!m || m->mb || m->publish || m->attached || !transform_sum7 || nc < 0 || ns < 0 || (nc > 0 && !corner_last) || (ns > 0 && !surf_last))
+  LIO_ENTER(m);
+  if (m->mb || m->publish || m->attached || !transform_sum7 || nc < 0 || ns < 0 || (nc > 0 && !corner_last) || (ns > 0 && !surf_last))
     return LIO_ERR_INVALID;
   if (nc > m->max_points || ns > m->max_points) return LIO_ERR_CAPACITY;
-  LIO_CUDA_OK(cudaSetDevice(m->device));
   const float *src[2] = {corner_last, surf_last};
   const int nin[2] = {nc, ns};
-  int rc = pm_upload(m, src, nin, nullptr, 0);
-  if (rc != LIO_OK) return rc;
+  LIO_TRY(pm_upload(m, src, nin, nullptr, 0));
   const float4 *dsrc[2] = {m->d_in[0], m->d_in[1]};
   const int n_max[3] = {nc, ns, 0};
   return pm_process(m, dsrc, nullptr, m->d_cnt + 8, n_max, transform_sum7, transform_tobe_mapped7, nullptr, info3, 3);
@@ -624,10 +621,10 @@ extern "C" int lio_pm_process_host(lio_pm *m, const float *corner_last, int nc, 
 extern "C" int lio_pm_process_dev(lio_pm *m, const float *corner_dev, const float *surf_dev, const float *full_dev, const int *n3_dev,
                                   const int n3_max[3], const float transform_sum7[7], float transform_tobe_mapped7[7], float transform_aft_mapped7[7],
                                   int info5[5]) {
-  if (!m || m->mb || m->attached || !transform_sum7 || !n3_dev || !n3_max || n3_max[0] < 0 || n3_max[1] < 0 || n3_max[2] < 0 || (n3_max[0] > 0 && !corner_dev) ||
+  LIO_ENTER(m);
+  if (m->mb || m->attached || !transform_sum7 || !n3_dev || !n3_max || n3_max[0] < 0 || n3_max[1] < 0 || n3_max[2] < 0 || (n3_max[0] > 0 && !corner_dev) ||
       (n3_max[1] > 0 && !surf_dev) || (m->publish && n3_max[2] > 0 && !full_dev))
     return LIO_ERR_INVALID;
-  LIO_CUDA_OK(cudaSetDevice(m->device));
   const float4 *dsrc[2] = {reinterpret_cast<const float4 *>(corner_dev), reinterpret_cast<const float4 *>(surf_dev)};
   // without publishing the full cloud is not read: its count gets no bound, so it never reports an overflow
   const int n_max[3] = {std::min(n3_max[0], m->max_points), std::min(n3_max[1], m->max_points), m->publish ? std::min(n3_max[2], m->max_full) : INT_MAX};
@@ -637,7 +634,8 @@ extern "C" int lio_pm_process_dev(lio_pm *m, const float *corner_dev, const floa
 
 extern "C" int lio_pm_update_map_database_host(lio_pm *m, const float *corner_ds, int nc, const float *surf_ds, int ns, const long long *valid,
                                                int nv, const float tf7[7], const int margin_centre3[3]) {
-  if (!m || m->attached || !tf7 || !margin_centre3 || nc < 0 || ns < 0 || nv < 0 || (nc > 0 && !corner_ds) || (ns > 0 && !surf_ds) || (nv > 0 && !valid))
+  LIO_ENTER(m);
+  if (m->attached || !tf7 || !margin_centre3 || nc < 0 || ns < 0 || nv < 0 || (nc > 0 && !corner_ds) || (ns > 0 && !surf_ds) || (nv > 0 && !valid))
     return LIO_ERR_INVALID;
   if (nc > m->max_points || ns > m->max_points || nv > 125) return LIO_ERR_CAPACITY;
   std::vector<size_t> v(valid, valid + nv);
@@ -645,7 +643,6 @@ extern "C" int lio_pm_update_map_database_host(lio_pm *m, const float *corner_ds
     if (valid[i] < 0 || valid[i] >= kCubes) return LIO_ERR_INVALID;
     for (int k = 0; k < i; ++k) if (valid[k] == valid[i]) return LIO_ERR_INVALID;
   }
-  LIO_CUDA_OK(cudaSetDevice(m->device));
   cudaStream_t st = m->stream;
   const int n_ds[2] = {nc, ns};
   if (nc > 0) LIO_CUDA_OK(cudaMemcpyAsync(m->d_ds[0], corner_ds, sizeof(float4) * nc, cudaMemcpyHostToDevice, st));
@@ -657,7 +654,8 @@ extern "C" int lio_pm_update_map_database_host(lio_pm *m, const float *corner_ds
 }
 
 extern "C" int lio_pm_update_stats(lio_pm *m, int info4[4]) {
-  if (!m || !info4) return LIO_ERR_INVALID;
+  LIO_ENTER_HOST(m);
+  if (!info4) return LIO_ERR_INVALID;
   for (int k = 0; k < 4; ++k) info4[k] = m->upd_stats[k];
   return LIO_OK;
 }
@@ -760,12 +758,12 @@ extern "C" int lio_mb_create(const lio_mb_config *cfg, int max_points, int max_f
 }
 
 extern "C" int lio_pm_enable_publish(lio_pm *m, float map_filter_size, int max_full_points) {
-  if (!m || m->mb || m->publish || m->started || !(map_filter_size > 0) || max_full_points < 1) {
-    if (m && (m->mb || m->publish || m->started))
+  LIO_ENTER(m);
+  if (m->mb || m->publish || m->started || !(map_filter_size > 0) || max_full_points < 1) {
+    if (m->mb || m->publish || m->started)
       lio_set_last_error(__FILE__, __LINE__, "lio_pm_enable_publish: only once, on a plain PointMapping handle, before its first process call");
     return LIO_ERR_INVALID;
   }
-  LIO_CUDA_OK(cudaSetDevice(m->device));
   if (!pm_alloc_publish(m, max_full_points)) { lio_set_last_error(__FILE__, __LINE__, "lio_pm_enable_publish: allocation failed"); return LIO_ERR_CUDA; }
   m->map_leaf = map_filter_size;
   m->publish = true;
@@ -815,15 +813,14 @@ static int mb_process_map(lio_pm *m, const float4 *const src[2], const float4 *f
 
 extern "C" int lio_mb_process_map_host(lio_pm *m, const float *corner_last, int nc, const float *surf_last, int ns, const float *full_cloud, int nf,
                                        const float transform_sum7[7], float transform_tobe_mapped7[7], float transform_aft_mapped7[7], int info6[6]) {
-  if (!m || !m->mb || !transform_sum7 || nc < 0 || ns < 0 || nf < 0 || (nc > 0 && !corner_last) || (ns > 0 && !surf_last) ||
+  LIO_ENTER(m);
+  if (!m->mb || !transform_sum7 || nc < 0 || ns < 0 || nf < 0 || (nc > 0 && !corner_last) || (ns > 0 && !surf_last) ||
       (nf > 0 && !full_cloud))
     return LIO_ERR_INVALID;
   if (nc > m->max_points || ns > m->max_points || nf > m->max_full) return LIO_ERR_CAPACITY;
-  LIO_CUDA_OK(cudaSetDevice(m->device));
   const float *src[2] = {corner_last, surf_last};
   const int nin[2] = {nc, ns};
-  int rc = pm_upload(m, src, nin, full_cloud, nf);
-  if (rc != LIO_OK) return rc;
+  LIO_TRY(pm_upload(m, src, nin, full_cloud, nf));
   const float4 *dsrc[2] = {m->d_in[0], m->d_in[1]};
   const int n_max[3] = {nc, ns, nf};
   return mb_process_map(m, dsrc, m->d_full_in, m->d_cnt + 8, n_max, transform_sum7, transform_tobe_mapped7, transform_aft_mapped7, info6);
@@ -832,10 +829,10 @@ extern "C" int lio_mb_process_map_host(lio_pm *m, const float *corner_last, int 
 extern "C" int lio_mb_process_map_dev(lio_pm *m, const float *corner_dev, const float *surf_dev, const float *full_dev, const int *n3_dev,
                                       const int n3_max[3], const float transform_sum7[7], float transform_tobe_mapped7[7],
                                       float transform_aft_mapped7[7], int info6[6]) {
-  if (!m || !m->mb || !transform_sum7 || !n3_dev || !n3_max || n3_max[0] < 0 || n3_max[1] < 0 || n3_max[2] < 0 ||
+  LIO_ENTER(m);
+  if (!m->mb || !transform_sum7 || !n3_dev || !n3_max || n3_max[0] < 0 || n3_max[1] < 0 || n3_max[2] < 0 ||
       (n3_max[0] > 0 && !corner_dev) || (n3_max[1] > 0 && !surf_dev) || (n3_max[2] > 0 && !full_dev))
     return LIO_ERR_INVALID;
-  LIO_CUDA_OK(cudaSetDevice(m->device));
   const float4 *dsrc[2] = {reinterpret_cast<const float4 *>(corner_dev), reinterpret_cast<const float4 *>(surf_dev)};
   const int n_max[3] = {std::min(n3_max[0], m->max_points), std::min(n3_max[1], m->max_points), std::min(n3_max[2], m->max_full)};
   return mb_process_map(m, dsrc, reinterpret_cast<const float4 *>(full_dev), n3_dev, n_max, transform_sum7, transform_tobe_mapped7,
@@ -843,44 +840,41 @@ extern "C" int lio_mb_process_map_dev(lio_pm *m, const float *corner_dev, const 
 }
 
 extern "C" int lio_mb_surround_dev(lio_pm *m, const float **ptr, int *n) {
-  if (!m || !(m->mb || m->publish) || !ptr || !n) return LIO_ERR_INVALID;
+  LIO_ENTER_HOST(m);
+  if (!(m->mb || m->publish) || !ptr || !n) return LIO_ERR_INVALID;
   *ptr = (const float *)m->d_sur_ds.get(); *n = m->n_surround;
   return LIO_OK;
 }
 
 extern "C" int lio_mb_full_dev(lio_pm *m, const float **ptr, int *n) {
-  if (!m || !(m->mb || m->publish) || !ptr || !n) return LIO_ERR_INVALID;
+  LIO_ENTER_HOST(m);
+  if (!(m->mb || m->publish) || !ptr || !n) return LIO_ERR_INVALID;
   *ptr = (const float *)m->d_full_out.get(); *n = m->n_full;
   return LIO_OK;
 }
 
-static int mb_download(lio_pm *m, const float4 *src, int count, float *out, int cap, int *n) {
-  *n = count;
-  if (count > cap) return LIO_ERR_CAPACITY;
-  LIO_CUDA_OK(cudaSetDevice(m->device));
-  if (count > 0) LIO_CUDA_OK(cudaMemcpyAsync(out, src, sizeof(float4) * count, cudaMemcpyDeviceToHost, m->stream));
-  LIO_CUDA_OK(cudaStreamSynchronize(m->stream));
-  return LIO_OK;
-}
-
 extern "C" int lio_mb_surround_download(lio_pm *m, float *out_xyzi, int cap, int *n) {
-  if (!m || !(m->mb || m->publish) || !n || (!out_xyzi && cap > 0)) return LIO_ERR_INVALID;
-  return mb_download(m, m->d_sur_ds, m->n_surround, out_xyzi, cap, n);
+  LIO_ENTER(m);
+  if (!(m->mb || m->publish) || !n || (!out_xyzi && cap > 0)) return LIO_ERR_INVALID;
+  return read_back((float4 *)out_xyzi, m->d_sur_ds, m->n_surround, cap, m->stream, n);
 }
 
 extern "C" int lio_mb_full_download(lio_pm *m, float *out_xyzi, int cap, int *n) {
-  if (!m || !(m->mb || m->publish) || !n || (!out_xyzi && cap > 0)) return LIO_ERR_INVALID;
-  return mb_download(m, m->d_full_out, m->n_full, out_xyzi, cap, n);
+  LIO_ENTER(m);
+  if (!(m->mb || m->publish) || !n || (!out_xyzi && cap > 0)) return LIO_ERR_INVALID;
+  return read_back((float4 *)out_xyzi, m->d_full_out, m->n_full, cap, m->stream, n);
 }
 
 extern "C" int lio_pm_map_centre(lio_pm *m, int centre3[3]) {
-  if (!m || !centre3) return LIO_ERR_INVALID;
+  LIO_ENTER_HOST(m);
+  if (!centre3) return LIO_ERR_INVALID;
   centre3[0] = m->cen_l; centre3[1] = m->cen_w; centre3[2] = m->cen_h;
   return LIO_OK;
 }
 
 extern "C" int lio_pm_cube_lists(lio_pm *m, long long valid[125], long long surround[125], int n2[2]) {
-  if (!m || !n2) return LIO_ERR_INVALID;
+  LIO_ENTER_HOST(m);
+  if (!n2) return LIO_ERR_INVALID;
   n2[0] = (int)m->last_valid.size(); n2[1] = (int)m->last_surround.size();
   if (valid) for (int i = 0; i < n2[0]; ++i) valid[i] = (long long)m->last_valid[i];
   if (surround) for (int i = 0; i < n2[1]; ++i) surround[i] = (long long)m->last_surround[i];
@@ -888,24 +882,19 @@ extern "C" int lio_pm_cube_lists(lio_pm *m, long long valid[125], long long surr
 }
 
 extern "C" int lio_pm_cube_size(lio_pm *m, int cube_index, int which, int *n) {
-  if (!m || !n || cube_index < 0 || cube_index >= kCubes || which < 0 || which > 1) return LIO_ERR_INVALID;
-  LIO_CUDA_OK(cudaSetDevice(m->device));
-  int rc = pm_counts(m);
-  if (rc != LIO_OK) return rc;
+  LIO_ENTER(m);
+  if (!n || cube_index < 0 || cube_index >= kCubes || which < 0 || which > 1) return LIO_ERR_INVALID;
+  LIO_TRY(pm_counts(m));
   *n = m->cube[which][cube_index].n;
   return LIO_OK;
 }
 
 extern "C" int lio_pm_cube_download(lio_pm *m, int cube_index, int which, float *out_xyzi, int cap) {
-  if (!m || !out_xyzi || cube_index < 0 || cube_index >= kCubes || which < 0 || which > 1) return LIO_ERR_INVALID;
-  LIO_CUDA_OK(cudaSetDevice(m->device));
-  int rc = pm_counts(m);
-  if (rc != LIO_OK) return rc;
+  LIO_ENTER(m);
+  if (!out_xyzi || cube_index < 0 || cube_index >= kCubes || which < 0 || which > 1) return LIO_ERR_INVALID;
+  LIO_TRY(pm_counts(m));
   const lio_pm::Cube &c = m->cube[which][cube_index];
-  if (c.n > cap) return LIO_ERR_CAPACITY;
-  if (c.n > 0) LIO_CUDA_OK(cudaMemcpyAsync(out_xyzi, c.p, sizeof(float4) * c.n, cudaMemcpyDeviceToHost, m->stream));
-  LIO_CUDA_OK(cudaStreamSynchronize(m->stream));
-  return LIO_OK;
+  return read_back((float4 *)out_xyzi, c.p, c.n, cap, m->stream);
 }
 
 // ---- the device estimator's map after initialisation (cubemap.cuh, lio_est_attach_map) ------------------------------------
@@ -928,9 +917,7 @@ int pm_attach(lio_pm *m, int device, float corner_leaf, float surf_leaf, int ins
     lio_set_last_error(__FILE__, __LINE__, msg);
     return LIO_ERR_CAPACITY;
   }
-  LIO_CUDA_OK(cudaSetDevice(m->device));
-  int rc = pm_counts(m);
-  if (rc != LIO_OK) return rc;
+  LIO_TRY(pm_counts(m));
   if (ins_bound > m->ins_cap) {   // an accumulated surf slot exceeds 2 * max_points: new insert buffers, swapped in on success
     LIO_CUDA_OK(cudaStreamSynchronize(m->stream));
     DevMem<float4> mapped;
@@ -976,7 +963,6 @@ int pm_est_upload(lio_pm *m, const float *corner, int nc, const float *surf, int
   }
   const float *in[2] = {corner, surf};
   const int nin[2] = {nc, ns};
-  LIO_CUDA_OK(cudaSetDevice(m->device));
   if (nf > 0) LIO_CUDA_OK(cudaMemcpyAsync(m->d_full_in, full, sizeof(float4) * nf, cudaMemcpyHostToDevice, m->stream));
   int rc = pm_upload(m, in, nin, full, nf);   // full goes up above: pm_upload copies it for a map builder only
   if (rc != LIO_OK) return rc;
@@ -986,7 +972,6 @@ int pm_est_upload(lio_pm *m, const float *corner, int nc, const float *surf, int
 }
 
 int pm_est_process(lio_pm *m, const float4 *const src[2], const float4 *full, const int *n3_dev, const int n_max[3], const float sum7[7]) {
-  LIO_CUDA_OK(cudaSetDevice(m->device));
   return pm_process(m, src, full, n3_dev, n_max, sum7, nullptr, nullptr, nullptr, 0);
 }
 

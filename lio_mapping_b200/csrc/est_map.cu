@@ -24,7 +24,8 @@ k_local_gather(const LocalGather G, int *__restrict__ n_out) {
 
 // ---- /local/* clouds (Estimator.cc:474-482, :628-693, :2355-2375, :2416) ------------------------------------------------
 extern "C" int lio_est_enable_local_clouds(lio_est *e, float corner_filter_size, int max_corner_points, int max_full_points) {
-  if (!e || !(corner_filter_size > 0) || max_corner_points < 1 || max_full_points < 1) return LIO_ERR_INVALID;
+  LIO_ENTER(e);
+  if (!(corner_filter_size > 0) || max_corner_points < 1 || max_full_points < 1) return LIO_ERR_INVALID;
   if (e->lc.on || e->frames_started) {
     lio_set_last_error(__FILE__, __LINE__, "lio_est_enable_local_clouds: call it once, before the first lio_est_init_frame");
     return LIO_ERR_INVALID;
@@ -33,7 +34,6 @@ extern "C" int lio_est_enable_local_clouds(lio_est *e, float corner_filter_size,
     lio_set_last_error(__FILE__, __LINE__, "lio_est_enable_local_clouds: not supported on a sharded context");
     return LIO_ERR_INVALID;
   }
-  LIO_CUDA_OK(cudaSetDevice(e->device));
   const int W = e->W;
   LocalClouds lc;
   lc.corner_leaf = corner_filter_size;
@@ -72,12 +72,11 @@ static int lc_stage_wait(lio_est *e) {
 }
 
 extern "C" int lio_est_set_scan_clouds_host(lio_est *e, const float *corner, int nc, const float *full, int nf) {
-  if (!e || nc < 0 || nf < 0 || (nc > 0 && !corner) || (nf > 0 && !full)) return LIO_ERR_INVALID;
+  LIO_ENTER(e);
+  if (nc < 0 || nf < 0 || (nc > 0 && !corner) || (nf > 0 && !full)) return LIO_ERR_INVALID;
   if (!e->lc.on) { lio_set_last_error(__FILE__, __LINE__, "local clouds are off: call lio_est_enable_local_clouds first"); return LIO_ERR_INVALID; }
   if (nc > e->lc.cap[0] || nf > e->lc.cap[1]) { lio_set_last_error(__FILE__, __LINE__, "staged cloud exceeds the local-cloud capacity"); return LIO_ERR_CAPACITY; }
-  LIO_CUDA_OK(cudaSetDevice(e->device));
-  int rc = lc_stage_wait(e);
-  if (rc != LIO_OK) return rc;
+  LIO_TRY(lc_stage_wait(e));
   const int hn[2] = {nc, nf};
   if (nc > 0) LIO_CUDA_OK(cudaMemcpyAsync(e->lc.d_stage[0], corner, sizeof(float4) * nc, cudaMemcpyHostToDevice, e->stream));
   if (nf > 0) LIO_CUDA_OK(cudaMemcpyAsync(e->lc.d_stage[1], full, sizeof(float4) * nf, cudaMemcpyHostToDevice, e->stream));
@@ -89,11 +88,10 @@ extern "C" int lio_est_set_scan_clouds_host(lio_est *e, const float *corner, int
 
 extern "C" int lio_est_set_scan_clouds_dev(lio_est *e, const float *corner_dev, const int *nc_dev, int nc_max, const float *full_dev,
                                            const int *nf_dev, int nf_max) {
-  if (!e || !corner_dev || !nc_dev || !full_dev || !nf_dev || nc_max < 0 || nf_max < 0) return LIO_ERR_INVALID;
+  LIO_ENTER(e);
+  if (!corner_dev || !nc_dev || !full_dev || !nf_dev || nc_max < 0 || nf_max < 0) return LIO_ERR_INVALID;
   if (!e->lc.on) { lio_set_last_error(__FILE__, __LINE__, "local clouds are off: call lio_est_enable_local_clouds first"); return LIO_ERR_INVALID; }
-  LIO_CUDA_OK(cudaSetDevice(e->device));
-  int rc = lc_stage_wait(e);
-  if (rc != LIO_OK) return rc;
+  LIO_TRY(lc_stage_wait(e));
   const float *src[2] = {corner_dev, full_dev};
   const int *n_src[2] = {nc_dev, nf_dev};
   const int n_max[2] = {std::min(nc_max, e->lc.cap[0]), std::min(nf_max, e->lc.cap[1])};   // counts are clamped on the device
@@ -153,7 +151,7 @@ int lc_join(lio_est *e) {
 }
 
 extern "C" int lio_est_local_clouds_dev(lio_est *e, const float *ptr[3], const int **n_dev, int n_host[3]) {
-  if (!e) return LIO_ERR_INVALID;
+  LIO_ENTER_HOST(e);
   if (!e->lc.on) { lio_set_last_error(__FILE__, __LINE__, "local clouds are off"); return LIO_ERR_INVALID; }
   for (int w = 0; w < 3; ++w) {
     if (ptr) ptr[w] = reinterpret_cast<const float *>(e->lc.d_pub[w].get());
@@ -163,17 +161,13 @@ extern "C" int lio_est_local_clouds_dev(lio_est *e, const float *ptr[3], const i
   return LIO_OK;
 }
 extern "C" int lio_est_local_clouds_download(lio_est *e, int which, float *out, int cap, int *n) {
-  if (!e || !n || which < 0 || which > 2 || (cap > 0 && !out)) return LIO_ERR_INVALID;
+  LIO_ENTER(e);
+  if (!n || which < 0 || which > 2 || (cap > 0 && !out)) return LIO_ERR_INVALID;
   if (!e->lc.on) { lio_set_last_error(__FILE__, __LINE__, "local clouds are off"); return LIO_ERR_INVALID; }
-  LIO_CUDA_OK(cudaSetDevice(e->device));
   if (e->lc.pending) LIO_CUDA_OK(cudaStreamSynchronize(e->lc.stream));   // inside an open scan: the forked work has not been joined yet
-  LIO_CUDA_OK(cudaMemcpyAsync(e->h_counts + e->W + 12, e->lc.d_pub_n + which, sizeof(int), cudaMemcpyDeviceToHost, e->stream));
-  LIO_CUDA_OK(cudaStreamSynchronize(e->stream));
-  *n = e->h_counts[e->W + 12];
-  if (*n > cap) return LIO_ERR_CAPACITY;
-  if (*n > 0) LIO_CUDA_OK(cudaMemcpyAsync(out, e->lc.d_pub[which], sizeof(float4) * *n, cudaMemcpyDeviceToHost, e->stream));
-  LIO_CUDA_OK(cudaStreamSynchronize(e->stream));
-  return LIO_OK;
+  int *count = e->h_counts + e->W + 12;
+  LIO_TRY(read_back(count, e->lc.d_pub_n + which, 1, 1, e->stream));
+  return read_back((float4 *)out, e->lc.d_pub[which], *count, cap, e->stream, n);
 }
 
 // ---- the global cube map after initialisation (lio_est_attach_map; Estimator.cc:703-723, :776-812) -------------------------
@@ -266,7 +260,6 @@ void AttachedMap::detach() {
 
 // The estimator's side of both attaches: the map-step events, the W == O de-skew copies, and the handle's own checks (pm_attach).
 static int attach_common(lio_est *e, lio_pm *pm, bool fresh) {
-  LIO_CUDA_OK(cudaSetDevice(e->device));
   const bool keep = e->W == e->O && map_deskew(e);
   AttachedMap map;
   bool ok = create(map.ev_in) && create(map.ev_done);
@@ -282,7 +275,8 @@ static int attach_common(lio_est *e, lio_pm *pm, bool fresh) {
 }
 
 extern "C" int lio_est_attach_map(lio_est *e, lio_pm *pm) {
-  if (!e || !pm) return LIO_ERR_INVALID;
+  LIO_ENTER(e);
+  if (!pm) return LIO_ERR_INVALID;
   const char *why = nullptr;
   if (e->map.pm) why = "lio_est_attach_map: a map is attached already";
   else if (!e->tmp_pre) why = "lio_est_attach_map: call it after lio_est_finish_init";
@@ -295,7 +289,7 @@ extern "C" int lio_est_attach_map(lio_est *e, lio_pm *pm) {
 }
 
 extern "C" int lio_est_map_poses(lio_est *e, float tobe7[7], float aft7[7], float insert7[7], int info4[4]) {
-  if (!e) return LIO_ERR_INVALID;
+  LIO_ENTER_HOST(e);
   if (!e->map.pm) { lio_set_last_error(__FILE__, __LINE__, "no map attached (lio_est_attach_map)"); return LIO_ERR_INVALID; }
   auto out = [](const lio::TwistF &t, float *o) { if (o) { o[0] = t.qx; o[1] = t.qy; o[2] = t.qz; o[3] = t.qw; o[4] = t.px; o[5] = t.py; o[6] = t.pz; } };
   out(*pm_tobe(e->map.pm), tobe7);
@@ -319,7 +313,7 @@ void predict_state_w(lio_est *e) {
 }
 
 static int attach_mapping(lio_est *e, lio_pm *pm, bool imu) {
-  if (!e || !pm) return LIO_ERR_INVALID;
+  if (!pm) return LIO_ERR_INVALID;
   const char *why = nullptr;
   if (e->map.pm) why = "a map is attached already";
   else if (e->frames_started || e->tmp_pre) why = "call it before lio_est_init_frame / lio_est_finish_init and the first scan";
@@ -343,11 +337,11 @@ static int attach_mapping(lio_est *e, lio_pm *pm, bool imu) {
   return LIO_OK;
 }
 
-extern "C" int lio_est_attach_mapping(lio_est *e, lio_pm *pm) { return attach_mapping(e, pm, false); }
-extern "C" int lio_est_attach_imu_mapping(lio_est *e, lio_pm *pm) { return attach_mapping(e, pm, true); }
+extern "C" int lio_est_attach_mapping(lio_est *e, lio_pm *pm) { LIO_ENTER(e); return attach_mapping(e, pm, false); }
+extern "C" int lio_est_attach_imu_mapping(lio_est *e, lio_pm *pm) { LIO_ENTER(e); return attach_mapping(e, pm, true); }
 
 extern "C" int lio_est_enable_extrinsic_calibration(lio_est *e) {
-  if (!e) return LIO_ERR_INVALID;
+  LIO_ENTER_HOST(e);
   const char *why = nullptr;
   if (!e->cfg.imu_factor || e->extrinsic_stage != 2) why = "lio_est_enable_extrinsic_calibration needs imu_factor = 1 and estimate_extrinsic = 2";
   else if (e->calib.on) why = "lio_est_enable_extrinsic_calibration: call it once";
@@ -538,12 +532,10 @@ static int compact_check(lio_est *e, double stamp) {
 
 static int compact_dev(lio_est *e, const float *corner_dev, const float *surf_dev, const float *full_dev, const int *n3_dev, const int n3_max[3],
                        const float transform_sum7[7], double stamp) {
-  if (!e || !n3_dev || !n3_max || !transform_sum7 || n3_max[0] < 0 || n3_max[1] < 0 || n3_max[2] < 0 || (n3_max[0] > 0 && !corner_dev) ||
+  if (!n3_dev || !n3_max || !transform_sum7 || n3_max[0] < 0 || n3_max[1] < 0 || n3_max[2] < 0 || (n3_max[0] > 0 && !corner_dev) ||
       (n3_max[1] > 0 && !surf_dev) || (n3_max[2] > 0 && !full_dev))
     return LIO_ERR_INVALID;
-  int rc = compact_check(e, stamp);
-  if (rc != LIO_OK) return rc;
-  LIO_CUDA_OK(cudaSetDevice(e->device));
+  LIO_TRY(compact_check(e, stamp));
   int n_max[3];
   pm_est_caps(e->map.pm, n3_max, n_max);
   const float4 *src[3] = {reinterpret_cast<const float4 *>(corner_dev), reinterpret_cast<const float4 *>(surf_dev), reinterpret_cast<const float4 *>(full_dev)};
@@ -552,10 +544,9 @@ static int compact_dev(lio_est *e, const float *corner_dev, const float *surf_de
 
 static int compact_host(lio_est *e, const float *corner, int nc, const float *surf, int ns, const float *full, int nf, const float transform_sum7[7],
                         double stamp) {
-  if (!e || !transform_sum7 || nc < 0 || ns < 0 || nf < 0 || (nc > 0 && !corner) || (ns > 0 && !surf) || (nf > 0 && !full)) return LIO_ERR_INVALID;
+  if (!transform_sum7 || nc < 0 || ns < 0 || nf < 0 || (nc > 0 && !corner) || (ns > 0 && !surf) || (nf > 0 && !full)) return LIO_ERR_INVALID;
   int rc = compact_check(e, stamp);
   if (rc != LIO_OK) return rc;
-  LIO_CUDA_OK(cudaSetDevice(e->device));
   if (e->poisoned || nf > e->lc.cap[1] || (map_deskew(e) && nc > e->lc.cap[0])) {
     const int n_max[3] = {nc, ns, nf};
     return compact_common(e, nullptr, nullptr, n_max, transform_sum7, stamp);
@@ -571,35 +562,39 @@ static int compact_host(lio_est *e, const float *corner, int nc, const float *su
 
 extern "C" int lio_est_process_compact_dev(lio_est *e, const float *corner_dev, const float *surf_dev, const float *full_dev, const int *n3_dev,
                                            const int n3_max[3], const float transform_sum7[7]) {
+  LIO_ENTER(e);
   return compact_dev(e, corner_dev, surf_dev, full_dev, n3_dev, n3_max, transform_sum7, std::nan(""));
 }
 extern "C" int lio_est_process_compact_host(lio_est *e, const float *corner, int nc, const float *surf, int ns, const float *full, int nf,
                                             const float transform_sum7[7]) {
+  LIO_ENTER(e);
   return compact_host(e, corner, nc, surf, ns, full, nf, transform_sum7, std::nan(""));
 }
 extern "C" int lio_est_process_compact_stamped_dev(lio_est *e, const float *corner_dev, const float *surf_dev, const float *full_dev,
                                                    const int *n3_dev, const int n3_max[3], const float transform_sum7[7], double stamp) {
+  LIO_ENTER(e);
   if (std::isnan(stamp)) return LIO_ERR_INVALID;
   return compact_dev(e, corner_dev, surf_dev, full_dev, n3_dev, n3_max, transform_sum7, stamp);
 }
 extern "C" int lio_est_process_compact_stamped_host(lio_est *e, const float *corner, int nc, const float *surf, int ns, const float *full, int nf,
                                                     const float transform_sum7[7], double stamp) {
+  LIO_ENTER(e);
   if (std::isnan(stamp)) return LIO_ERR_INVALID;
   return compact_host(e, corner, nc, surf, ns, full, nf, transform_sum7, stamp);
 }
 
 extern "C" int lio_est_compact_status(lio_est *e, int info4[4]) {
-  if (!e || !info4) return LIO_ERR_INVALID;
-  int rc = compact_check(e);
-  if (rc != LIO_OK) return rc;
+  LIO_ENTER_HOST(e);
+  if (!info4) return LIO_ERR_INVALID;
+  LIO_TRY(compact_check(e));
   for (int k = 0; k < 4; ++k) info4[k] = e->mapping.compact_info[k];
   return LIO_OK;
 }
 
 extern "C" int lio_est_imu_init_status(lio_est *e, int info4[4], double g3[3], double R_WI9[9], double *states16) {
-  if (!e || !info4) return LIO_ERR_INVALID;
-  int rc = compact_check(e);
-  if (rc != LIO_OK) return rc;
+  LIO_ENTER_HOST(e);
+  if (!info4) return LIO_ERR_INVALID;
+  LIO_TRY(compact_check(e));
   info4[0] = e->mapping.attempts; info4[1] = e->mapping.outcome; info4[2] = e->mapping.attempted ? 1 : 0; info4[3] = e->mapping.inited ? 1 : 0;
   if (g3) for (int k = 0; k < 3; ++k) g3[k] = e->g_vec[k];
   if (R_WI9) for (int a = 0; a < 3; ++a) for (int b = 0; b < 3; ++b) R_WI9[3 * a + b] = e->mapping.R_WI(a, b);
@@ -609,7 +604,8 @@ extern "C" int lio_est_imu_init_status(lio_est *e, int info4[4], double g3[3], d
 }
 
 extern "C" int lio_est_extrinsic_calib_status(lio_est *e, int info4[4], double sv4[4]) {
-  if (!e || !info4) return LIO_ERR_INVALID;
+  LIO_ENTER_HOST(e);
+  if (!info4) return LIO_ERR_INVALID;
   info4[0] = e->calib.runs; info4[1] = e->calib.result; info4[2] = e->calib.ran ? 1 : 0; info4[3] = e->extrinsic_stage;
   if (sv4) for (int k = 0; k < 4; ++k) sv4[k] = e->calib.sv[k];
   return LIO_OK;

@@ -105,12 +105,10 @@ extern "C" int lio_est_create(const lio_est_config *cfg, int device, void *cuda_
     lio_set_last_error(__FILE__, __LINE__, "lio_est_create: configuration outside supported limits");
     return LIO_ERR_INVALID;
   }
-  if (lio_device_count() <= 0) return LIO_ERR_NO_DEVICE;
-  LIO_CUDA_OK(cudaSetDevice(device));
   std::unique_ptr<lio_est> e(new (std::nothrow) lio_est());
   if (!e) return LIO_ERR_INVALID;
+  LIO_TRY(select_device(device, &e->sm_count));
   e->cfg = *cfg; e->W = W; e->O = O; e->device = device; e->stream = (cudaStream_t)cuda_stream;
-  cudaDeviceGetAttribute(&e->sm_count, cudaDevAttrMultiProcessorCount, device);
   e->noise.acc_n = cfg->acc_n; e->noise.gyr_n = cfg->gyr_n; e->noise.acc_w = cfg->acc_w; e->noise.gyr_w = cfg->gyr_w; e->noise.g_norm = cfg->g_norm;
   e->g_vec = V3(0, 0, -cfg->g_norm);
   e->extrinsic_stage = cfg->estimate_extrinsic;
@@ -186,26 +184,28 @@ extern "C" int lio_est_create(const lio_est_config *cfg, int device, void *cuda_
 }
 
 extern "C" int lio_est_set_extrinsic(lio_est *e, const float tf7[7]) {
-  if (!e || !tf7) return LIO_ERR_INVALID;
+  LIO_ENTER_HOST(e);
+  if (!tf7) return LIO_ERR_INVALID;
   for (int k = 0; k < 4; ++k) e->tlb_q[k] = tf7[k];
   for (int k = 0; k < 3; ++k) e->tlb_p[k] = tf7[4 + k];
   return LIO_OK;
 }
 extern "C" int lio_est_get_extrinsic(lio_est *e, float tf7[7]) {
-  if (!e || !tf7) return LIO_ERR_INVALID;
+  LIO_ENTER_HOST(e);
+  if (!tf7) return LIO_ERR_INVALID;
   for (int k = 0; k < 4; ++k) tf7[k] = e->tlb_q[k];
   for (int k = 0; k < 3; ++k) tf7[4 + k] = e->tlb_p[k];
   return LIO_OK;
 }
 
 extern "C" int lio_est_init_frame(lio_est *e, int k, const double s[16], const float *surf_ds, int n, lio_pim *pim) {
-  if (!e || !s || k < 0 || k >= e->W || n < 0 || (n > 0 && !surf_ds)) return LIO_ERR_INVALID;
+  LIO_ENTER(e);
+  if (!s || k < 0 || k >= e->W || n < 0 || (n > 0 && !surf_ds)) return LIO_ERR_INVALID;
   if (n > e->cfg.max_frame_points) return LIO_ERR_CAPACITY;
   if (e->lc.on && !e->lc.staged) {
     lio_set_last_error(__FILE__, __LINE__, "local clouds are on: stage the frame's corner / full cloud with lio_est_set_scan_clouds_* first");
     return LIO_ERR_INVALID;
   }
-  LIO_CUDA_OK(cudaSetDevice(e->device));
   e->frames_started = true;
   if (e->mapping.on) { lio_set_last_error(__FILE__, __LINE__, "a mapping is attached: the window starts from the mapped poses"); return LIO_ERR_INVALID; }
   if (e->lc.on) {   // the pre-initialisation corner_stack_ / full_stack_ entries (Estimator.cc:474-482), verbatim
@@ -230,7 +230,8 @@ extern "C" int lio_est_init_frame(lio_est *e, int k, const double s[16], const f
 }
 
 extern "C" int lio_est_finish_init(lio_est *e, const double a[3], const double g[3]) {
-  if (!e || !a || !g || e->mapping.on) return LIO_ERR_INVALID;
+  LIO_ENTER_HOST(e);
+  if (!a || !g || e->mapping.on) return LIO_ERR_INVALID;
   const int W = e->W;
   e->Ps[W] = e->Ps[W - 1]; e->Rs[W] = e->Rs[W - 1]; e->Vs[W] = e->Vs[W - 1]; e->Bas[W] = e->Bas[W - 1]; e->Bgs[W] = e->Bgs[W - 1];
   e->acc_last = V3(a); e->gyr_last = V3(g);
@@ -241,7 +242,8 @@ extern "C" int lio_est_finish_init(lio_est *e, const double a[3], const double g
 }
 
 extern "C" int lio_est_process_imu(lio_est *e, double dt, const double a[3], const double g[3], double stamp) {
-  if (!e || !a || !g) return LIO_ERR_INVALID;
+  LIO_ENTER_HOST(e);
+  if (!a || !g) return LIO_ERR_INVALID;
   const V3 acc(a), gyr(g);
   if (!e->first_imu) { e->first_imu = true; e->acc_last = acc; e->gyr_last = gyr; }
   if (!e->tmp_pre) return LIO_ERR_INVALID;
@@ -271,10 +273,10 @@ extern "C" int lio_est_process_imu(lio_est *e, double dt, const double a[3], con
 }
 
 extern "C" int lio_est_process_imu_batch(lio_est *e, int n, const double *dt, const double *acc3, const double *gyr3, const double *stamp) {
-  if (!e || n < 0 || (n > 0 && (!dt || !acc3 || !gyr3 || !stamp))) return LIO_ERR_INVALID;
+  LIO_ENTER_HOST(e);
+  if (n < 0 || (n > 0 && (!dt || !acc3 || !gyr3 || !stamp))) return LIO_ERR_INVALID;
   for (int k = 0; k < n; ++k) {
-    const int rc = lio_est_process_imu(e, dt[k], acc3 + 3 * k, gyr3 + 3 * k, stamp[k]);
-    if (rc != LIO_OK) return rc;
+    LIO_TRY(lio_est_process_imu(e, dt[k], acc3 + 3 * k, gyr3 + 3 * k, stamp[k]));
   }
   return LIO_OK;
 }
@@ -436,16 +438,15 @@ int process_scan_body(lio_est *e, const float4 *scan_dev, const int *n_dev, int 
 }
 
 extern "C" int lio_est_begin_scan(lio_est *e) {
-  if (!e) return LIO_ERR_INVALID;
+  LIO_ENTER_HOST(e);
   if (e->cfg.overlap_marginalization) marg_start(e);
   return LIO_OK;
 }
 
 // The host entries upload surf_last into d_scan and its count into d_counts[0]; the device entries read the caller's buffers.
 static int scan_host(lio_est *e, const float *surf_last, int n, bool open_only) {
-  if (!e || n < 0 || (n > 0 && !surf_last)) return LIO_ERR_INVALID;
+  if (n < 0 || (n > 0 && !surf_last)) return LIO_ERR_INVALID;
   if (n > e->cfg.max_scan_points) return LIO_ERR_CAPACITY;
-  LIO_CUDA_OK(cudaSetDevice(e->device));
   if (n > 0) LIO_CUDA_OK(cudaMemcpyAsync(e->d_scan, surf_last, sizeof(float4) * n, cudaMemcpyHostToDevice, e->stream));
   e->h_counts[e->W + 8] = n;
   LIO_CUDA_OK(cudaMemcpyAsync(e->d_counts, e->h_counts + e->W + 8, sizeof(int), cudaMemcpyHostToDevice, e->stream));
@@ -453,22 +454,23 @@ static int scan_host(lio_est *e, const float *surf_last, int n, bool open_only) 
 }
 
 static int scan_dev(lio_est *e, const float *surf_last_dev, const int *n_dev, int n_max, bool open_only) {
-  if (!e || !surf_last_dev || !n_dev || n_max <= 0) return LIO_ERR_INVALID;
+  if (!surf_last_dev || !n_dev || n_max <= 0) return LIO_ERR_INVALID;
   if (n_max > e->cfg.max_scan_points) n_max = e->cfg.max_scan_points;   // the voxel filter clamps *n_dev to n_max on the device
-  LIO_CUDA_OK(cudaSetDevice(e->device));
   return process_scan_common(e, reinterpret_cast<const float4 *>(surf_last_dev), n_dev, n_max, open_only);
 }
 
-extern "C" int lio_est_process_scan_host(lio_est *e, const float *surf_last, int n) { return scan_host(e, surf_last, n, false); }
+extern "C" int lio_est_process_scan_host(lio_est *e, const float *surf_last, int n) { LIO_ENTER(e); return scan_host(e, surf_last, n, false); }
 
 extern "C" int lio_est_process_scan_dev(lio_est *e, const float *surf_last_dev, const int *n_dev, int n_max) {
+  LIO_ENTER(e);
   return scan_dev(e, surf_last_dev, n_dev, n_max, false);
 }
 
 // ---- stepwise API: the phases of ProcessLaserOdom / SolveOptimization one by one ----------------------------------------
-extern "C" int lio_est_open_scan_host(lio_est *e, const float *surf_last, int n) { return scan_host(e, surf_last, n, true); }
+extern "C" int lio_est_open_scan_host(lio_est *e, const float *surf_last, int n) { LIO_ENTER(e); return scan_host(e, surf_last, n, true); }
 
 extern "C" int lio_est_open_scan_dev(lio_est *e, const float *surf_last_dev, const int *n_dev, int n_max) {
+  LIO_ENTER(e);
   return scan_dev(e, surf_last_dev, n_dev, n_max, true);
 }
 
@@ -497,9 +499,8 @@ static void store_parameters(const lio_est *e, double *pose, double *sb, double 
 }
 
 extern "C" int lio_est_get_parameters(lio_est *e, double *pose, double *speed_bias, double *ex) {
-  if (!e) return LIO_ERR_INVALID;
-  int rc = need_open(e);
-  if (rc != LIO_OK) return rc;
+  LIO_ENTER_HOST(e);
+  LIO_TRY(need_open(e));
   store_parameters(e, pose, speed_bias, ex);
   return LIO_OK;
 }
@@ -508,10 +509,10 @@ extern "C" int lio_est_last_normal_equations(lio_est *e, double *H, double *g, d
 
 extern "C" int lio_est_assemble(lio_est *e, const double *pose, const double *speed_bias, const double *ex, double *H, double *g,
                                 double *cost, int *n) {
-  if (!e || !n) return LIO_ERR_INVALID;
+  LIO_ENTER(e);
+  if (!n) return LIO_ERR_INVALID;
   int rc = need_open(e);
   if (rc != LIO_OK) return rc;
-  LIO_CUDA_OK(cudaSetDevice(e->device));
   // evaluate at the caller's blocks, then put the estimator's own blocks back
   std::vector<double> kp(7 * (e->O + 1)), ks(9 * (e->O + 1));
   double kx[7];
@@ -538,10 +539,10 @@ extern "C" int lio_est_assemble(lio_est *e, const double *pose, const double *sp
 }
 
 extern "C" int lio_est_solve(lio_est *e, double *pose, double *speed_bias, double *ex, int max_iter, double summary[8]) {
-  if (!e || max_iter < 0) return LIO_ERR_INVALID;
+  LIO_ENTER(e);
+  if (max_iter < 0) return LIO_ERR_INVALID;
   int rc = need_open(e);
   if (rc != LIO_OK) return rc;
-  LIO_CUDA_OK(cudaSetDevice(e->device));
   if (e->use_dev_solver && max_iter > 22) return LIO_ERR_INVALID;
   load_parameters(e, pose, speed_bias, ex);
   rc = scan_solve(e, max_iter);
@@ -556,10 +557,9 @@ extern "C" int lio_est_solve(lio_est *e, double *pose, double *speed_bias, doubl
 }
 
 extern "C" int lio_est_close_scan(lio_est *e, const double *pose, const double *speed_bias, const double *ex) {
-  if (!e) return LIO_ERR_INVALID;
+  LIO_ENTER(e);
   int rc = need_open(e);
   if (rc != LIO_OK) return rc;
-  LIO_CUDA_OK(cudaSetDevice(e->device));
   load_parameters(e, pose, speed_bias, ex);
   rc = scan_close_window(e);
   return rc != LIO_OK ? scan_failed(e, rc) : rc;
@@ -571,7 +571,8 @@ extern "C" int lio_est_frame_owner(int frame_rel, int world) {  // frame_rel in 
 }
 
 extern "C" int lio_est_set_shard(lio_est *e, int rank, int world, lio_allreduce_fn fn, void *user) {
-  if (!e || world < 1 || rank < 0 || rank >= world) return LIO_ERR_INVALID;
+  LIO_ENTER_HOST(e);
+  if (world < 1 || rank < 0 || rank >= world) return LIO_ERR_INVALID;
   if (e->lc.on) { lio_set_last_error(__FILE__, __LINE__, "local clouds are not supported on a sharded context"); return LIO_ERR_INVALID; }
   e->rank = rank; e->world = world; e->allreduce = fn; e->allreduce_user = user;
   e->px.npeers = 0;
@@ -581,14 +582,16 @@ extern "C" int lio_est_set_shard(lio_est *e, int rank, int world, lio_allreduce_
 }
 
 extern "C" int lio_est_exchange_buffer(lio_est *e, void **dev_ptr, size_t *bytes) {
-  if (!e || !dev_ptr) return LIO_ERR_INVALID;
+  LIO_ENTER_HOST(e);
+  if (!dev_ptr) return LIO_ERR_INVALID;
   *dev_ptr = e->px.xbuf;
   if (bytes) *bytes = kXBytes;
   return LIO_OK;
 }
 
 extern "C" int lio_est_set_peers(lio_est *e, int world, void *const *peer_ptrs) {
-  if (!e || !peer_ptrs || world != e->world || world < 2 || world > kMaxPeers || e->lc.on) return LIO_ERR_INVALID;
+  LIO_ENTER_HOST(e);
+  if (!peer_ptrs || world != e->world || world < 2 || world > kMaxPeers || e->lc.on) return LIO_ERR_INVALID;
   for (int r = 0; r < world; ++r) {
     e->px.peer_base[r] = r == e->rank ? e->px.xbuf : static_cast<char *>(peer_ptrs[r]);
     if (!e->px.peer_base[r]) return LIO_ERR_INVALID;
@@ -598,14 +601,16 @@ extern "C" int lio_est_set_peers(lio_est *e, int world, void *const *peer_ptrs) 
 }
 
 extern "C" int lio_est_feature_slab(lio_est *e, void **dev_ptr, size_t *bytes) {
-  if (!e || !dev_ptr) return LIO_ERR_INVALID;
+  LIO_ENTER_HOST(e);
+  if (!dev_ptr) return LIO_ERR_INVALID;
   *dev_ptr = e->px.fslab;
   if (bytes) *bytes = e->px.fslab_bytes;
   return LIO_OK;
 }
 
 extern "C" int lio_est_set_feature_peers(lio_est *e, int world, void *const *peer_slabs) {
-  if (!e || !peer_slabs || world != e->world || world < 2 || world > kMaxPeers || e->lc.on) return LIO_ERR_INVALID;
+  LIO_ENTER_HOST(e);
+  if (!peer_slabs || world != e->world || world < 2 || world > kMaxPeers || e->lc.on) return LIO_ERR_INVALID;
   if (e->window_open) { lio_set_last_error(__FILE__, __LINE__, "lio_est_set_feature_peers inside an open scan"); return LIO_ERR_INVALID; }
   for (int r = 0; r < world; ++r) {
     e->px.fpeer_base[r] = r == e->rank ? e->px.fslab : static_cast<char *>(peer_slabs[r]);
@@ -641,7 +646,8 @@ extern "C" int lio_ipc_close(void *dev_ptr) {
 
 // ---- getters --------------------------------------------------------------------------------------
 extern "C" int lio_est_get_states(lio_est *e, double *out) {
-  if (!e || !out) return LIO_ERR_INVALID;
+  LIO_ENTER_HOST(e);
+  if (!out) return LIO_ERR_INVALID;
   for (int k = 0; k <= e->W; ++k) {
     double *s = out + 16 * k;
     Q q = fromR(e->Rs[k]);
@@ -652,7 +658,8 @@ extern "C" int lio_est_get_states(lio_est *e, double *out) {
 }
 
 extern "C" int lio_est_summary(lio_est *e, double *o) {
-  if (!e || !o) return LIO_ERR_INVALID;
+  LIO_ENTER_HOST(e);
+  if (!o) return LIO_ERR_INVALID;
   const bool has_prior = e->prior.valid || e->mjob.stashed || e->mjob.running;  // does not force the pending algebra
   for (int k = 0; k < 32; ++k) o[k] = 0;
   o[0] = e->summary.iterations; o[1] = e->summary.successful_steps; o[2] = e->summary.termination;
@@ -668,56 +675,50 @@ extern "C" int lio_est_summary(lio_est *e, double *o) {
 }
 
 extern "C" int lio_est_feature_count(lio_est *e, int frame, int *n) {
-  if (!e || !n || frame < 0 || frame > e->W) return LIO_ERR_INVALID;
+  LIO_ENTER_HOST(e);
+  if (!n || frame < 0 || frame > e->W) return LIO_ERR_INVALID;
   *n = e->h_feat_n[frame];
   return LIO_OK;
 }
 
 extern "C" int lio_est_get_features(lio_est *e, int frame, float *pts4, float *coef4, int32_t *src, int cap) {
-  if (!e || frame < 0 || frame > e->W) return LIO_ERR_INVALID;
+  LIO_ENTER(e);
+  if (frame < 0 || frame > e->W) return LIO_ERR_INVALID;
   const int n = e->h_feat_n[frame];
   if (n > cap) return LIO_ERR_CAPACITY;
   if (n == 0) return LIO_OK;
-  LIO_CUDA_OK(cudaSetDevice(e->device));
   const FeatureOut &f = e->feats[frame];
-  if (pts4) LIO_CUDA_OK(cudaMemcpyAsync(pts4, f.pts, sizeof(float4) * n, cudaMemcpyDeviceToHost, e->stream));
-  if (coef4) LIO_CUDA_OK(cudaMemcpyAsync(coef4, f.coef, sizeof(float4) * n, cudaMemcpyDeviceToHost, e->stream));
-  if (src) LIO_CUDA_OK(cudaMemcpyAsync(src, f.src, sizeof(int) * n, cudaMemcpyDeviceToHost, e->stream));
-  LIO_CUDA_OK(cudaStreamSynchronize(e->stream));
+  if (pts4) LIO_TRY(read_back((float4 *)pts4, f.pts, n, cap, e->stream));
+  if (coef4) LIO_TRY(read_back((float4 *)coef4, f.coef, n, cap, e->stream));
+  if (src) LIO_TRY(read_back((int *)src, f.src, n, cap, e->stream));
   return LIO_OK;
 }
 
 extern "C" int lio_est_map_size(lio_est *e, int *n) {
-  if (!e || !n) return LIO_ERR_INVALID;
+  LIO_ENTER_HOST(e);
+  if (!n) return LIO_ERR_INVALID;
   *n = e->h_map_n;
   return LIO_OK;
 }
 extern "C" int lio_est_get_map(lio_est *e, float *out, int cap) {
-  if (!e || !out) return LIO_ERR_INVALID;
-  if (e->h_map_n > cap) return LIO_ERR_CAPACITY;
-  LIO_CUDA_OK(cudaSetDevice(e->device));
-  if (e->h_map_n > 0) LIO_CUDA_OK(cudaMemcpyAsync(out, e->d_map, sizeof(float4) * e->h_map_n, cudaMemcpyDeviceToHost, e->stream));
-  LIO_CUDA_OK(cudaStreamSynchronize(e->stream));
-  return LIO_OK;
+  LIO_ENTER(e);
+  if (!out) return LIO_ERR_INVALID;
+  return read_back((float4 *)out, e->d_map, e->h_map_n, cap, e->stream);
 }
 extern "C" int lio_est_frame_size(lio_est *e, int frame, int *n) {
-  if (!e || !n || frame < 0 || frame > e->W) return LIO_ERR_INVALID;
-  LIO_CUDA_OK(cudaSetDevice(e->device));
-  LIO_CUDA_OK(cudaMemcpyAsync(n, e->d_slot_n + e->slot_of[frame], sizeof(int), cudaMemcpyDeviceToHost, e->stream));
-  LIO_CUDA_OK(cudaStreamSynchronize(e->stream));
-  return LIO_OK;
+  LIO_ENTER(e);
+  if (!n || frame < 0 || frame > e->W) return LIO_ERR_INVALID;
+  return read_back(n, e->d_slot_n + e->slot_of[frame], 1, 1, e->stream);
 }
 extern "C" int lio_est_get_frame(lio_est *e, int frame, float *out, int cap) {
+  LIO_ENTER(e);
   int n = 0;
-  int rc = lio_est_frame_size(e, frame, &n);
-  if (rc != LIO_OK) return rc;
-  if (n > cap) return LIO_ERR_CAPACITY;
-  if (n > 0) LIO_CUDA_OK(cudaMemcpyAsync(out, e->slot_ptr[e->slot_of[frame]], sizeof(float4) * n, cudaMemcpyDeviceToHost, e->stream));
-  LIO_CUDA_OK(cudaStreamSynchronize(e->stream));
-  return LIO_OK;
+  LIO_TRY(lio_est_frame_size(e, frame, &n));
+  return read_back((float4 *)out, e->slot_ptr[e->slot_of[frame]], n, cap, e->stream);
 }
 extern "C" int lio_est_get_local_transform(lio_est *e, int frame, float tf7[7]) {
-  if (!e || !tf7 || frame < 0 || frame > e->W) return LIO_ERR_INVALID;
+  LIO_ENTER_HOST(e);
+  if (!tf7 || frame < 0 || frame > e->W) return LIO_ERR_INVALID;
   const TransformF &t = e->local_tf[frame];
   tf7[0] = t.qx; tf7[1] = t.qy; tf7[2] = t.qz; tf7[3] = t.qw; tf7[4] = t.px; tf7[5] = t.py; tf7[6] = t.pz;
   return LIO_OK;
@@ -725,7 +726,8 @@ extern "C" int lio_est_get_local_transform(lio_est *e, int frame, float tf7[7]) 
 // /local_laser_odom (Estimator.cc:725-742): rot = Quaterniond(Rs_[pivot] * transform_lb.rot.inverse()), pos = Ps_[pivot] - rot *
 // transform_lb.pos with transform_lb = transform_lb_.cast<double>(), rounded to float like LaserOdometryHandler (PointMapping.cc:267-282)
 extern "C" int lio_est_local_laser_odom(lio_est *e, float tf7[7]) {
-  if (!e || !tf7) return LIO_ERR_INVALID;
+  LIO_ENTER_HOST(e);
+  if (!tf7) return LIO_ERR_INVALID;
   const int pivot = e->W - e->O;
   const Tw t = lidar_pose(e->Ps[pivot], e->Rs[pivot], tlb_double(e));
   tf7[0] = (float)t.rot.x; tf7[1] = (float)t.rot.y; tf7[2] = (float)t.rot.z; tf7[3] = (float)t.rot.w;
@@ -733,13 +735,15 @@ extern "C" int lio_est_local_laser_odom(lio_est *e, float tf7[7]) {
   return LIO_OK;
 }
 extern "C" int lio_est_prior_dim(lio_est *e, int *n) {
-  if (!e || !n) return LIO_ERR_INVALID;
+  LIO_ENTER_HOST(e);
+  if (!n) return LIO_ERR_INVALID;
   prior_join(e);
   *n = e->prior.valid ? e->prior.n : 0;
   return LIO_OK;
 }
 extern "C" int lio_est_get_prior(lio_est *e, double *Hp, double *bp) {
-  if (!e || !Hp || !bp) return LIO_ERR_INVALID;
+  LIO_ENTER_HOST(e);
+  if (!Hp || !bp) return LIO_ERR_INVALID;
   prior_join(e);
   if (!e->prior.valid) return LIO_ERR_INVALID;
   std::memcpy(Hp, e->prior.Hp.d.data(), sizeof(double) * e->prior.n * e->prior.n);
@@ -747,13 +751,13 @@ extern "C" int lio_est_get_prior(lio_est *e, double *Hp, double *bp) {
   return LIO_OK;
 }
 extern "C" int lio_est_last_normal_equations(lio_est *e, double *H, double *g, double *cost, int *n) {
-  if (!e || !n) return LIO_ERR_INVALID;
+  LIO_ENTER(e);
+  if (!n) return LIO_ERR_INVALID;
   if (!e->have_H0) { *n = 0; return LIO_OK; }
   if (e->use_dev_solver) {
     // device layout keeps the 6 extrinsic slots; report the reduced system when the extrinsic was constant
     const int nf = 15 * (e->O + 1) + 6, nr = e->ex_constant ? nf - 6 : nf;
     *n = nr;
-    LIO_CUDA_OK(cudaSetDevice(e->device));
     std::vector<double> Hf((size_t)nf * nf), gf(nf);
     LIO_CUDA_OK(cudaMemcpy(Hf.data(), e->ds.H0, sizeof(double) * nf * nf, cudaMemcpyDeviceToHost));
     LIO_CUDA_OK(cudaMemcpy(gf.data(), e->ds.g0, sizeof(double) * nf, cudaMemcpyDeviceToHost));
@@ -772,15 +776,16 @@ extern "C" int lio_est_last_launches(lio_est *e) { return e ? e->launches : 0; }
 extern "C" const char *lio_est_last_error(lio_est *e) { return e ? e->err : "null handle"; }
 
 extern "C" int lio_est_solver_trace(lio_est *e, long long *out, int cap) {
-  if (!e || !out || cap < 24 * 16 + 4 * 28 + 4) return LIO_ERR_INVALID;
+  LIO_ENTER(e);
+  if (!out || cap < 24 * 16 + 4 * 28 + 4) return LIO_ERR_INVALID;
   if (!e->use_dev_solver) { std::memset(out, 0, sizeof(long long) * (24 * 16 + 4 * 28 + 4)); return LIO_OK; }
-  LIO_CUDA_OK(cudaSetDevice(e->device));
   LIO_CUDA_OK(cudaMemcpy(out, reinterpret_cast<const char *>(e->ds.st.get()) + offsetof(DevSolveState, dbg), sizeof(long long) * (24 * 16 + 4 * 28 + 4), cudaMemcpyDeviceToHost));
   return LIO_OK;
 }
 
 extern "C" int lio_est_kernel_profile(lio_est *e, double out[8], int reset) {
-  if (!e || !out) return LIO_ERR_INVALID;
+  LIO_ENTER_HOST(e);
+  if (!out) return LIO_ERR_INVALID;
   out[0] = e->asm_ms_sum; out[1] = (double)e->asm_launch_count; out[2] = (double)e->asm_feat_sum; out[3] = 32.0;
   out[4] = e->knn_ms_sum; out[5] = (double)e->knn_launch_count; out[6] = (double)e->knn_query_sum; out[7] = 128.0;
   if (reset) { e->asm_ms_sum = 0; e->asm_launch_count = 0; e->asm_feat_sum = 0; e->knn_ms_sum = 0; e->knn_launch_count = 0; e->knn_query_sum = 0; }
@@ -790,8 +795,7 @@ extern "C" int lio_est_kernel_profile(lio_est *e, double out[8], int reset) {
 // ---- C-ABI: TransformToEnd on an explicit host array (parity entry) ----------------------------------------------
 extern "C" int lio_transform_to_end_host(float *cloud, int n, const float *tf7_es, float time_factor, int device) {
   if (!cloud || !tf7_es || n < 0) return LIO_ERR_INVALID;
-  if (lio_device_count() <= 0) return LIO_ERR_NO_DEVICE;
-  LIO_CUDA_OK(cudaSetDevice(device));
+  LIO_TRY(select_device(device));
   if (n == 0) return LIO_OK;
   DevBufs db;
   float4 *d = nullptr;

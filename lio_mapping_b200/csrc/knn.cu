@@ -597,8 +597,7 @@ static int features_batch_host(const float *map, int K, float cell_size, float m
 static int features_one_frame(const float *map, int K, const float *surf, int M, const float *tf7, float min_match_sq_dis,
                               float min_plane_dis, float *pts4, float *coef4, int32_t *src, int *n_out, int device, int fit) {
   if (!map || !surf || !tf7 || !n_out || K < 0 || M < 0) return LIO_ERR_INVALID;
-  if (lio_device_count() <= 0) return LIO_ERR_NO_DEVICE;
-  LIO_CUDA_OK(cudaSetDevice(device));
+  LIO_TRY(select_device(device));
   *n_out = 0;
   if (M == 0) return LIO_OK;
   const float cell = sqrtf(min_match_sq_dis) * (1.0f + 1.0f / 1024.0f);   // cell edge >= search radius (with margin, see header)
@@ -628,8 +627,7 @@ extern "C" int lio_cell_hash_build_host(const float *map, int n, int n_max, int 
   if (!map || !eff_size || !keys || !count || !start || !cellpts || n < 0 || n > n_max || cap_points < 1 || n_max > cap_points ||
       !(cell_size > 0.f) || prev_n < 0 || prev_n > cap_points || (prev_n > 0 && !prev_map))
     return LIO_ERR_INVALID;
-  if (lio_device_count() <= 0) return LIO_ERR_NO_DEVICE;
-  LIO_CUDA_OK(cudaSetDevice(device));
+  LIO_TRY(select_device(device));
   DevBufs d;
   CellHash h;
   float4 *d_map = nullptr;
@@ -671,8 +669,7 @@ extern "C" int lio_calculate_features_batch_host(const float *map, int K, float 
         (long long)base + (long long)per * n_per_frame[k] > out_cap_per_frame[k])
       return LIO_ERR_INVALID;
   }
-  if (lio_device_count() <= 0) return LIO_ERR_NO_DEVICE;
-  LIO_CUDA_OK(cudaSetDevice(device));
+  LIO_TRY(select_device(device));
   return features_batch_host(map, K, cell_size, min_match_sq_dis, min_plane_dis, nframes, surf_cat, n_per_frame, n_bound_per_frame,
                              tf7_per_frame, append_per_frame, zaxis3, fit, done_flag_value, work_queries, out_cap_per_frame, pts4_cat,
                              coef4_cat, src_cat, count_per_frame);

@@ -114,14 +114,12 @@ extern "C" int lio_node_create(const lio_node_config *cfg, int device, void *cud
     lio_set_last_error(__FILE__, __LINE__, "lio_node_create: sensor_type must be 16, 32, 64 or 320; odom_io, capacities and max_pending >= 1");
     return LIO_ERR_INVALID;
   }
-  if (lio_device_count() <= 0) return LIO_ERR_NO_DEVICE;
-  LIO_CUDA_OK(cudaSetDevice(device));
   std::unique_ptr<lio_node> nd(new (std::nothrow) lio_node());
   if (!nd) return LIO_ERR_INVALID;
+  LIO_TRY(select_device(device, &nd->sm_count));
   nd->cfg = *cfg;
   nd->device = device;
   nd->stream = (cudaStream_t)cuda_stream;
-  cudaDeviceGetAttribute(&nd->sm_count, cudaDevAttrMultiProcessorCount, device);
   nd->pairing = lio::MeasurementPairing(cfg->msg_time_delay);
   // processor_node.cc:64-74: the sensor presets (320 = RS-32 with the ring field)
   lio_pp_config pc = cfg->pp;
@@ -254,10 +252,10 @@ static int refuse_poisoned(lio_node *nd) {
 }
 
 extern "C" int lio_node_push_imu_batch(lio_node *nd, int n, const double *stamp, const double *acc3, const double *gyr3) {
-  if (!nd || n < 0 || (n > 0 && (!stamp || !acc3 || !gyr3))) return LIO_ERR_INVALID;
+  LIO_ENTER(nd);
+  if (n < 0 || (n > 0 && (!stamp || !acc3 || !gyr3))) return LIO_ERR_INVALID;
   int rc = refuse_poisoned(nd);
   if (rc != LIO_OK) return rc;
-  LIO_CUDA_OK(cudaSetDevice(nd->device));
   for (int k = 0; k < n; ++k) {
     lio::ImuMsg m{stamp[k], {acc3[3 * k], acc3[3 * k + 1], acc3[3 * k + 2]}, {gyr3[3 * k], gyr3[3 * k + 1], gyr3[3 * k + 2]}};
     if (nd->pairing.push_imu(m) && (rc = drain(nd)) != LIO_OK) return rc;
@@ -266,16 +264,17 @@ extern "C" int lio_node_push_imu_batch(lio_node *nd, int n, const double *stamp,
 }
 
 extern "C" int lio_node_push_imu(lio_node *nd, double stamp, const double acc[3], const double gyr[3]) {
+  LIO_ENTER(nd);
   if (!acc || !gyr) return LIO_ERR_INVALID;
   return lio_node_push_imu_batch(nd, 1, &stamp, acc, gyr);
 }
 
 extern "C" int lio_node_push_sweep_dev(lio_node *nd, const float *xyzi_dev, const uint16_t *rings_dev, int n, double stamp) {
-  if (!nd || n < 0 || (n > 0 && !xyzi_dev) || std::isnan(stamp)) return LIO_ERR_INVALID;
+  LIO_ENTER(nd);
+  if (n < 0 || (n > 0 && !xyzi_dev) || std::isnan(stamp)) return LIO_ERR_INVALID;
   int rc = check_rings(nd, rings_dev != nullptr, n);
   if (rc != LIO_OK) return rc;
   if ((rc = refuse_poisoned(nd)) != LIO_OK) return rc;
-  if (rc != LIO_OK) return rc;
   if (n > nd->cfg.max_points) return LIO_ERR_CAPACITY;
   // the io_ratio gate of the coming odometry call (PointOdometry.cc:302-310, :725): the first call never publishes
   const long long c = nd->po_calls;
@@ -284,7 +283,6 @@ extern "C" int lio_node_push_sweep_dev(lio_node *nd, const float *xyzi_dev, cons
     lio_set_last_error(__FILE__, __LINE__, "lio_node: the /compact_data queue is full (max_pending messages wait for IMU)");
     return LIO_ERR_CAPACITY;
   }
-  LIO_CUDA_OK(cudaSetDevice(nd->device));
   rc = ring_sensor(nd) ? lio_pp_process_dev_ring(nd->pp, xyzi_dev, rings_dev, n) : lio_pp_process_dev(nd->pp, xyzi_dev, n);
   if (rc != LIO_OK) return rc;
   static const int which[5] = {LIO_PP_CORNER_SHARP, LIO_PP_CORNER_LESS_SHARP, LIO_PP_SURF_FLAT, LIO_PP_SURF_LESS_FLAT, LIO_PP_CLOUD_IN_RINGS};
@@ -323,12 +321,12 @@ extern "C" int lio_node_push_sweep_dev(lio_node *nd, const float *xyzi_dev, cons
 }
 
 extern "C" int lio_node_push_sweep_host(lio_node *nd, const float *xyzi, const uint16_t *rings, int n, double stamp) {
-  if (!nd || n < 0 || (n > 0 && !xyzi) || std::isnan(stamp)) return LIO_ERR_INVALID;
+  LIO_ENTER(nd);
+  if (n < 0 || (n > 0 && !xyzi) || std::isnan(stamp)) return LIO_ERR_INVALID;
   int rc = check_rings(nd, rings != nullptr, n);
   if (rc != LIO_OK) return rc;
   if ((rc = refuse_poisoned(nd)) != LIO_OK) return rc;
   if (n > nd->cfg.max_points) return LIO_ERR_CAPACITY;
-  LIO_CUDA_OK(cudaSetDevice(nd->device));
   if (!nd->d_in && !lio::alloc(nd->d_in, nd->cfg.max_points)) return LIO_ERR_CUDA;
   if (rings && !nd->d_rings && !lio::alloc(nd->d_rings, nd->cfg.max_points)) return LIO_ERR_CUDA;
   if (n > 0) {
@@ -342,7 +340,8 @@ extern "C" int lio_node_push_sweep_host(lio_node *nd, const float *xyzi, const u
 }
 
 extern "C" int lio_node_status(lio_node *nd, lio_node_info *s) {
-  if (!nd || !s) return LIO_ERR_INVALID;
+  LIO_ENTER_HOST(nd);
+  if (!s) return LIO_ERR_INVALID;
   s->sweeps = nd->sweeps;
   s->published = nd->published;
   s->processed = nd->processed;
@@ -357,7 +356,7 @@ extern "C" int lio_node_status(lio_node *nd, lio_node_info *s) {
 }
 
 extern "C" int lio_node_handles(lio_node *nd, lio_pp **pp, lio_po **po, lio_est **est, lio_pm **pm) {
-  if (!nd) return LIO_ERR_INVALID;
+  LIO_ENTER_HOST(nd);
   if (pp) *pp = nd->pp;
   if (po) *po = nd->po;
   if (est) *est = nd->est;
@@ -366,7 +365,8 @@ extern "C" int lio_node_handles(lio_node *nd, lio_pp **pp, lio_po **po, lio_est 
 }
 
 extern "C" int lio_node_enable_map_builder(lio_node *nd, const lio_mb_config *cfg) {
-  if (!nd || !cfg) return LIO_ERR_INVALID;
+  LIO_ENTER(nd);
+  if (!cfg) return LIO_ERR_INVALID;
   if (nd->mb || nd->sweeps > 0 || nd->poisoned) {
     lio_set_last_error(__FILE__, __LINE__, "lio_node_enable_map_builder: once, before the first sweep");
     return LIO_ERR_INVALID;
@@ -374,14 +374,13 @@ extern "C" int lio_node_enable_map_builder(lio_node *nd, const lio_mb_config *cf
   const float *ptr[3];
   const int *n_dev = nullptr;
   int n_host[3];
-  int rc = lio_est_local_clouds_dev(nd->est, ptr, &n_dev, n_host);
-  if (rc != LIO_OK) return rc;
-  LIO_CUDA_OK(cudaSetDevice(nd->device));
+  LIO_TRY(lio_est_local_clouds_dev(nd->est, ptr, &n_dev, n_host));
   return make(nd->mb, [&](lio_pm **h) { return lio_mb_create(cfg, std::max(n_host[0], n_host[1]), n_host[2], nd->device, nd->stream, h); });
 }
 
 extern "C" int lio_node_map_builder(lio_node *nd, lio_pm **mb) {
-  if (!nd || !mb) return LIO_ERR_INVALID;
+  LIO_ENTER_HOST(nd);
+  if (!mb) return LIO_ERR_INVALID;
   *mb = nd->mb;
   if (nd->mb) return LIO_OK;
   lio_set_last_error(__FILE__, __LINE__, "lio_node_map_builder: no map builder (lio_node_enable_map_builder)");
@@ -389,7 +388,8 @@ extern "C" int lio_node_map_builder(lio_node *nd, lio_pm **mb) {
 }
 
 extern "C" int lio_node_map_builder_poses(lio_node *nd, double *stamp, float *tobe7, float *aft7, int *info6, int cap, int *n) {
-  if (!nd || !n || cap < 0) return LIO_ERR_INVALID;
+  LIO_ENTER_HOST(nd);
+  if (!n || cap < 0) return LIO_ERR_INVALID;
   if (!nd->mb) {
     lio_set_last_error(__FILE__, __LINE__, "lio_node_map_builder_poses: no map builder (lio_node_enable_map_builder)");
     return LIO_ERR_INVALID;
@@ -408,7 +408,8 @@ extern "C" int lio_node_map_builder_poses(lio_node *nd, double *stamp, float *to
 }
 
 extern "C" int lio_node_attach_registered_map(lio_node *nd, lio_rm *rm, int source) {
-  if (!nd || !rm) return LIO_ERR_INVALID;
+  LIO_ENTER_HOST(nd);
+  if (!rm) return LIO_ERR_INVALID;
   const char *why = nullptr;
   if (source != LIO_NODE_MAP_ESTIMATOR && source != LIO_NODE_MAP_BUILDER) why = "lio_node_attach_registered_map: unknown source";
   else if (source == LIO_NODE_MAP_BUILDER && !nd->mb) why = "lio_node_attach_registered_map: the map builder's source needs lio_node_enable_map_builder first";

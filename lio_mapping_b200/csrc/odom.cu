@@ -270,8 +270,8 @@ extern "C" int lio_scan_to_map_host(const float *corner_map, int Kc, const float
                                     int *n_out, int *iters, int device) {
   if (!corner_map || !surf_map || !corner || !surf || !tf7 || Kc < 0 || Ks < 0 || Mc < 0 || Ms < 0 || max_iter < 0 || variant < 0 || variant > 1)
     return LIO_ERR_INVALID;
-  if (lio_device_count() <= 0) return LIO_ERR_NO_DEVICE;
-  LIO_CUDA_OK(cudaSetDevice(device));
+  int sm = 132;
+  LIO_TRY(select_device(device, &sm));
   if (n_out) *n_out = 0;
   if (iters) *iters = 0;
   if (Kc <= 10 || Ks <= 100 || max_iter == 0) return LIO_OK;  // PointMapping.cc:327-329: nothing to optimise against
@@ -279,8 +279,7 @@ extern "C" int lio_scan_to_map_host(const float *corner_map, int Kc, const float
   ScanToMapWork W;
   float4 *d_cmap = nullptr, *d_smap = nullptr, *d_corner = nullptr, *d_surf = nullptr;
   int *d_cnt = nullptr;
-  int rc = LIO_OK, sm = 132;
-  cudaDeviceGetAttribute(&sm, cudaDevAttrMultiProcessorCount, device);
+  int rc = LIO_OK;
   const int hn[2] = {Mc, Ms};
   if (W.init(Kc, Ks, Mc + Ms) != 0) { lio_set_last_error(__FILE__, __LINE__, "cudaMalloc failed"); rc = LIO_ERR_CUDA; }
   else if (!d.alloc(&d_cmap, Kc) || !d.alloc(&d_smap, Ks) || !d.alloc(&d_corner, Mc) || !d.alloc(&d_surf, Ms) || !d.alloc(&d_cnt, 2) ||
@@ -305,8 +304,8 @@ extern "C" int lio_laser_odom_host(const float *map, int K, const float *surf, i
                                    float min_plane_dis, int keep_features, int max_iter, float *pts4, float *coef4, int32_t *src,
                                    int *n_out, int *iters, int device) {
   if (!map || !surf || !tf7 || !n_out || K < 0 || M < 0 || max_iter < 0) return LIO_ERR_INVALID;
-  if (lio_device_count() <= 0) return LIO_ERR_NO_DEVICE;
-  LIO_CUDA_OK(cudaSetDevice(device));
+  int sm = 132;
+  LIO_TRY(select_device(device, &sm));
   *n_out = 0;
   if (iters) *iters = 0;
   if (M == 0 || max_iter == 0) return LIO_OK;
@@ -320,8 +319,7 @@ extern "C" int lio_laser_odom_host(const float *map, int K, const float *surf, i
   TransformF *d_tf = nullptr;
   OdomState *d_odom = nullptr;
   double *d_partial = nullptr;
-  int rc = LIO_OK, sm = 132;
-  cudaDeviceGetAttribute(&sm, cudaDevAttrMultiProcessorCount, device);
+  int rc = LIO_OK;
   const int Kc = K > 0 ? K : 1;
   const int hn[3] = {K, M, 0};
   if (h.init(Kc) != 0 || w.init(M) != 0) { lio_set_last_error(__FILE__, __LINE__, "cudaMalloc failed"); rc = LIO_ERR_CUDA; }
@@ -359,10 +357,8 @@ extern "C" int lio_odom_normal_equations_host(const float *pts4, const float *co
   if ((n > 0 && (!pts4 || !coef4)) || !tf7 || !AtA || !AtB || n < 0 || kernel < 0 || kernel > 3 || blocks < 0 || blocks > kMaxBlocks ||
       (kernel == 3 && blocks > 1))
     return LIO_ERR_INVALID;
-  if (lio_device_count() <= 0) return LIO_ERR_NO_DEVICE;
-  LIO_CUDA_OK(cudaSetDevice(device));
   int sm = 132;
-  cudaDeviceGetAttribute(&sm, cudaDevAttrMultiProcessorCount, device);
+  LIO_TRY(select_device(device, &sm));
   DevBufs d;
   float4 *d_pts = nullptr, *d_coef = nullptr;
   int *d_n = nullptr;
@@ -402,8 +398,7 @@ __global__ void k_odom_step_variant(OdomState *__restrict__ st, TransformF *__re
 extern "C" int lio_odom_step_host(int rounds, const double *AtA, const double *AtB, const int *n_feat, int variant, double delta_r_abort,
                                   double delta_t_abort, float *tf7, float *tf_per_round, int *state_out, float *matP, int device) {
   if (rounds < 0 || (rounds > 0 && (!AtA || !AtB || !n_feat)) || !tf7 || variant < 0 || variant > 3) return LIO_ERR_INVALID;
-  if (lio_device_count() <= 0) return LIO_ERR_NO_DEVICE;
-  LIO_CUDA_OK(cudaSetDevice(device));
+  LIO_TRY(select_device(device));
   DevBufs d;
   TransformF *d_tf = nullptr;
   OdomState *d_odom = nullptr;

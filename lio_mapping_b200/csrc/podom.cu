@@ -367,12 +367,10 @@ extern "C" int lio_po_destroy(lio_po *p) {
 extern "C" int lio_po_create(float scan_period, int io_ratio, int num_max_iterations, int max_feature_points, int max_full_points, int device,
                              void *cuda_stream, lio_po **out) {
   if (!out || !(scan_period > 0) || num_max_iterations < 0 || max_feature_points < 16 || max_full_points < 16) return LIO_ERR_INVALID;
-  if (lio_device_count() <= 0) return LIO_ERR_NO_DEVICE;
-  LIO_CUDA_OK(cudaSetDevice(device));
   std::unique_ptr<lio_po> p(new (std::nothrow) lio_po());
   if (!p) return LIO_ERR_INVALID;
+  LIO_TRY(select_device(device, &p->sm));
   p->device = device; p->stream = (cudaStream_t)cuda_stream;
-  cudaDeviceGetAttribute(&p->sm, cudaDevAttrMultiProcessorCount, device);
   p->time_factor = 1 / scan_period; p->io_ratio = io_ratio; p->max_iter = num_max_iterations;
   p->cap_feat = max_feature_points; p->cap_full = max_full_points;
   const int nf = max_feature_points;
@@ -386,7 +384,7 @@ extern "C" int lio_po_create(float scan_period, int io_ratio, int num_max_iterat
 }
 
 extern "C" int lio_po_set_enable_odom(lio_po *p, int enable) {   // the /enable_odom service, PointOdometry.cc:126-131
-  if (!p) return LIO_ERR_INVALID;
+  LIO_ENTER_HOST(p);
   p->enable_odom = enable > 0;
   return LIO_OK;
 }
@@ -466,14 +464,14 @@ static int po_run(lio_po *p, const float4 *sharp, int n_sharp, int n_less_sharp,
 extern "C" int lio_po_process_host(lio_po *p, const float *sharp, int n_sharp, const float *less_sharp, int n_less_sharp, const float *flat,
                                    int n_flat, const float *less_flat, int n_less_flat, const float *full, int n_full, float transform_sum7[7],
                                    float transform_es7[7], int info4[4]) {
-  if (!p || n_sharp < 0 || n_less_sharp < 0 || n_flat < 0 || n_less_flat < 0 || n_full < 0 || (n_sharp && !sharp) || (n_less_sharp && !less_sharp) ||
+  LIO_ENTER(p);
+  if (n_sharp < 0 || n_less_sharp < 0 || n_flat < 0 || n_less_flat < 0 || n_full < 0 || (n_sharp && !sharp) || (n_less_sharp && !less_sharp) ||
       (n_flat && !flat) || (n_less_flat && !less_flat) || (n_full && !full))
     return LIO_ERR_INVALID;
   if (std::max(std::max(n_sharp, n_less_sharp), std::max(n_flat, n_less_flat)) > p->cap_feat || n_full > p->cap_full) {
     lio_set_last_error(__FILE__, __LINE__, "lio_po_process_host: a cloud exceeds the capacity given to lio_po_create");
     return LIO_ERR_CAPACITY;
   }
-  LIO_CUDA_OK(cudaSetDevice(p->device));
   cudaStream_t st = p->stream;
   const float *src[5] = {sharp, less_sharp, flat, less_flat, full};
   float4 *dst[5] = {p->d_sharp, p->d_less_sharp, p->d_flat, p->d_less_flat, p->d_full};
@@ -488,14 +486,14 @@ extern "C" int lio_po_process_host(lio_po *p, const float *sharp, int n_sharp, c
 
 extern "C" int lio_po_process_dev(lio_po *p, const float *const clouds_dev[5], const int *const n_dev[5], const int n_max[5], float transform_sum7[7],
                                   float transform_es7[7], int info4[4]) {
-  if (!p || !clouds_dev || !n_dev || !n_max) return LIO_ERR_INVALID;
+  LIO_ENTER(p);
+  if (!clouds_dev || !n_dev || !n_max) return LIO_ERR_INVALID;
   for (int k = 0; k < 5; ++k)
     if (n_max[k] < 0 || !n_dev[k] || (n_max[k] > 0 && !clouds_dev[k])) return LIO_ERR_INVALID;
   if (std::max(std::max(n_max[0], n_max[1]), std::max(n_max[2], n_max[3])) > p->cap_feat || n_max[4] > p->cap_full) {
     lio_set_last_error(__FILE__, __LINE__, "lio_po_process_dev: a bound n_max exceeds the capacity given to lio_po_create");
     return LIO_ERR_CAPACITY;
   }
-  LIO_CUDA_OK(cudaSetDevice(p->device));
   cudaStream_t st = p->stream;
   PoStage sg;
   for (int k = 0; k < 5; ++k) sg.n[k] = n_dev[k];
@@ -516,7 +514,8 @@ extern "C" int lio_po_process_dev(lio_po *p, const float *const clouds_dev[5], c
 }
 
 extern "C" int lio_po_clouds_dev(lio_po *p, const float *ptr[3], const int **n_dev, int n_host[3]) {
-  if (!p || !ptr || !n_dev || !n_host) return LIO_ERR_INVALID;
+  LIO_ENTER_HOST(p);
+  if (!ptr || !n_dev || !n_host) return LIO_ERR_INVALID;
   ptr[0] = (const float *)p->d_last_corner.get(); ptr[1] = (const float *)p->d_last_surf.get(); ptr[2] = (const float *)p->d_full.get();
   *n_dev = p->d_pub_n;
   n_host[0] = p->n_last_corner; n_host[1] = p->n_last_surf; n_host[2] = p->n_full;
@@ -533,31 +532,29 @@ static int po_cloud(lio_po *p, int which, const float4 **d, int *n) {
 }
 
 extern "C" int lio_po_cloud_size(lio_po *p, int which, int *n) {
+  LIO_ENTER_HOST(p);
   const float4 *d;
-  if (!p || !n) return LIO_ERR_INVALID;
+  if (!n) return LIO_ERR_INVALID;
   return po_cloud(p, which, &d, n);
 }
 
 extern "C" int lio_po_cloud_download(lio_po *p, int which, float *out_xyzi, int cap) {
+  LIO_ENTER(p);
   const float4 *d;
   int n = 0;
-  if (!p || !out_xyzi) return LIO_ERR_INVALID;
+  if (!out_xyzi) return LIO_ERR_INVALID;
   if (po_cloud(p, which, &d, &n) != LIO_OK) return LIO_ERR_INVALID;
-  if (n > cap) return LIO_ERR_CAPACITY;
-  LIO_CUDA_OK(cudaSetDevice(p->device));
-  if (n) LIO_CUDA_OK(cudaMemcpyAsync(out_xyzi, d, sizeof(float4) * n, cudaMemcpyDeviceToHost, p->stream));
-  LIO_CUDA_OK(cudaStreamSynchronize(p->stream));
-  return LIO_OK;
+  return read_back((float4 *)out_xyzi, d, n, cap, p->stream);
 }
 
 // the /compact_data payload of the sweep just processed (:732-762): 3 header points, then corner || surf || full
 extern "C" int lio_po_compact_data(lio_po *p, float *out_xyzi, int cap_points, int *n_points) {
-  if (!p || !out_xyzi || !n_points) return LIO_ERR_INVALID;
+  LIO_ENTER(p);
+  if (!out_xyzi || !n_points) return LIO_ERR_INVALID;
   if (!p->published) { lio_set_last_error(__FILE__, __LINE__, "lio_po_compact_data: the last sweep was not published (io_ratio gate or first sweep)"); return LIO_ERR_INVALID; }
   const int total = 3 + p->n_last_corner + p->n_last_surf + p->n_full;
   *n_points = total;
   if (total > cap_points) return LIO_ERR_CAPACITY;
-  LIO_CUDA_OK(cudaSetDevice(p->device));
   float *o = out_xyzi;
   o[0] = p->sum.px; o[1] = p->sum.py; o[2] = p->sum.pz; o[3] = 0.f;
   o[4] = p->sum.qx; o[5] = p->sum.qy; o[6] = p->sum.qz; o[7] = p->sum.qw;
@@ -566,10 +563,9 @@ extern "C" int lio_po_compact_data(lio_po *p, float *out_xyzi, int cap_points, i
   const float4 *src[3] = {p->d_last_corner, p->d_last_surf, p->d_full};
   const int cnt[3] = {p->n_last_corner, p->n_last_surf, p->n_full};
   for (int k = 0; k < 3; ++k) {
-    if (cnt[k]) LIO_CUDA_OK(cudaMemcpyAsync(o, src[k], sizeof(float4) * cnt[k], cudaMemcpyDeviceToHost, p->stream));
+    LIO_TRY(read_back((float4 *)o, src[k], cnt[k], cnt[k], p->stream));
     o += 4 * (size_t)cnt[k];
   }
-  LIO_CUDA_OK(cudaStreamSynchronize(p->stream));
   return LIO_OK;
 }
 
@@ -577,10 +573,10 @@ extern "C" int lio_po_last_launches(lio_po *p) { return p ? p->launches : 0; }
 
 // test aid: the match indices of the last search (kind 0: 2 per sharp point, kind 1: 3 per flat point)
 extern "C" int lio_po_matches(lio_po *p, int kind, int32_t *out, int cap_queries) {
-  if (!p || !out || (kind != 0 && kind != 1)) return LIO_ERR_INVALID;
+  LIO_ENTER(p);
+  if (!out || (kind != 0 && kind != 1)) return LIO_ERR_INVALID;
   const int nq = kind == 0 ? p->n_sharp : p->n_flat, per = kind == 0 ? 2 : 3;
   if (nq > cap_queries) return LIO_ERR_CAPACITY;
-  LIO_CUDA_OK(cudaSetDevice(p->device));
   if (nq) LIO_CUDA_OK(cudaMemcpy(out, kind == 0 ? p->d_idx_c : p->d_idx_s, sizeof(int) * per * nq, cudaMemcpyDeviceToHost));
   return LIO_OK;
 }

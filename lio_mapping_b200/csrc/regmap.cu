@@ -298,7 +298,6 @@ extern "C" int lio_rm_destroy(lio_rm *m) {
 
 // One cloud already in HBM, after an optional upload of a host cloud into the scratch (host_src != nullptr).
 static int rm_insert(lio_rm *m, const float4 *src, const float *host_src, int n) {
-  LIO_CUDA_OK(cudaSetDevice(m->device));
   cudaStream_t st = m->stream;
   m->inserts += 1; m->offered += n;
   int launches = 0;
@@ -342,48 +341,42 @@ int rm_device(const lio_rm *m) { return m->device; }
 cudaStream_t rm_stream(const lio_rm *m) { return m->stream; }
 
 extern "C" int lio_rm_insert_dev(lio_rm *m, const float *xyzi_dev, int n) {
-  if (!m || n < 0 || (n > 0 && !xyzi_dev)) return LIO_ERR_INVALID;
+  LIO_ENTER(m);
+  if (n < 0 || (n > 0 && !xyzi_dev)) return LIO_ERR_INVALID;
   return rm_insert(m, reinterpret_cast<const float4 *>(xyzi_dev), nullptr, n);
 }
 
 extern "C" int lio_rm_insert_host(lio_rm *m, const float *xyzi, int n) {
-  if (!m || n < 0 || (n > 0 && !xyzi)) return LIO_ERR_INVALID;
+  LIO_ENTER(m);
+  if (n < 0 || (n > 0 && !xyzi)) return LIO_ERR_INVALID;
   static const float kNone[4] = {0.f, 0.f, 0.f, 0.f};
   return rm_insert(m, nullptr, n > 0 ? xyzi : kNone, n);
 }
 
-// Every host wait of the handle goes through here, so that lio_rm_stats can show that inserts make none.
-static int rm_sync(lio_rm *m) {
-  m->waits += 1;
-  LIO_CUDA_OK(cudaStreamSynchronize(m->stream));
-  return LIO_OK;
-}
-
-// Reads the state after the work enqueued so far (one wait; raw mode keeps it on the host and only waits).
+// Reads the state after the work enqueued so far (one wait; raw mode keeps it on the host and only waits).  Every host wait of the
+// handle is counted in waits, so that lio_rm_stats can show that inserts make none.
 static int rm_read_state(lio_rm *m, RmState *s) {
-  LIO_CUDA_OK(cudaSetDevice(m->device));
-  if (m->leaf > 0.f) LIO_CUDA_OK(cudaMemcpyAsync(m->h_state, m->d_state, sizeof(RmState), cudaMemcpyDeviceToHost, m->stream));
-  int rc = rm_sync(m);
-  if (rc != LIO_OK) return rc;
+  m->waits += 1;
+  LIO_TRY(read_back(m->h_state.get(), m->d_state, m->leaf > 0.f ? 1 : 0, 1, m->stream));
   *s = m->leaf > 0.f ? *m->h_state : RmState{m->n_raw, m->raw_overflow, m->n_raw, 0};
   return LIO_OK;
 }
 
 extern "C" int lio_rm_stats(lio_rm *m, long long out[8]) {
-  if (!m || !out) return LIO_ERR_INVALID;
+  LIO_ENTER(m);
+  if (!out) return LIO_ERR_INVALID;
   RmState s;
-  int rc = rm_read_state(m, &s);
-  if (rc != LIO_OK) return rc;
+  LIO_TRY(rm_read_state(m, &s));
   const long long v[8] = {m->inserts, m->offered, s.size, s.overflow, s.accepted, s.dropped, m->waits, m->last_launches};
   std::memcpy(out, v, sizeof(v));
   return LIO_OK;
 }
 
 extern "C" int lio_rm_export_dev(lio_rm *m, const float **ptr, long long *n) {
-  if (!m || !ptr || !n) return LIO_ERR_INVALID;
+  LIO_ENTER(m);
+  if (!ptr || !n) return LIO_ERR_INVALID;
   RmState s;
-  int rc = rm_read_state(m, &s);
-  if (rc != LIO_OK) return rc;
+  LIO_TRY(rm_read_state(m, &s));
   if (m->leaf == 0.f) { *ptr = (const float *)m->d_pts.get(); *n = m->n_raw; return LIO_OK; }
   if (s.size > 0) k_rm_export<<<(unsigned)rm_blocks(s.size), kRmThreads, 0, m->stream>>>(m->d_sum, m->d_cnt, s.size, m->d_export);
   LIO_CUDA_OK(cudaGetLastError());
@@ -392,18 +385,17 @@ extern "C" int lio_rm_export_dev(lio_rm *m, const float **ptr, long long *n) {
 }
 
 extern "C" int lio_rm_download(lio_rm *m, float *out, long long cap, long long *n) {
-  if (!m || !n || cap < 0 || (cap > 0 && !out)) return LIO_ERR_INVALID;
+  LIO_ENTER(m);
+  if (!n || cap < 0 || (cap > 0 && !out)) return LIO_ERR_INVALID;
   const float *p = nullptr;
-  int rc = lio_rm_export_dev(m, &p, n);
-  if (rc != LIO_OK) return rc;
+  LIO_TRY(lio_rm_export_dev(m, &p, n));
   if (*n > cap) return LIO_ERR_CAPACITY;
-  if (*n > 0) LIO_CUDA_OK(cudaMemcpyAsync(out, p, sizeof(float4) * *n, cudaMemcpyDeviceToHost, m->stream));
-  return rm_sync(m);
+  m->waits += 1;   // lio_rm_stats counts the read-back's wait
+  return read_back((float4 *)out, (const float4 *)p, *n, cap, m->stream);
 }
 
 extern "C" int lio_rm_reset(lio_rm *m) {
-  if (!m) return LIO_ERR_INVALID;
-  LIO_CUDA_OK(cudaSetDevice(m->device));
+  LIO_ENTER(m);
   return rm_clear(m);
 }
 
@@ -423,13 +415,13 @@ extern "C" int lio_pcd_write_xyzi(const char *path, const float *xyzi, long long
 }
 
 extern "C" int lio_rm_write_pcd(lio_rm *m, const char *path) {
-  if (!m || !path) return LIO_ERR_INVALID;
+  LIO_ENTER(m);
+  if (!path) return LIO_ERR_INVALID;
   const float *p = nullptr;
   long long n = 0;
-  int rc = lio_rm_export_dev(m, &p, &n);
-  if (rc != LIO_OK) return rc;
-  std::vector<float> h((size_t)n * 4);
-  if (n > 0) LIO_CUDA_OK(cudaMemcpyAsync(h.data(), p, sizeof(float4) * n, cudaMemcpyDeviceToHost, m->stream));
-  if ((rc = rm_sync(m)) != LIO_OK) return rc;
-  return lio_pcd_write_xyzi(path, h.data(), n);
+  LIO_TRY(lio_rm_export_dev(m, &p, &n));
+  std::vector<float4> h((size_t)n);
+  m->waits += 1;   // lio_rm_stats counts the read-back's wait
+  LIO_TRY(read_back(h.data(), (const float4 *)p, n, n, m->stream));
+  return lio_pcd_write_xyzi(path, (const float *)h.data(), n);
 }

@@ -24,9 +24,8 @@ int ppp_rows_launch(const float4 *pts, const float4 *coef, int n, const double *
 extern "C" int lio_ppp_evaluate_batch_host(const float *pts4, const float *coef4, int n, const double pose_pivot[7],
                                            const double pose_i[7], const double pose_ex[7], double *r_out, double *J_out, int device) {
   if (!pts4 || !coef4 || n < 0 || !pose_pivot || !pose_i || !pose_ex || !r_out || !J_out) return LIO_ERR_INVALID;
-  if (lio_device_count() <= 0) return LIO_ERR_NO_DEVICE;
+  LIO_TRY(select_device(device));
   if (n == 0) return LIO_OK;
-  LIO_CUDA_OK(cudaSetDevice(device));
   double Rt[12], M[108];
   ppp_frame_terms(pose_pivot, pose_i, pose_ex, Rt, Rt + 9, M);
   DevBufs d;
@@ -45,8 +44,8 @@ extern "C" int lio_ppp_evaluate_batch_host(const float *pts4, const float *coef4
 extern "C" int lio_asm_ppp_host(const float *pts4, const float *coef4, int n, const double R9[9], const double t3[3],
                                 double out32[32], int device) {
   if (!pts4 || !coef4 || n < 0 || !R9 || !t3 || !out32) return LIO_ERR_INVALID;
-  if (lio_device_count() <= 0) return LIO_ERR_NO_DEVICE;
-  LIO_CUDA_OK(cudaSetDevice(device));
+  int sms = 132;
+  LIO_TRY(select_device(device, &sms));
   DevBufs d;
   AsmWork w;
   float4 *dp = nullptr, *dc = nullptr;
@@ -64,8 +63,6 @@ extern "C" int lio_asm_ppp_host(const float *pts4, const float *coef4, int n, co
     std::memset(&ap, 0, sizeof(ap));
     ap.nframes = 1;
     ap.f[0].pts = dp; ap.f[0].coef = dc; ap.f[0].n = n;
-    int sms = 132;
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
     asm_plan(ap, sms);
     rc = asm_launch(ap, dRt, w, 0, nullptr);
     if (rc == LIO_OK && (!d.ok(cudaDeviceSynchronize()) || !d.down(out32, w.out, kAsmStride))) rc = LIO_ERR_CUDA;
@@ -103,8 +100,8 @@ extern "C" int lio_asm_set_fold_chunks(int chunks) {
 // launching stream.  out = {avg ms per launch, min ms, bytes per launch, launches}.
 extern "C" int lio_asm_stream_bench(long long n_features, int iters, int device, double out[4]) {
   if (n_features <= 0 || iters <= 0 || !out) return LIO_ERR_INVALID;
-  if (lio_device_count() <= 0) return LIO_ERR_NO_DEVICE;
-  LIO_CUDA_OK(cudaSetDevice(device));
+  int sms = 132;
+  LIO_TRY(select_device(device, &sms));
   const int O = 8;  // spread over 8 equal frames like a window
   const long long per = n_features / O;
   if (per <= 0 || per > 0x7fffffffLL) return LIO_ERR_INVALID;
@@ -132,8 +129,6 @@ extern "C" int lio_asm_stream_bench(long long n_features, int iters, int device,
       rc = LIO_ERR_CUDA;
   }
   if (rc == LIO_OK) {
-    int sms = 132;
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
     asm_plan(ap, sms);
     double sum = 0, mn = 1e30;
     for (int it = 0; it < iters + 3 && rc == LIO_OK; ++it) {

@@ -1530,8 +1530,7 @@ k_chol_test_x2(const double *__restrict__ A, const double *__restrict__ b, int n
 extern "C" int lio_dev_cholesky_solve_host(const double *A, const double *b, int n, double *x, int *ok, long long *prof, int device) {
   using namespace lio;
   if (!A || !b || !x || !ok || n < 1 || n > 15 * (kDsMaxOpt + 1) + 6) return LIO_ERR_INVALID;
-  if (lio_device_count() <= 0) return LIO_ERR_NO_DEVICE;
-  LIO_CUDA_OK(cudaSetDevice(device));
+  LIO_TRY(select_device(device));
   const int NB = (n + 7) / 8;
   const bool one = n <= 15 * (kDsMaxOpt1 + 1) + 6;
   const size_t smem = sizeof(double) * ((one ? (size_t)(NB * (NB + 1) / 2) * 64 : (size_t)TwoCta::kLocalTiles * 64) + (size_t)NB * 8);

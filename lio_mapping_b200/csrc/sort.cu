@@ -161,8 +161,7 @@ using namespace lio;
 extern "C" int lio_radix_sort_pairs_host(const uint32_t *keys, const uint32_t *vals, int n, int key_bits, uint32_t *keys_out,
                                          uint32_t *vals_out, int device) {
   if (n < 0 || key_bits < 1 || key_bits > 32 || (n > 0 && (!keys || !vals || !keys_out || !vals_out))) return LIO_ERR_INVALID;
-  if (lio_device_count() <= 0) return LIO_ERR_NO_DEVICE;
-  LIO_CUDA_OK(cudaSetDevice(device));
+  LIO_TRY(select_device(device));
   if (n == 0) return LIO_OK;
   DevBufs d;
   RadixSortTemp tmp;

@@ -706,8 +706,7 @@ extern "C" int lio_pp_create(const lio_pp_config *cfg, int max_points, int devic
     lio_set_last_error(__FILE__, __LINE__, "lio_pp_create: configuration outside supported limits");
     return LIO_ERR_INVALID;
   }
-  if (lio_device_count() <= 0) return LIO_ERR_NO_DEVICE;
-  LIO_CUDA_OK(cudaSetDevice(device));
+  LIO_TRY(select_device(device));
   std::unique_ptr<lio_pp> pp(new (std::nothrow) lio_pp());
   if (!pp) return LIO_ERR_INVALID;
   pp->cfg = *cfg;
@@ -750,9 +749,9 @@ extern "C" int lio_pp_destroy(lio_pp *pp) {
 }
 
 extern "C" int lio_pp_process_dev(lio_pp *pp, const float *xyzi_dev, int n) {
-  if (!pp || (!xyzi_dev && n > 0) || n < 0) return LIO_ERR_INVALID;
+  LIO_ENTER(pp);
+  if ((!xyzi_dev && n > 0) || n < 0) return LIO_ERR_INVALID;
   if (n > pp->max_points) return LIO_ERR_CAPACITY;
-  LIO_CUDA_OK(cudaSetDevice(pp->device));
   cudaStream_t st = pp->stream;
   const PPParams &P = pp->P;
   const int R = P.num_rings;
@@ -782,7 +781,6 @@ extern "C" int lio_pp_process_dev(lio_pp *pp, const float *xyzi_dev, int n) {
 
 static int pp_sync_counts(lio_pp *pp) {
   if (pp->counts_valid) return LIO_OK;
-  LIO_CUDA_OK(cudaSetDevice(pp->device));
   LIO_CUDA_OK(cudaStreamSynchronize(pp->stream));
   if (pp->h_counts[8] != 0) {
     lio_set_last_error(__FILE__, __LINE__, "stage A: a ring holds more points than the shared-memory ring kernel supports (8192)");
@@ -794,20 +792,19 @@ static int pp_sync_counts(lio_pp *pp) {
 }
 
 extern "C" int lio_pp_process_host(lio_pp *pp, const float *xyzi, int n) {
-  if (!pp || (!xyzi && n > 0) || n < 0) return LIO_ERR_INVALID;
+  LIO_ENTER(pp);
+  if ((!xyzi && n > 0) || n < 0) return LIO_ERR_INVALID;
   if (n > pp->max_points) return LIO_ERR_CAPACITY;
-  LIO_CUDA_OK(cudaSetDevice(pp->device));
   if (n > 0) LIO_CUDA_OK(cudaMemcpyAsync(pp->d_in, xyzi, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, pp->stream));
-  int rc = lio_pp_process_dev(pp, reinterpret_cast<const float *>(pp->d_in.get()), n);
-  if (rc != LIO_OK) return rc;
+  LIO_TRY(lio_pp_process_dev(pp, reinterpret_cast<const float *>(pp->d_in.get()), n));
   return pp_sync_counts(pp);
 }
 
 // PointToRing (ring-field variant, PointProcessor.cc:428-536) + ExtractFeaturePoints on device buffers; stream-ordered, no wait.
 extern "C" int lio_pp_process_dev_ring(lio_pp *pp, const float *xyzi_dev, const uint16_t *rings_dev, int n) {
-  if (!pp || ((!xyzi_dev || !rings_dev) && n > 0) || n < 0) return LIO_ERR_INVALID;
+  LIO_ENTER(pp);
+  if (((!xyzi_dev || !rings_dev) && n > 0) || n < 0) return LIO_ERR_INVALID;
   if (n > pp->max_points) return LIO_ERR_CAPACITY;
-  LIO_CUDA_OK(cudaSetDevice(pp->device));
   if (!pp->d_end_bits && !alloc(pp->d_end_bits, 1)) return LIO_ERR_CUDA;
   cudaStream_t st = pp->stream;
   const PPParams &P = pp->P;
@@ -841,23 +838,22 @@ extern "C" int lio_pp_process_dev_ring(lio_pp *pp, const float *xyzi_dev, const 
 
 // SetInputCloud(PointIR) + the device entry above; host buffers, synchronous.
 extern "C" int lio_pp_process_host_ring(lio_pp *pp, const float *xyzi, const uint16_t *rings, int n) {
-  if (!pp || ((!xyzi || !rings) && n > 0) || n < 0) return LIO_ERR_INVALID;
+  LIO_ENTER(pp);
+  if (((!xyzi || !rings) && n > 0) || n < 0) return LIO_ERR_INVALID;
   if (n > pp->max_points) return LIO_ERR_CAPACITY;
-  LIO_CUDA_OK(cudaSetDevice(pp->device));
   if (!pp->d_rings_in && !alloc(pp->d_rings_in, (size_t)pp->max_points)) return LIO_ERR_CUDA;
   if (n > 0) {
     LIO_CUDA_OK(cudaMemcpyAsync(pp->d_in, xyzi, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, pp->stream));
     LIO_CUDA_OK(cudaMemcpyAsync(pp->d_rings_in, rings, (size_t)n * sizeof(uint16_t), cudaMemcpyHostToDevice, pp->stream));
   }
-  int rc = lio_pp_process_dev_ring(pp, reinterpret_cast<const float *>(pp->d_in.get()), pp->d_rings_in, n);
-  if (rc != LIO_OK) return rc;
+  LIO_TRY(lio_pp_process_dev_ring(pp, reinterpret_cast<const float *>(pp->d_in.get()), pp->d_rings_in, n));
   return pp_sync_counts(pp);
 }
 
 extern "C" int lio_pp_cloud_sizes(lio_pp *pp, int sizes[LIO_PP_NUM_CLOUDS]) {
-  if (!pp || !sizes) return LIO_ERR_INVALID;
-  int rc = pp_sync_counts(pp);
-  if (rc != LIO_OK) return rc;
+  LIO_ENTER(pp);
+  if (!sizes) return LIO_ERR_INVALID;
+  LIO_TRY(pp_sync_counts(pp));
   sizes[0] = pp->h_counts[4]; sizes[1] = pp->h_counts[4]; sizes[2] = pp->h_counts[0]; sizes[3] = pp->h_counts[1];
   sizes[4] = pp->h_counts[2]; sizes[5] = pp->h_counts[3];
   return LIO_OK;
@@ -876,7 +872,8 @@ static const float4 *pp_cloud_ptr(lio_pp *pp, int which) {
 }
 
 extern "C" int lio_pp_cloud_dev(lio_pp *pp, int which, const float **ptr) {
-  if (!pp || !ptr) return LIO_ERR_INVALID;
+  LIO_ENTER_HOST(pp);
+  if (!ptr) return LIO_ERR_INVALID;
   const float4 *p = pp_cloud_ptr(pp, which);
   if (!p) return LIO_ERR_INVALID;
   *ptr = reinterpret_cast<const float *>(p);
@@ -884,25 +881,18 @@ extern "C" int lio_pp_cloud_dev(lio_pp *pp, int which, const float **ptr) {
 }
 
 extern "C" int lio_pp_download_cloud(lio_pp *pp, int which, float *out, int cap, int *n) {
-  if (!pp || !n) return LIO_ERR_INVALID;
+  LIO_ENTER(pp);
+  if (!n) return LIO_ERR_INVALID;
   int sizes[LIO_PP_NUM_CLOUDS];
-  int rc = lio_pp_cloud_sizes(pp, sizes);
-  if (rc != LIO_OK) return rc;
+  LIO_TRY(lio_pp_cloud_sizes(pp, sizes));
   if (which < 0 || which >= LIO_PP_NUM_CLOUDS) return LIO_ERR_INVALID;
-  *n = sizes[which];
-  if (sizes[which] > cap) return LIO_ERR_CAPACITY;
-  if (sizes[which] > 0) {
-    if (!out) return LIO_ERR_INVALID;
-    LIO_CUDA_OK(cudaMemcpyAsync(out, pp_cloud_ptr(pp, which), (size_t)sizes[which] * sizeof(float4), cudaMemcpyDeviceToHost, pp->stream));
-    LIO_CUDA_OK(cudaStreamSynchronize(pp->stream));
-  }
-  return LIO_OK;
+  return read_back((float4 *)out, pp_cloud_ptr(pp, which), sizes[which], cap, pp->stream, n);
 }
 
 extern "C" int lio_pp_download_index(lio_pp *pp, int which, int32_t *out, int cap, int *n) {
-  if (!pp || !n) return LIO_ERR_INVALID;
-  int rc = pp_sync_counts(pp);
-  if (rc != LIO_OK) return rc;
+  LIO_ENTER(pp);
+  if (!n) return LIO_ERR_INVALID;
+  LIO_TRY(pp_sync_counts(pp));
   const int *src = nullptr;
   int cnt = 0;
   switch (which) {
@@ -912,24 +902,16 @@ extern "C" int lio_pp_download_index(lio_pp *pp, int which, int32_t *out, int ca
     case LIO_PP_IDX_ORIG: src = pp->d_orig; cnt = pp->h_counts[4]; break;
     default: return LIO_ERR_INVALID;
   }
-  *n = cnt;
-  if (cnt > cap) return LIO_ERR_CAPACITY;
-  if (cnt > 0) {
-    if (!out) return LIO_ERR_INVALID;
-    LIO_CUDA_OK(cudaMemcpyAsync(out, src, (size_t)cnt * sizeof(int), cudaMemcpyDeviceToHost, pp->stream));
-    LIO_CUDA_OK(cudaStreamSynchronize(pp->stream));
-  }
-  return LIO_OK;
+  return read_back((int *)out, src, cnt, cap, pp->stream, n);
 }
 
 extern "C" int lio_pp_download_scan_ranges(lio_pp *pp, int32_t *out_2R) {
-  if (!pp || !out_2R) return LIO_ERR_INVALID;
-  int rc = pp_sync_counts(pp);
-  if (rc != LIO_OK) return rc;
+  LIO_ENTER(pp);
+  if (!out_2R) return LIO_ERR_INVALID;
+  LIO_TRY(pp_sync_counts(pp));
   const int R = pp->P.num_rings;
   int rs[kMaxRings + 1];
-  LIO_CUDA_OK(cudaMemcpyAsync(rs, pp->d_ring_start, (R + 1) * sizeof(int), cudaMemcpyDeviceToHost, pp->stream));
-  LIO_CUDA_OK(cudaStreamSynchronize(pp->stream));
+  LIO_TRY(read_back(rs, pp->d_ring_start, R + 1, kMaxRings + 1, pp->stream));
   for (int r = 0; r < R; ++r) {  // PointProcessor.cc:196-200
     out_2R[2 * r] = rs[r];
     out_2R[2 * r + 1] = rs[r + 1] > 0 ? rs[r + 1] - 1 : 0;
@@ -938,33 +920,28 @@ extern "C" int lio_pp_download_scan_ranges(lio_pp *pp, int32_t *out_2R) {
 }
 
 extern "C" int lio_pp_download_mask_labels(lio_pp *pp, uint8_t *mask, int8_t *labels, int cap) {
-  if (!pp) return LIO_ERR_INVALID;
-  int rc = pp_sync_counts(pp);
-  if (rc != LIO_OK) return rc;
+  LIO_ENTER(pp);
+  LIO_TRY(pp_sync_counts(pp));
   int n = pp->h_counts[4];
   if (n > cap) return LIO_ERR_CAPACITY;
   // rings too short to be processed (PointProcessor.cc:660) leave their slots untouched: zero-fill
-  if (n > 0) {
-    if (mask) LIO_CUDA_OK(cudaMemcpyAsync(mask, pp->d_mask, n, cudaMemcpyDeviceToHost, pp->stream));
-    if (labels) LIO_CUDA_OK(cudaMemcpyAsync(labels, pp->d_label, n, cudaMemcpyDeviceToHost, pp->stream));
-    LIO_CUDA_OK(cudaStreamSynchronize(pp->stream));
-  }
+  if (mask) LIO_TRY(read_back(mask, pp->d_mask, n, cap, pp->stream));
+  if (labels) LIO_TRY(read_back((signed char *)labels, pp->d_label, n, cap, pp->stream));
   return LIO_OK;
 }
 
 extern "C" int lio_pp_start_ori(lio_pp *pp, float *start_ori) {
-  if (!pp || !start_ori) return LIO_ERR_INVALID;
-  int rc = pp_sync_counts(pp);
-  if (rc != LIO_OK) return rc;
-  LIO_CUDA_OK(cudaMemcpyAsync(start_ori, pp->d_start_ori, sizeof(float), cudaMemcpyDeviceToHost, pp->stream));
-  LIO_CUDA_OK(cudaStreamSynchronize(pp->stream));
-  return LIO_OK;
+  LIO_ENTER(pp);
+  if (!start_ori) return LIO_ERR_INVALID;
+  LIO_TRY(pp_sync_counts(pp));
+  return read_back(start_ori, pp->d_start_ori, 1, 1, pp->stream);
 }
 
 extern "C" int lio_pp_last_launches(lio_pp *pp) { return pp ? pp->launches : 0; }
 
 extern "C" int lio_pp_cloud_count_dev(lio_pp *pp, int which, const int **n_dev) {
-  if (!pp || !n_dev) return LIO_ERR_INVALID;
+  LIO_ENTER_HOST(pp);
+  if (!n_dev) return LIO_ERR_INVALID;
   switch (which) {
     case LIO_PP_LASER_SCANS: case LIO_PP_CLOUD_IN_RINGS: *n_dev = pp->d_counts + 4; break;
     case LIO_PP_CORNER_SHARP: *n_dev = pp->d_counts + 0; break;

@@ -331,8 +331,7 @@ using namespace lio;
 
 extern "C" int lio_voxel_grid_host(const float *cloud, int n, float leaf, float *out, int cap, int *n_out, int device) {
   if ((!cloud && n > 0) || n < 0 || !n_out || !(leaf > 0)) return LIO_ERR_INVALID;
-  if (lio_device_count() <= 0) return LIO_ERR_NO_DEVICE;
-  LIO_CUDA_OK(cudaSetDevice(device));
+  LIO_TRY(select_device(device));
   *n_out = 0;
   if (n == 0) return LIO_OK;
   DevBufs d;
@@ -364,8 +363,7 @@ extern "C" int lio_seg_voxel_grid_host(const float *xyzi, const int *n_per_job, 
     total += n_per_job[j];
   }
   if (njobs > kVgMaxJobs || total >= (1LL << 30)) return LIO_ERR_CAPACITY;
-  if (lio_device_count() <= 0) return LIO_ERR_NO_DEVICE;
-  LIO_CUDA_OK(cudaSetDevice(device));
+  LIO_TRY(select_device(device));
   *index_bound_error = 0;
   DevBufs db;
   SegVoxelGrid sg;

@@ -206,11 +206,12 @@ def test_two_rank_shard_equals_single(oracle, vlp_seq, device_solver=1):
         except Exception as exc:   # pragma: no cover
             errs.append(exc)
             bar.abort()
+    # the reference first: a device-wide synchronise in a rank's callback would invalidate the reference's solver graph capture
+    for k in range(W, 8):
+        helpers.feed_scan(ref, vlp_seq, k)
     th = [threading.Thread(target=run, args=(r,)) for r in range(2)]
     for t_ in th:
         t_.start()
-    for k in range(W, 8):
-        helpers.feed_scan(ref, vlp_seq, k)
     for t_ in th:
         t_.join(timeout=300)
     assert not errs, errs
