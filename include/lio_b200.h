@@ -606,6 +606,11 @@ int lio_est_local_clouds_download(lio_est *est, int which, float *out, int cap, 
  * transform_lb = transform_lb_.cast<double>(), rounded to float as the map builder's LaserOdometryHandler keeps it
  * (PointMapping.cc:267-282): tf7 = {qx,qy,qz,qw,px,py,pz}.  Works with or without local clouds. */
 int lio_est_local_laser_odom(lio_est *est, float tf7[7]);
+/* The two poses ProcessLaserOdom's INITED branch publishes after SlideWindow, in double as nav_msgs/Odometry carries them:
+ * predict7 = /predict_laser_odom (Estimator.cc:744-758), the lidar pose of window slot W (rot = Quaterniond(Rs_.last() *
+ * transform_lb.rot.inverse()), pos = Ps_.last() - rot * transform_lb.pos); local7 = /local_laser_odom (:725-742), the same at slot
+ * W - O, i.e. lio_est_local_laser_odom before its rounding to float.  {qx,qy,qz,qw,px,py,pz}; either pointer may be NULL, not both. */
+int lio_est_laser_odom(lio_est *est, double predict7[7], double local7[7]);
 /* The global cube map after initialisation.  The reference's Estimator is a PointMapping: on every INITED scan it predicts
  * transform_tobe_mapped_ (ProcessCompactData, Estimator.cc:776-809), inserts the oldest optimised frame into the cube map
  * (UpdateMapDatabase, :703-708) and publishes (PublishResults, :721; PointMapping.cc:1210-1270).  PointMapping::Process is not run
@@ -983,6 +988,50 @@ int lio_node_enable_map_builder(lio_node *node, const lio_mb_config *cfg);
 int lio_node_map_builder(lio_node *node, lio_pm **mb);
 int lio_node_map_builder_poses(lio_node *node, double *stamp, float *tobe7, float *aft7, int *info6, int cap, int *n);
 int lio_node_attach_registered_map(lio_node *node, lio_rm *rm, int source);
+
+/* ---- The node's odometry topics: every pose the processor and estimator nodes publish, one row per publication, kept in host queues
+ * that the caller drains.  One push can release several messages and each message makes many ProcessImu calls, so the getters above
+ * (lio_est_get_states, lio_est_map_poses) only show the last of them; these queues keep every one.
+ *   lio_node_enable_odometry  opt-in: one queue per topic, each of capacity rows; a push onto a full queue drops its oldest row (a ROS
+ *                             publisher queue's behaviour, which bounds memory for a caller that never drains).  Only once, only before
+ *                             the first sweep, capacity >= 1 and not on a poisoned node; otherwise LIO_ERR_INVALID and nothing changes.
+ *                             Without it the node records nothing.  Recording reads host state only: no launch, no copy, no host wait.
+ *   row layout                16 doubles for every topic: [0] stamp, [1..7] tf7 {qx,qy,qz,qw,px,py,pz}, [8..14] the topic's extras
+ *                             (zero where it has none), [15] seq, the topic's publication count from 1 (a dropped row leaves a gap).
+ *                             Float sources are widened exactly, as nav_msgs/Odometry carries double.
+ *   topic                     publisher (reference), when, pose, extras, stamp:
+ *   LASER_ODOM_TO_INIT        PointOdometry::PublishResults (PointOdometry.cc:685-704): every odometry call but the first sweep's, which
+ *                             returns at :302-310; the pass-through after /enable_odom false still reaches :681.  transform_sum_;
+ *                             extras = transform_es_ (tf7, /laser_odom_to_last, :712-721); the sweep's stamp.
+ *   AFT_MAPPED_TO_INIT        PointMapping::PublishResults (PointMapping.cc:1255-1276): once per processed message (Process before
+ *                             INITED, decimated messages included; Estimator.cc:721 after; the rule of LIO_NODE_MAP_ESTIMATOR above).
+ *                             transform_aft_mapped_ (lio_est_map_poses aft7); the message's stamp (time_laser_odometry_, :230).
+ *   PREDICT_ODOM              Estimator::ProcessImu (Estimator.cc:406-425): after every ProcessImu call of a message that arrived INITED
+ *                             (not the start-up message's calls).  Ps_.last(), Quaterniond(Rs_.last()) (row W of lio_est_get_states);
+ *                             extras = Vs_.last() then Bas_.last() (the reference's twist.angular); the IMU message's stamp the call
+ *                             carries (:2706, :2725).
+ *   PREDICT_LASER_ODOM        ProcessLaserOdom, INITED branch after SlideWindow (:744-758), outside the opt_point_coeff_map_ size check:
+ *                             every message that arrives INITED.  lio_est_laser_odom predict7; the message's stamp.
+ *   LOCAL_LASER_ODOM          the same block (:725-742), the same messages.  lio_est_laser_odom local7; Headers_[pivot + 1] (the stamp of
+ *                             lio_node_map_builder_poses).
+ *   EXTRINSIC_LB              SolveOptimization's update_laser_imu block (:2279-2433, publish :2343-2353; every shipped YAML sets
+ *                             update_laser_imu): after every solve the estimator records (lio_est_compact_status info4[3]): the start-up
+ *                             solve (:505-517 with imu_factor = 0, :575 with imu_factor = 1) and every INITED solve.
+ *                             transform_lb_.cast<double>() after DoubleToVector (lio_est_get_extrinsic); Headers_.last().
+ *   lio_node_take_odometry    copies the min(cap, queued) oldest rows of topic into rows16 (16 doubles each), removes them, *n = the
+ *                             rows copied, *left (may be NULL) = the rows still queued.  Unknown topic, cap < 0 or no
+ *                             lio_node_enable_odometry: LIO_ERR_INVALID and nothing removed.  Works on a poisoned node. */
+enum {
+  LIO_NODE_ODOM_LASER_ODOM_TO_INIT = 0,   /* /laser_odom_to_init */
+  LIO_NODE_ODOM_AFT_MAPPED_TO_INIT = 1,   /* /aft_mapped_to_init */
+  LIO_NODE_ODOM_PREDICT_ODOM = 2,         /* /predict_odom */
+  LIO_NODE_ODOM_PREDICT_LASER_ODOM = 3,   /* /predict_laser_odom */
+  LIO_NODE_ODOM_LOCAL_LASER_ODOM = 4,     /* /local_laser_odom */
+  LIO_NODE_ODOM_EXTRINSIC_LB = 5,         /* /extrinsic_lb */
+  LIO_NODE_ODOM_TOPICS = 6
+};
+int lio_node_enable_odometry(lio_node *node, int capacity);
+int lio_node_take_odometry(lio_node *node, int topic, double *rows16, int cap, int *n, int *left);
 
 /* ------------------------------------------------------------------------------------------
  * Dense fp64 kernels of the host shell (host only; test seams).

@@ -214,6 +214,7 @@ def lib():
     L.lio_est_local_clouds_dev.argtypes = [vp, C.POINTER(vp), C.POINTER(vp), i32p]
     L.lio_est_local_clouds_download.argtypes = [vp, ip, f32p, ip, C.POINTER(ip)]
     L.lio_est_local_laser_odom.argtypes = [vp, f32p]
+    L.lio_est_laser_odom.argtypes = [vp, f64p, f64p]
     L.lio_est_attach_map.argtypes = [vp, vp]
     L.lio_est_map_poses.argtypes = [vp, f32p, f32p, f32p, i32p]
     L.lio_est_attach_mapping.argtypes = [vp, vp]
@@ -264,6 +265,8 @@ def lib():
     L.lio_node_map_builder.argtypes = [vp, C.POINTER(vp)]
     L.lio_node_map_builder_poses.argtypes = [vp, f64p, f32p, f32p, i32p, ip, C.POINTER(ip)]
     L.lio_node_attach_registered_map.argtypes = [vp, vp, ip]
+    L.lio_node_enable_odometry.argtypes = [vp, ip]
+    L.lio_node_take_odometry.argtypes = [vp, ip, vp, ip, C.POINTER(ip), C.POINTER(ip)]
     _LIB = L
     return L
 

@@ -734,6 +734,19 @@ extern "C" int lio_est_local_laser_odom(lio_est *e, float tf7[7]) {
   tf7[4] = (float)t.pos.x; tf7[5] = (float)t.pos.y; tf7[6] = (float)t.pos.z;
   return LIO_OK;
 }
+// /predict_laser_odom (Estimator.cc:744-758, state W) and /local_laser_odom (:725-742, state W - O) in double, as they are published:
+// the same lidar_pose as lio_est_local_laser_odom, not rounded
+extern "C" int lio_est_laser_odom(lio_est *e, double predict7[7], double local7[7]) {
+  LIO_ENTER_HOST(e);
+  if (!predict7 && !local7) return LIO_ERR_INVALID;
+  const Tw tlb = tlb_double(e);
+  auto out = [](const Tw &t, double *o) {
+    o[0] = t.rot.x; o[1] = t.rot.y; o[2] = t.rot.z; o[3] = t.rot.w; o[4] = t.pos.x; o[5] = t.pos.y; o[6] = t.pos.z;
+  };
+  if (predict7) out(lidar_pose(e->Ps[e->W], e->Rs[e->W], tlb), predict7);
+  if (local7) out(lidar_pose(e->Ps[e->W - e->O], e->Rs[e->W - e->O], tlb), local7);
+  return LIO_OK;
+}
 extern "C" int lio_est_prior_dim(lio_est *e, int *n) {
   LIO_ENTER_HOST(e);
   if (!n) return LIO_ERR_INVALID;

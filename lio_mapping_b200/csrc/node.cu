@@ -5,7 +5,8 @@
 // pairing and ProcessEstimation's IMU loop (measure.cc), and the /enable_odom call.  No kernel of its own: the slot copies are the
 // count-guarded copy_cloud of the estimator.  Optionally it also runs map_4D*.launch's map_builder_node on the estimator's /local/*
 // clouds (lio_node_enable_map_builder) and feeds drive maps (lio_node_attach_registered_map): the map builder's kernels and
-// lio_rm_insert_dev, enqueued on the same stream.
+// lio_rm_insert_dev, enqueued on the same stream.  With lio_node_enable_odometry it keeps every pose the two nodes publish in host
+// queues, read from host state the handles already hold.
 #include <algorithm>
 #include <cmath>
 #include <cstring>
@@ -36,6 +37,28 @@ struct DriveMap {             // an attached lio_rm and the /cloud_registered it
   lio_rm *rm;
   int source;
 };
+
+// One odometry topic (lio_node_enable_odometry): a ring of capacity rows of 16 doubles {stamp, tf7, extras7, seq}; a push onto a full
+// ring drops the oldest row, as a ROS publisher queue does
+struct OdomTopic {
+  std::vector<double> rows;
+  int head = 0, count = 0;    // the oldest row and the number queued
+  long long seq = 0;          // publications so far
+  int capacity() const { return (int)rows.size() / 16; }
+  void push(double stamp, const double tf7[7], const double *extra7) {
+    const int cap = capacity();
+    if (count == cap) { head = head + 1 == cap ? 0 : head + 1; --count; }
+    const int tail = count < cap - head ? head + count : count - (cap - head);
+    double *r = rows.data() + 16 * (size_t)tail;
+    r[0] = stamp;
+    std::memcpy(r + 1, tf7, 7 * sizeof(double));
+    for (int k = 0; k < 7; ++k) r[8 + k] = extra7 ? extra7[k] : 0.0;
+    r[15] = (double)++seq;
+    ++count;
+  }
+};
+
+static void widen7(const float *f, double *d) { for (int k = 0; k < 7; ++k) d[k] = (double)f[k]; }
 
 // The sub-handles a node creates, destroyed through their own entries (each counts as one live resource)
 template <class T, int (*Destroy)(T *)> struct DestroyHandle { void operator()(T *h) const { Destroy(h); } };
@@ -77,6 +100,9 @@ struct lio_node {
   std::deque<double> headers;          // Headers_ (Estimator.cc:441): the stamps of the last W + 1 pushed messages
   std::vector<MbRow> mb_rows;
   std::vector<DriveMap> maps;          // lio_node_attach_registered_map, in attach order
+  bool odometry = false;               // lio_node_enable_odometry
+  OdomTopic topics[LIO_NODE_ODOM_TOPICS];
+  std::vector<double> states;          // (W + 1) x 16, lio_est_get_states for /predict_odom
 };
 
 static bool ring_sensor(const lio_node *nd) { return nd->cfg.sensor_type == 320; }
@@ -196,16 +222,53 @@ static int insert_registered(lio_node *nd, int source) {
   return LIO_OK;
 }
 
+// /predict_odom after a ProcessImu call made INITED (Estimator.cc:406-425): Ps_.last(), Quaterniond(Rs_.last()), Vs_.last() and
+// Bas_.last() (the reference's twist.angular) are row W of lio_est_get_states; the stamp is the IMU message's that the call carries
+// (:2706, :2725).
+static int record_predict_odom(lio_node *nd, double stamp) {
+  LIO_TRY(lio_est_get_states(nd->est, nd->states.data()));
+  const double *s = nd->states.data() + 16 * nd->cfg.est.window_size;
+  const double tf7[7] = {s[3], s[4], s[5], s[6], s[0], s[1], s[2]};
+  const double v_ba[7] = {s[7], s[8], s[9], s[10], s[11], s[12], 0.0};
+  nd->topics[LIO_NODE_ODOM_PREDICT_ODOM].push(stamp, tf7, v_ba);
+  return LIO_OK;
+}
+
+// The estimator's publications of one processed message (see lio_node_enable_odometry), once its call has returned: /aft_mapped_to_init
+// always, /extrinsic_lb when the call solved, /predict_laser_odom and /local_laser_odom when the message arrived INITED.
+static int record_message(lio_node *nd, const Slot &s, bool was_inited, bool solved) {
+  float f7[7];
+  double tf7[7];
+  // PointMapping::PublishResults (PointMapping.cc:1255-1276): transform_aft_mapped_, stamped time_laser_odometry_ (:230)
+  LIO_TRY(lio_est_map_poses(nd->est, nullptr, f7, nullptr, nullptr));
+  widen7(f7, tf7);
+  nd->topics[LIO_NODE_ODOM_AFT_MAPPED_TO_INIT].push(s.stamp, tf7, nullptr);
+  if (solved) {   // SolveOptimization's update_laser_imu block (Estimator.cc:2343-2353): transform_lb_.cast<double>(), Headers_.last()
+    LIO_TRY(lio_est_get_extrinsic(nd->est, f7));
+    widen7(f7, tf7);
+    nd->topics[LIO_NODE_ODOM_EXTRINSIC_LB].push(nd->headers.back(), tf7, nullptr);
+  }
+  if (was_inited) {   // ProcessLaserOdom's INITED branch after SlideWindow (:725-758), outside the opt_point_coeff_map_ check
+    double local7[7];
+    LIO_TRY(lio_est_laser_odom(nd->est, tf7, local7));
+    nd->topics[LIO_NODE_ODOM_PREDICT_LASER_ODOM].push(s.stamp, tf7, nullptr);
+    nd->topics[LIO_NODE_ODOM_LOCAL_LASER_ODOM].push(nd->headers[nd->headers.size() - nd->cfg.est.opt_window_size], local7, nullptr);
+  }
+  return LIO_OK;
+}
+
 // One released message: ProcessEstimation's ProcessImu calls, then ProcessCompactData on its slot (Estimator.cc:2682-2736), then the
-// /enable_odom call of the RunInitialization success path (:542-560); with a map builder, its call when the message arrived INITED;
-// then the drive-map inserts.  Any failure poisons the node.
+// /enable_odom call of the RunInitialization success path (:542-560); with odometry topics, the message's rows; with a map builder, its
+// call when the message arrived INITED; then the drive-map inserts.  Any failure poisons the node.
 static int process_message(lio_node *nd, const Slot &s) {
   nd->calls.clear();
   nd->pairing.integrate(s.stamp, nd->list, &nd->calls);
   int rc = LIO_OK;
   const bool was_inited = nd->inited;
-  for (const lio::ImuCall &c : nd->calls)
+  for (const lio::ImuCall &c : nd->calls) {
     if ((rc = lio_est_process_imu(nd->est, c.dt, c.acc, c.gyr, c.stamp)) != LIO_OK) break;
+    if (nd->odometry && was_inited && (rc = record_predict_odom(nd, c.stamp)) != LIO_OK) break;
+  }
   if (rc == LIO_OK) rc = lio_est_process_compact_stamped_dev(nd->est, (const float *)s.cloud[0].get(), (const float *)s.cloud[1].get(), (const float *)s.cloud[2].get(),
                                                             s.d_n, s.n, s.sum7, s.stamp);
   int info[4] = {};
@@ -224,6 +287,7 @@ static int process_message(lio_node *nd, const Slot &s) {
     nd->odom_on = false;
   }
   nd->inited = now_inited;
+  if (nd->odometry && (rc = record_message(nd, s, was_inited, info[3] != 0)) != LIO_OK) { nd->poisoned = true; return rc; }
   if (nd->mb && was_inited && (rc = map_builder_step(nd)) != LIO_OK) { nd->poisoned = true; return rc; }
   // the estimator's PointMapping publishes /cloud_registered once per processed message (see lio_node_attach_registered_map)
   if ((rc = insert_registered(nd, LIO_NODE_MAP_ESTIMATOR)) != LIO_OK) { nd->poisoned = true; return rc; }
@@ -299,6 +363,12 @@ extern "C" int lio_node_push_sweep_dev(lio_node *nd, const float *xyzi_dev, cons
   if ((rc = lio_po_process_dev(nd->po, clouds, counts, n_max, sum7, es7, info4)) != LIO_OK) return rc;
   ++nd->po_calls;
   ++nd->sweeps;
+  if (nd->odometry && c >= 1) {   // PublishResults (:681-721), pass-through included: transform_sum_, then transform_es_ as the extras
+    double tf7[7], ex7[7];
+    widen7(sum7, tf7);
+    widen7(es7, ex7);
+    nd->topics[LIO_NODE_ODOM_LASER_ODOM_TO_INIT].push(stamp, tf7, ex7);
+  }
   if (info4[1]) {   // published (:727): copy the three clouds, transform_sum_ and the stamp into a queue slot
     const float *ptr[3];
     const int *n_dev;
@@ -404,6 +474,44 @@ extern "C" int lio_node_map_builder_poses(lio_node *nd, double *stamp, float *to
     if (aft7) std::memcpy(aft7 + 7 * r, row.aft7, sizeof(row.aft7));
     if (info6) std::memcpy(info6 + 6 * r, row.info6, sizeof(row.info6));
   }
+  return LIO_OK;
+}
+
+extern "C" int lio_node_enable_odometry(lio_node *nd, int capacity) {
+  LIO_ENTER_HOST(nd);
+  if (capacity < 1 || nd->odometry || nd->sweeps > 0 || nd->poisoned) {
+    lio_set_last_error(__FILE__, __LINE__, "lio_node_enable_odometry: capacity >= 1, once, before the first sweep, on a node that is not poisoned");
+    return LIO_ERR_INVALID;
+  }
+  try {
+    for (OdomTopic &t : nd->topics) t.rows.assign(16 * (size_t)capacity, 0.0);
+    nd->states.assign(16 * (size_t)(nd->cfg.est.window_size + 1), 0.0);
+  } catch (const std::bad_alloc &) {
+    for (OdomTopic &t : nd->topics) std::vector<double>().swap(t.rows);
+    lio_set_last_error(__FILE__, __LINE__, "lio_node_enable_odometry: the queues do not fit in host memory");
+    return LIO_ERR_CAPACITY;
+  }
+  nd->odometry = true;
+  return LIO_OK;
+}
+
+extern "C" int lio_node_take_odometry(lio_node *nd, int topic, double *rows16, int cap, int *n, int *left) {
+  LIO_ENTER_HOST(nd);
+  if (!n || cap < 0 || (cap > 0 && !rows16)) return LIO_ERR_INVALID;
+  *n = 0;
+  const char *why = nullptr;
+  if (topic < 0 || topic >= LIO_NODE_ODOM_TOPICS) why = "lio_node_take_odometry: unknown topic";
+  else if (!nd->odometry) why = "lio_node_take_odometry: no odometry topics (lio_node_enable_odometry)";
+  if (why) { lio_set_last_error(__FILE__, __LINE__, why); return LIO_ERR_INVALID; }
+  OdomTopic &t = nd->topics[topic];
+  const int k = std::min(cap, t.count), size = t.capacity();
+  for (int r = 0; r < k; ++r) {
+    std::memcpy(rows16 + 16 * (size_t)r, t.rows.data() + 16 * (size_t)t.head, 16 * sizeof(double));
+    t.head = t.head + 1 == size ? 0 : t.head + 1;
+  }
+  t.count -= k;
+  *n = k;
+  if (left) *left = t.count;
   return LIO_OK;
 }
 

@@ -330,6 +330,13 @@ class Estimator:
         _lib.check(_lib.lib().lio_est_local_laser_odom(self.h, t), "lio_est_local_laser_odom")
         return t
 
+    def laser_odom(self):
+        """(/predict_laser_odom, /local_laser_odom) as the INITED branch of ProcessLaserOdom publishes them (Estimator.cc:725-758):
+        float64 tf7 lidar poses of window slots W and W - O.  The second is local_laser_odom() before its rounding to float."""
+        predict, local = np.zeros(7), np.zeros(7)
+        _lib.check(_lib.lib().lio_est_laser_odom(self.h, predict, local), "lio_est_laser_odom")
+        return predict, local
+
     # ---- /local/* publication (lio_est_enable_local_clouds): the map builder's input
     LOCAL_CLOUDS = ("corner", "surf", "full")
 

@@ -9,7 +9,11 @@ each of them.  LioNode.shipped(name, ...) builds a node from one; the capacities
 The second line of the reference's example, launch/map_4D*.launch (map_builder_node on the estimator's /local/* clouds), runs inside the
 node after enable_map_builder() (or shipped(name, map_4d=True)): one MapBuilder::ProcessMap per message that reaches the estimator
 INITED, on the node's stream.  map_builder_poses() is the drive's 4-D trajectory; attach_registered_map() feeds a RegisteredMap (the
-save_bag_to_pcd tool) from the estimator's or the map builder's /cloud_registered."""
+save_bag_to_pcd tool) from the estimator's or the map builder's /cloud_registered.
+
+enable_odometry() (or shipped(name, odometry=True)) keeps the pose topics the two nodes publish, one row per publication, in queues the
+caller drains with take_odometry(topic): TOPICS maps the reference's topic names to the C-ABI's ids.  write_tum() writes a trajectory
+in the TUM format that trajectory-evaluation tools read."""
 from __future__ import annotations
 
 import ctypes as C
@@ -82,6 +86,24 @@ SHIPPED = {
 _EST_KEYS = ("min_plane_dis", "min_match_sq_dis", "surf_filter_size", "window_size", "opt_window_size", "init_window_factor",
              "estimate_extrinsic", "opt_extrinsic", "imu_factor", "point_distance_factor", "prior_factor", "marginalization_factor",
              "acc_n", "gyr_n", "acc_w", "gyr_w", "g_norm", "enable_deskew", "cutoff_deskew", "keep_features")
+
+
+# The odometry topics of lio_node_enable_odometry (include/lio_b200.h: LIO_NODE_ODOM_*), by the reference's topic names
+TOPICS = {"/laser_odom_to_init": 0, "/aft_mapped_to_init": 1, "/predict_odom": 2, "/predict_laser_odom": 3, "/local_laser_odom": 4,
+          "/extrinsic_lb": 5}
+# The named extras of a topic's row (columns 8..14): /laser_odom_to_init carries transform_es_ (/laser_odom_to_last), /predict_odom
+# Vs_.last() and Bas_.last()
+_EXTRAS = {"/laser_odom_to_init": (("es", 7),), "/predict_odom": (("v", 3), ("ba", 3))}
+
+
+def write_tum(path, stamp, tf7):
+    """One pose per line, "stamp tx ty tz qx qy qz qw" (the TUM trajectory format): stamp (n,), tf7 (n, 7) in the repository's order
+    qx qy qz qw px py pz (take_odometry(topic)["tf7"])."""
+    t = np.asarray(stamp, np.float64).reshape(-1)
+    p = np.asarray(tf7, np.float64).reshape(-1, 7)
+    if p.shape[0] != t.shape[0]:
+        raise ValueError("one tf7 row per stamp")
+    np.savetxt(path, np.column_stack([t, p[:, 4:7], p[:, 0:4]]), fmt="%.9f")
 
 
 def shipped_tf_lb7(name):
@@ -167,9 +189,10 @@ class LioNode:
         self._maps = []   # attached RegisteredMaps: the node inserts into them, so it keeps them alive
 
     @classmethod
-    def shipped(cls, name, map_4d=False, **overrides):
+    def shipped(cls, name, map_4d=False, odometry=False, **overrides):
         """A node with the values of SHIPPED[name]; keyword arguments (capacities, tf_lb7, any config field) take precedence.  map_4d=True
-        also runs map_4D*.launch's map builder with its defaults (enable_map_builder())."""
+        also runs map_4D*.launch's map builder with its defaults (enable_map_builder()); odometry=True keeps the odometry topics
+        (enable_odometry() with its default capacity)."""
         s = SHIPPED[name]
         kw = dict(sensor_type=s["sensor_type"], odom_io=s["odom_io"], msg_time_delay=s["msg_time_delay"], tf_lb7=shipped_tf_lb7(name),
                   corner_filter_size=s["corner_filter_size"], surf_filter_size=s["surf_filter_size"], map_filter_size=s["map_filter_size"])
@@ -178,6 +201,8 @@ class LioNode:
         node = cls(**kw)
         if map_4d:
             node.enable_map_builder()
+        if odometry:
+            node.enable_odometry()
         return node
 
     def enable_map_builder(self, **cfg):
@@ -212,6 +237,35 @@ class LioNode:
         out = dict(stamp=stamp[:k], tobe=tobe[:k], aft=aft[:k])
         for j, name in enumerate(("iterations", "optimised", "corner_from_map", "surf_from_map", "surround_published", "surround_size")):
             out[name] = info[:k, j].astype(bool) if name in ("optimised", "surround_published") else info[:k, j].copy()
+        return out
+
+    def enable_odometry(self, capacity=1 << 16):
+        """Keep every publication of the TOPICS (lio_node_enable_odometry): one queue of capacity rows per topic, the oldest row dropped
+        when a queue is full.  Once, before the first sweep."""
+        _lib.check(_lib.lib().lio_node_enable_odometry(self.h, int(capacity)), "lio_node_enable_odometry")
+
+    def take_odometry(self, topic, cap=None):
+        """Removes and returns the oldest queued rows of topic (a name of TOPICS or its id), all of them unless cap is given: dict of
+        stamp (n,), tf7 (n, 7) {qx qy qz qw px py pz}, the topic's extras (/laser_odom_to_init: es (n, 7); /predict_odom: v and ba
+        (n, 3)), seq (n,) int64 (the publication count from 1: a gap is a dropped row) and left, the rows still queued.  float64."""
+        name = topic if isinstance(topic, str) else next((k for k, v in TOPICS.items() if v == topic), None)
+        tid = TOPICS.get(name, -1) if isinstance(topic, str) else int(topic)
+        L = _lib.lib()
+        n, left = C.c_int(), C.c_int()
+        if cap is None:   # how many are queued: a take of none
+            _lib.check(L.lio_node_take_odometry(self.h, tid, None, 0, C.byref(n), C.byref(left)), "lio_node_take_odometry")
+            cap = left.value
+        rows = np.zeros((max(int(cap), 1), 16))
+        _lib.check(L.lio_node_take_odometry(self.h, tid, rows.ctypes.data_as(C.c_void_p), int(cap), C.byref(n), C.byref(left)),
+                   "lio_node_take_odometry")
+        rows = rows[:n.value]
+        out = dict(stamp=rows[:, 0].copy(), tf7=rows[:, 1:8].copy())
+        col = 8
+        for key, width in _EXTRAS.get(name, ()):
+            out[key] = rows[:, col:col + width].copy()
+            col += width
+        out["seq"] = rows[:, 15].astype(np.int64)
+        out["left"] = left.value
         return out
 
     def attach_registered_map(self, rm, source="estimator"):
