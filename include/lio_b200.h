@@ -91,8 +91,8 @@ int lio_pp_process_dev(lio_pp *pp, const float *xyzi_dev, int n);
 /* The overload for sensors that deliver the ring index (lio::PointXYZIR, include/point_processor/point_types.h:37-52):
  * PointToRing(PointCloud<PointIR>) PointProcessor.cc:428-536 — ring id from `rings` (n x uint16), rel_time scaled by the
  * observed azimuth range end_ori_ - start_ori_ — followed by the shared ExtractFeaturePoints.  Synchronous.
- * Round-1 status: restated in the oracle and pinned by a CPU test; the device path was written after the round's GPU
- * budget was spent and is exercised by a non-strict xfail test until it has run on hardware. */
+ * Checked against the oracle (tests/test_zz_ring_field_gpu.py) and against a plain numpy statement of PointProcessor at
+ * its edges (tests/test_stage_a_edges_gpu.py) on the device. */
 int lio_pp_process_host_ring(lio_pp *pp, const float *xyzi, const uint16_t *rings, int n);
 /* The same with xyzi (n x float4) and rings (n x uint16) already on the device, e.g. a sensor driver's DMA target: the kernels of
  * lio_pp_process_host_ring without its uploads (which is "upload, then this entry").  Stream rule and count accessors as for

@@ -5,9 +5,16 @@
 // Bit-exactness contract (SURVEY.md App. C): this translation unit is compiled with -fmad=false,
 // IEEE sqrt/div, and every float expression is written in the reference's source order, so the
 // ring-ordered cloud, the occlusion mask, the curvature sort and the sharp / less-sharp / flat /
-// less-flat index sets are identical to the CPU path.  atan2f is evaluated as a correctly rounded
-// double atan2 (rel_time / intensity are tolerance-checked, ring ids are exact away from bucket
-// edges).
+// less-flat index sets are identical to the CPU path.
+//
+// Angle contract: the elevation and the azimuth are float(atan2 in double), i.e. atan2f correctly
+// rounded up to the device's double atan2 error.  The reference calls atan2f, which glibc does not
+// promise to round correctly, so a point can differ from the reference only where that rounding
+// matters: its double angle lies within a few double ulps of a float rounding midpoint, or its
+// ring id changes when the elevation moves one float ulp (a point on a bucket edge).  Such a point
+// may land in the neighbouring ring, and its ring + rel_time / int(I) + rel_time may differ by one
+// float ulp of the azimuth; every other point's ring, order, xyz and intensities are bit-exact
+// (tests/pp_ref.py states the contract and its `ambiguous` points).
 //
 // Pipeline (one stream, 5 launches):
 //   a_classify : per point ring id + azimuth, per-block ring histogram, first accepted point
@@ -699,9 +706,11 @@ extern "C" void lio_pp_default_config(lio_pp_config *c) {
 
 extern "C" int lio_pp_create(const lio_pp_config *cfg, int max_points, int device, void *cuda_stream, lio_pp **out) {
   if (!cfg || !out || max_points <= 0) return LIO_ERR_INVALID;
+  // a negative pick budget would make a_compact's min(n_less, max_sharp) offsets, and so the sharp count, negative
   if (cfg->num_rings < 1 || cfg->num_rings > kMaxRings || cfg->num_scan_subregions < 1 || cfg->num_scan_subregions > kMaxSub ||
       cfg->num_curvature_regions < 1 || cfg->num_curvature_regions > 16 || cfg->max_corner_less_sharp > kMaxLessSharp ||
-      cfg->max_surf_flat > kMaxFlat || cfg->max_corner_sharp > cfg->max_corner_less_sharp || !(cfg->less_flat_filter_size > 0) ||
+      cfg->max_surf_flat > kMaxFlat || cfg->max_corner_sharp > cfg->max_corner_less_sharp || cfg->max_corner_sharp < 0 ||
+      cfg->max_corner_less_sharp < 0 || cfg->max_surf_flat < 0 || !(cfg->less_flat_filter_size > 0) ||
       !(cfg->upper_bound > cfg->lower_bound)) {
     lio_set_last_error(__FILE__, __LINE__, "lio_pp_create: configuration outside supported limits");
     return LIO_ERR_INVALID;
